@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- images/sec of the full ColorHandPose3DNetwork.inference pipeline on synthetic 320x320 batches.
 
-  python bench.py --gpus N --steps K --warmup W            # our sm_100a path (one rank per GPU under torchrun)
+  python bench.py --gpus N --steps K --warmup W            # our sm_90a path (one rank per GPU under torchrun)
   python bench.py --impl reference --gpus N --steps K ...   # the CPU restatement of the TF1 reference (oracle)
 
 One JSON line on stdout (rank 0).  A "step" is one pass of the full pipeline (HandSegNet -> mask/crop ->
@@ -63,20 +63,20 @@ def stage_gflop_per_image(stage, H, W):
     return (seg + pose + net(arch.POSEPRIOR, 32, 32) + net(arch.VIEWPOINT, 32, 32)) / 1e9
 
 
-def measured_traffic(precision="bf16x3"):
-    """DRAM bytes per launch of the dominant kernel from the committed ncu capture (profiles/*_summary.json), or None."""
-    best = None
-    pdir = os.path.join(ROOT, "profiles")
-    if os.path.isdir(pdir):
-        for fn in sorted(os.listdir(pdir)):
-            if fn.endswith("_summary.json") and (("f8c" in fn) == (precision == "fp16_f8c")):
-                try:
-                    d = json.load(open(os.path.join(pdir, fn)))
-                    if "tc_conv" in d:
-                        best = (fn, d["tc_conv"])
-                except Exception:
-                    pass
-    return best
+def dump_outputs(res, out_dir, limit_bytes=64 << 20):
+    """Writes the tensors one pipeline step returned as out_dir/<name>.npy: floating point as float32, integers as float64 (exact).
+    An array larger than its share of limit_bytes is replaced by a fixed-seed sample of its flattened elements (sorted indices)."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: v for k, v in res.items() if torch.is_tensor(v)}
+    share = limit_bytes // max(1, len(arrays))
+    for name, t in sorted(arrays.items()):
+        a = t.detach().cpu().numpy()
+        a = a.astype(np.float32) if a.dtype.kind == "f" else a.astype(np.float64)
+        if a.nbytes > share:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, share // a.itemsize, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def measured_peaks():
@@ -88,7 +88,8 @@ def measured_peaks():
                     "hbm_gbs": float(d["hbm_gbs"]), "source": "measured (MEASURED_PEAKS.json)"}
         except Exception:
             pass
-    return {"tflops_burst": 1590.0, "tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (700 W card): dense BF16 and HBM3 bandwidth; a card set to a lower power limit reaches less
+    return {"tflops_burst": 989.0, "tflops_sustained": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet, not measured"}
 
 
 class ClockSampler(threading.Thread):
@@ -304,6 +305,7 @@ def run_ours(args):
             replay, res = ctx.capture_pipeline(dev_imgs[k], dev_hs[k] if full else None, full, outputs="keypoints")
             graphs.append((replay, res, (ctx.launch_count - c0) // 2))   # warm-up + capture each issue the step once
     graph_launches = [0]
+    last = [None]   # the result tensors of the latest step (--dump-outputs)
 
     def step_device(i):
         if graphs is not None:
@@ -312,6 +314,7 @@ def run_ours(args):
             graph_launches[0] += nl
         else:
             r = run_stage(dev_imgs[i % NBUF], dev_hs[i % NBUF])
+        last[0] = r
         return exchange(r)
 
     def barrier():
@@ -360,6 +363,8 @@ def run_ours(args):
     sampler.stop_flag = True
     sampler.join(timeout=2.0)
     value = world * B * args.steps / (ms / 1000.0)
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(last[0], args.dump_outputs)
 
     # ---- sustained: the same loop for several seconds (power / thermal steady state), reported beside the K-step value
     sustained = None
@@ -487,15 +492,12 @@ def run_ours(args):
     d = prof[dominant]
     if d["ms"] > 0:
         achieved = d["flops"] / (d["ms"] * 1e-3) / 1e12
-        peak = peaks["tflops_sustained"] if dominant == "tc_conv" else 75.0
-        tr = measured_traffic(args.precision) if (dominant == "tc_conv" and args.precision in ("bf16x3", "fp16_f8c") and full and B == 32) else None
+        peak = peaks["tflops_sustained"] if dominant == "tc_conv" else 67.0
         passes = 3 if args.precision in ("bf16x3", "fp16x3") else (2 if args.precision == "fp16_f8c" else 1)
-        roof = {"bound": "tensor", "kernel": "conv_tc2_kernel / conv_tc_kernel / conv_c64x2_kernel / conv_c64_kernel / conv_c1f_kernel (tcgen05 implicit GEMM: every conv layer - conv1_1 fused into conv1_2 - and the FC stacks)" if dominant == "tc_conv" else "conv_direct_kernel (fp32 FFMA)",
+        roof = {"bound": "tensor", "kernel": "conv_tc_kernel / conv_c3_tc_kernel / fc_chain_kernel (wgmma implicit GEMM: every conv layer and the FC stacks)" if dominant == "tc_conv" else "conv_direct_kernel (fp32 FFMA)",
                 "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                "traffic": tr[1]["dram_bytes_per_launch"] if tr else None,
-                "traffic_source": ("ncu dram__bytes_read+write per launch, B=32, profiles/%s" % tr[0]) if tr else None,
                 "achieved_per_launch": {"gflop": d["flops"] / max(1, d["launches"]) / 1e9, "us": 1e3 * d["ms"] / max(1, d["launches"])},
-                "peak_source": peaks["source"] + (", bf16 sustained" if dominant == "tc_conv" else ", nominal fp32 FFMA"),
+                "peak_source": peaks["source"] + (", dense bf16" if dominant == "tc_conv" else ", fp32 FFMA"),
                 "launches_per_step": d["launches"] // prof_steps, "ms_per_step": d["ms"] / prof_steps,
                 "mma_passes": passes,
                 # fp32 parity costs `passes` tensor-core passes per algorithmic FLOP: the executed rate is what the tensor pipe sees
@@ -560,9 +562,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--gather", default=os.environ.get("H3D_GATHER", "p2p"), choices=["p2p", "nccl"], help="multi-GPU result exchange")
     ap.add_argument("--cuda-graph", type=int, default=None, help="replay the step from a CUDA graph")
-    ap.add_argument("--sustain-seconds", type=float, default=3.0, help="extra sustained loop after the timed K steps (0 = off)")
+    ap.add_argument("--sustain-seconds", type=float, default=0.0, help="extra sustained loop after the timed K steps (0 = off)")
     ap.add_argument("--e2e-input", default="records", choices=["records", "f32"], help="what the end-to-end loop copies host -> device")
     ap.add_argument("--e2e-all-outputs", type=int, default=1, help="also time the end-to-end loop with every reference output read back")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the tensors the last timed step returned as DIR/<name>.npy (at most 64 MB)")
     args = ap.parse_args()
     cfg = CONFIGS[args.config]
     for k in ("batch", "stage", "height", "width", "precision", "cuda_graph"):

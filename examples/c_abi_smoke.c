@@ -4,7 +4,7 @@
  *       -Wl,-rpath,$PWD/hand3d_b200
  *
  * Runs bone_rel_trafo_inv, the TF1-legacy bilinear resize, the mask post-processing and a small fp32 convolution with
- * known answers; exits 0 on success.  Without an sm_100a device h3d_create() must fail with H3D_ENODEVICE (exit code 77).
+ * known answers; exits 0 on success.  Without an sm_90a device h3d_create() must fail with H3D_ENODEVICE (exit code 77).
  */
 #include <cuda_runtime_api.h>
 #include <math.h>
@@ -28,7 +28,7 @@
 int main(void) {
     h3d_ctx* ctx = NULL;
     int rc = h3d_create(&ctx, 0);
-    if (rc == H3D_ENODEVICE) { printf("no sm_100a device: %s\n", h3d_last_error()); return 77; }
+    if (rc == H3D_ENODEVICE) { printf("no sm_90a device: %s\n", h3d_last_error()); return 77; }
     if (rc != H3D_OK) { fprintf(stderr, "h3d_create: %s\n", h3d_last_error()); return 1; }
     printf("hand3d_b200 C ABI version %d\n", h3d_version());
 

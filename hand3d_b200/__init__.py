@@ -1,4 +1,4 @@
-"""hand3d_b200 -- B200-native (sm_100a) forward pass of ColorHandPose3D behind the reference's Python API.
+"""hand3d_b200 -- H100-native (sm_90a) forward pass of ColorHandPose3D behind the reference's Python API.
 
     from hand3d_b200.nets.ColorHandPose3DNetwork import ColorHandPose3DNetwork
     from hand3d_b200.utils.general import detect_keypoints, trafo_coords

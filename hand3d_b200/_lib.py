@@ -1,7 +1,7 @@
 """ctypes binding of libhand3d_b200.so (include/hand3d_b200.h).
 
 There is deliberately no fallback: if the shared library is missing and cannot be built, or a compute
-entry point fails (e.g. no sm_100a device), a RuntimeError is raised with h3d_last_error().
+entry point fails (e.g. no sm_90a device), a RuntimeError is raised with h3d_last_error().
 """
 from __future__ import annotations
 

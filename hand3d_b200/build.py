@@ -1,4 +1,4 @@
-"""Builds libhand3d_b200.so (hand-written sm_100a CUDA + the C ABI) in-tree with nvcc.
+"""Builds libhand3d_b200.so (hand-written sm_90a CUDA + the C ABI) in-tree with nvcc.
 
 The shared library links the CUDA runtime statically and resolves the driver's
 cuTensorMapEncodeTiled at run time, so it loads (and exports every symbol of include/hand3d_b200.h)
@@ -16,9 +16,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libhand3d_b200.so")
 STAMP = os.path.join(HERE, ".libhand3d_b200.stamp")
-SOURCES = ["api.cu", "elementwise.cu", "reader.cu", "conv_direct.cu", "conv_tc.cu"]
+SOURCES = ["api.cu", "elementwise.cu", "reader.cu", "conv_direct.cu", "conv_wgmma.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--cudart=static", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",
     "-Xptxas", "-v",
 ]
@@ -63,7 +63,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(out)
             raise RuntimeError("nvcc failed on %s" % src)
     tmp = LIB + ".tmp"       # link next to the target and rename: a reader (or a repo snapshot) never sees a half-written library
-    cmd = [_nvcc(), "-shared", "--cudart=static", "-gencode", "arch=compute_100a,code=sm_100a", "-o", tmp, *objs]
+    cmd = [_nvcc(), "-shared", "--cudart=static", "-gencode", "arch=compute_90a,code=sm_90a", "-o", tmp, *objs]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout)

@@ -121,8 +121,9 @@ struct StagePlan {
     int cur_lane = 0;                   // lane given to steps as they are appended (see seal())
     int B = 0, H = 0, W = 0, variant = -1;
     int64_t flops = 0;
-    // layer chains (conv_tc.cu "Layer chains"): per chained launch one ticket word + B per-image completion counters, zeroed by the
-    // plan's first step; chain_prev = the chained launch appended last, iff it is the plan's most recent step
+    // layer chains (per chained launch one ticket word + B per-image completion counters, zeroed by the plan's first step;
+    // chain_prev = the chained launch appended last, iff it is the plan's most recent step): only for plans that
+    // tc_conv_plan_chainable() accepts, none in the sm_90a build
     int* sync = nullptr;
     int sync_slots = 0;
     TcConvPlan* chain_prev = nullptr;
@@ -506,7 +507,8 @@ static int build_trunk(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, co
         const int c_off = last_layer ? final_c_off : 0;
         const bool pool_after = !strcmp(l.name, "conv1_2") || !strcmp(l.name, "conv2_2") || !strcmp(l.name, "conv3_4");
         const bool fuse_pool = use_tc && pool_after && (h % 2 == 0) && (w % 2 == 0) && !tc_tuning().no_pool_fusion;
-        // conv1_1 + conv1_2 as one launch (conv_c1f_kernel): layer 0 is skipped here and handed to layer 1
+        // conv1_1 + conv1_2 as one launch where tc_conv_can_fuse_first() allows it (never in the sm_90a build): layer 0 is skipped
+        // here and handed to layer 1
         if (tc && i == 0 && n > 1 && l.cin == 3 && l.cout == 64 && l.k == 3 && l.stride == 1 &&
             !strcmp(layers[1].name, "conv1_2") && (h % 2 == 0) && (w % 2 == 0) && !tc_tuning().no_pool_fusion &&
             tc_conv_can_fuse_first(h, w, layers[1].cin, layers[1].cout, layers[1].k, lo, 1)) {
@@ -685,7 +687,7 @@ static int add_fc(h3d_ctx* ctx, StagePlan* pl, const std::string& name, const fl
 }
 
 // PosePrior (+ ViewpointNet for the 'proposed' variant): two 6-layer stride-1 / stride-2 conv pyramids on the 32x32 score map
-// and their FC stacks.  With a 3-pass tensor-core precision the pyramids run on the tcgen05 kernel (stride 2 = odd pixels of
+// and their FC stacks.  With a 3-pass tensor-core precision the pyramids run on the wgmma kernel (stride 2 = odd pixels of
 // the stride-1 result, Cin / Cout padded to 64 with zero channels); otherwise on the fp32 CUDA-core kernel.  The two networks
 // are independent until the final rotation, so ViewpointNet is put on the context's side stream.
 static int build_lifting(h3d_ctx* ctx, int B, int variant) {
@@ -1003,7 +1005,7 @@ int h3d_device_available(void) {
     if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) { cudaGetLastError(); return 0; }
     cudaDeviceProp p;
     if (cudaGetDeviceProperties(&p, 0) != cudaSuccess) { cudaGetLastError(); return 0; }
-    return p.major == 10 ? 1 : 0;
+    return p.major == 9 && p.minor == 0 ? 1 : 0;
 }
 
 int h3d_create(h3d_ctx** out, int device) {
@@ -1012,8 +1014,8 @@ int h3d_create(h3d_ctx** out, int device) {
     if (rc) return rc;
     cudaDeviceProp p;
     H3D_CUDA(cudaGetDeviceProperties(&p, device));
-    if (p.major != 10) {
-        set_error("device %d (%s) has compute capability %d.%d; hand3d_b200 is built for sm_100a only", device, p.name, p.major, p.minor);
+    if (p.major != 9 || p.minor != 0) {
+        set_error("device %d (%s) has compute capability %d.%d; hand3d_b200 is built for sm_90a only", device, p.name, p.major, p.minor);
         return H3D_ENODEVICE;
     }
     H3D_CUDA(cudaSetDevice(device));
@@ -1051,10 +1053,10 @@ int h3d_check_errors(h3d_ctx* ctx, int* code) {
     const int c = ctx->err_flag ? *(volatile int*)ctx->err_flag : 0;
     if (code) *code = c;
     if (c == 0) return H3D_OK;
-    static const char* what[] = {"", "TMA producer waiting for a free shared-memory stage", "MMA issuer waiting for a drained TMEM accumulator",
-                                 "MMA issuer waiting for a TMA stage", "epilogue waiting for a finished accumulator", "MMA issuer waiting for the resident weights"};
+    static const char* what[] = {"", "TMA producer waiting for a free shared-memory stage", "unused wait code",
+                                 "wgmma warpgroup waiting for a TMA stage", "unused wait code", "unused wait code"};
     if (c >= 100) set_error("device-side timeout: gather_records_p2p never saw the records of peer rank %d (code %d)", c - 100, c);
-    else set_error("device-side timeout in a tcgen05 convolution kernel: %s (code %d); the kernel trapped", c >= 1 && c <= 5 ? what[c] : "unknown wait", c);
+    else set_error("device-side timeout in a tensor-core convolution kernel: %s (code %d); the kernel trapped", c >= 1 && c <= 5 ? what[c] : "unknown wait", c);
     return H3D_ECUDA;
 }
 

@@ -1,4 +1,4 @@
-// Shared declarations for the hand3d_b200 CUDA sources (sm_100a only).
+// Shared declarations for the hand3d_b200 CUDA sources (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -160,7 +160,7 @@ int launch_concat_handside(const float* feat, const float* hand_side, float* out
 // same as 16-bit split planes [B, Kpad] (Kpad % 64 == 0, zero padded): input of the tensor-core FC stack
 int launch_concat_handside_split(const float* feat, const float* hand_side, Split out, int B, int feat_n, int Kpad, Half16 t, cudaStream_t s);
 
-// ---------------------------------------------------------------- kernels (conv_tc.cu)
+// ---------------------------------------------------------------- kernels (conv_wgmma.cu)
 // first layer (Cin = 3, 3x3, 64 output channels) on the tensor cores, writing split planes (hi, lo optional)
 int launch_conv_c3_tc(const float* x, const float* w, const float* bias, Split y, int Cs_total, int cs_off, int B, int H, int W, int leaky,
                       Half16 half, cudaStream_t s, int* err_flag = nullptr);
@@ -184,30 +184,32 @@ struct TcConvDesc {
     Half16 half;
     int pool = 0;  // 1: fuse the following 2x2/2 max-pool; 2: stride-2 'SAME' convolution (even H, W); outputs are [B, H/2, W/2, C]
     int* err_flag = nullptr;   // device int: a barrier wait that times out stores its code here before trapping (h3d_ctx owns it)
-    // conv1_1 fused into this layer (conv1_2: 64 -> 64, 3x3, pooled, 3-pass): the first layer's device fp32 weights HWIO [3,3,3,64] and
-    // bias [64]; x is then unused and the fp32 image [B,H,W,3] is passed at launch (tc_conv_launch_image)
+    // conv1_1 fused into this layer: tc_conv_plan_create rejects it in the sm_90a build (tc_conv_can_fuse_first is false)
     const float* c1_w = nullptr; const float* c1_bias = nullptr; int c1_leaky = 0;
 };
-// Tuning switches: initialised from the environment once (H3D_TC_2CTA, H3D_TC_BN, ...), changed only through tc_set_tuning().
+// Tuning switches: initialised from the environment once (H3D_TC_BN, H3D_FC_CHAIN, ...), changed only through tc_set_tuning().
 struct TcTuning {
-    int two_cta = -1;      // -1 policy, 0 / 1 force the single-CTA / CTA-pair kernel family
-    int bn = 0;            // 0 policy, else forced N tile
+    // two_cta, c64, c64x2, pair128, stack, exp, c3_tma, c64_tma_out, chain, small_batch_split and fuse_c1 chose between kernel
+    // variants of an earlier build; the sm_90a build has one convolution kernel family and accepts them without effect.
+    int two_cta = -1;
+    int bn = 0;            // 0 policy, else forced N tile (64 or 128)
     int c64 = 1, c64x2 = 1, pair128 = 1, stack = 1;
-    int chunk_kb = 0;      // 0 policy
-    int exp = 0;           // timing experiments (wrong results allowed), see TcParams::exp
-    int no_side_stream = 0, no_pool_fusion = 0, lift_direct = 0, c3_ffma = 0;
+    int chunk_kb = 0;      // 0 policy, else K blocks per tensor-core partial sum
+    int exp = 0;
+    int no_side_stream = 0, no_pool_fusion = 0, lift_direct = 0;
+    int c3_ffma = 0;       // 1: first layer on the register-tiled FFMA kernel instead of the tensor cores
     int no_seg_fusion = 0; // 1: HandSegNet's x8 up-sampling as its own launch (instead of fused into the mask post-processing)
-    int c64_tma_out = 1;   // 64-channel pair kernel: bulk-tensor-store epilogue for un-pooled layers (conv2_1)
+    int c64_tma_out = 1;
     int fc_chain = 1;      // FC stacks + rotation epilogue of the lifting stage as one kernel (0 = one launch per layer)
-    int fuse_c1 = 1;       // conv1_1 computed inside conv1_2's kernel (conv_c1f_kernel, DESIGN 4.10); 0 = conv_c3_tma_kernel + conv_c64x2_kernel
-    int small_batch_split = 1;   // few pixel tiles: narrow single-CTA tiles instead of CTA-pair items (same arithmetic, shorter critical path)
-    int chain = 1;         // layer chains: dynamic tile tickets + per-image dependencies between consecutive CTA-pair conv launches (2 = tickets only)
+    int fuse_c1 = 1;
+    int small_batch_split = 1;
+    int chain = 1;
     int pdl = 1;           // programmatic dependent launch between the tensor-core kernels (prologue overlaps the previous kernel's tail)
-    int c3_tma = 1;        // first layer: shared-memory staged epilogue + bulk tensor stores (0 = direct 16-byte global stores)
+    int c3_tma = 1;
 };
 TcTuning& tc_tuning();
 int tc_set_tuning(const char* key, int value);
-// FC stack of a lifting network as ONE kernel (conv_tc.cu: fc_chain_kernel): up to 4 fully connected layers per chain, the
+// FC stack of a lifting network as ONE kernel (conv_wgmma.cu: fc_chain_kernel): up to 4 fully connected layers per chain, the
 // activations of every layer as split planes [B, width_pad] (row stride = width rounded up to 64), the last layer fp32.
 struct FcLayerDesc {
     Split x; int x_stride, in_features;      // input planes [B, x_stride], K = in_features rounded up to 64
@@ -231,7 +233,7 @@ int tc_conv_plan_signal_target(const TcConvPlan* p);
 const TcConvDesc& tc_conv_plan_desc(const TcConvPlan* p);
 void tc_conv_plan_set_chain(TcConvPlan* p, int* sched, const int* dep_cnt, int dep_target, int* sig_cnt);
 int tc_conv_launch(const TcConvPlan* p, cudaStream_t s);
-int tc_conv_launch_image(const TcConvPlan* p, const float* image, cudaStream_t s);   // plans created with TcConvDesc::c1_w
+int tc_conv_launch_image(const TcConvPlan* p, const float* image, cudaStream_t s);   // plans with TcConvDesc::c1_w (none on sm_90a)
 bool tc_conv_can_fuse_first(int H, int W, int Cin, int Cout, int k, int passes, int pool);
 int64_t tc_conv_flops(const TcConvPlan* p);
 int tc_num_sms();

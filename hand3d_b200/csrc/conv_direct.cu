@@ -328,7 +328,7 @@ static void plan_direct(const DirectConvArgs& a, ConvGeom* gp, dim3* gridp, int*
     int ksplit = 1;
     const int ctas = (int)(grid.x * grid.y);
     if (a.splitk_scratch && a.y && !a.ys.hi && ctas < 296 && Ktot >= 256) {
-        // tiny spatial maps (the stride-2 lifting pyramids): too few tiles to fill 148 SMs -> split the reduction
+        // tiny spatial maps (the stride-2 lifting pyramids): too few tiles to fill 132 SMs -> split the reduction
         ksplit = std::min(ceil_div(Ktot, 128), std::max(1, 592 / ctas));
         if (ksplit > 1 && (int64_t)ksplit * M * a.Cout <= a.splitk_scratch_floats) {
             g.k_per_split = (int)align_up(ceil_div(Ktot, ksplit), KC);

@@ -75,7 +75,7 @@ int launch_resize_bilinear_tf1(const float* x, float* y, int B, int H, int W, in
     const float hscale = (float)H / (float)oh, wscale = (float)W / (float)ow;
     const int64_t total = (int64_t)B * oh * ((ow * C + 3) / 4);
     const int threads = 256;
-    const int blocks = (int)std::min<int64_t>(ceil_div64(total, threads), 148 * 32);
+    const int blocks = (int)std::min<int64_t>(ceil_div64(total, threads), 132 * 32);
     if (C == 21) resize_bilinear_tf1_kernel<21><<<blocks, threads, 0, s>>>(x, y, B, H, W, C, oh, ow, hscale, wscale);
     else if (C == 2) resize_bilinear_tf1_kernel<2><<<blocks, threads, 0, s>>>(x, y, B, H, W, C, oh, ow, hscale, wscale);
     else resize_bilinear_tf1_kernel<0><<<blocks, threads, 0, s>>>(x, y, B, H, W, C, oh, ow, hscale, wscale);
@@ -123,10 +123,10 @@ int launch_maxpool_f32(const float* x, float* y, int B, int H, int W, int C, cud
     const int threads = 256;
     if ((C & 3) == 0) {
         const int64_t total = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
-        maxpool_f32_kernel<<<(int)std::min<int64_t>(ceil_div64(total, threads), 148 * 32), threads, 0, s>>>(x, y, B, H, W, C);
+        maxpool_f32_kernel<<<(int)std::min<int64_t>(ceil_div64(total, threads), 132 * 32), threads, 0, s>>>(x, y, B, H, W, C);
     } else {
         const int64_t total = (int64_t)B * (H / 2) * (W / 2) * C;
-        maxpool_f32_scalar_kernel<<<(int)std::min<int64_t>(ceil_div64(total, threads), 148 * 32), threads, 0, s>>>(x, y, B, H, W, C);
+        maxpool_f32_scalar_kernel<<<(int)std::min<int64_t>(ceil_div64(total, threads), 132 * 32), threads, 0, s>>>(x, y, B, H, W, C);
     }
     H3D_CHECK_LAUNCH();
     return H3D_OK;
@@ -182,7 +182,7 @@ int launch_maxpool_split(Split x, Split y, int B, int H, int W, int C, Half16 t,
     H3D_REQUIRE((C & 7) == 0, "maxpool_split: C %% 8 != 0");
     const int threads = 256;
     const int64_t total = (int64_t)B * (H / 2) * (W / 2) * (C / 8);
-    const int blocks = (int)std::min<int64_t>(ceil_div64(total, threads), 148 * 32);
+    const int blocks = (int)std::min<int64_t>(ceil_div64(total, threads), 132 * 32);
     const uint4 *xh = (const uint4*)x.hi, *xl = (const uint4*)x.lo;
     uint4 *yh = (uint4*)y.hi, *yl = (uint4*)y.lo;
     const bool lo = x.lo != nullptr;
@@ -219,7 +219,7 @@ __global__ void avgpool8_kernel(const float* __restrict__ x, float* __restrict__
 int launch_avgpool8(const float* x, float* y, int B, int H, int W, int C, cudaStream_t s) {
     H3D_REQUIRE(H % 8 == 0 && W % 8 == 0, "avgpool8: H, W must be multiples of 8");
     const int64_t total = (int64_t)B * (H / 8) * (W / 8) * C;
-    avgpool8_kernel<<<(int)std::min<int64_t>(ceil_div64(total, 256), 148 * 32), 256, 0, s>>>(x, y, B, H, W, C);
+    avgpool8_kernel<<<(int)std::min<int64_t>(ceil_div64(total, 256), 132 * 32), 256, 0, s>>>(x, y, B, H, W, C);
     H3D_CHECK_LAUNCH();
     return H3D_OK;
 }
@@ -272,11 +272,11 @@ __global__ void f8c_to_f32_kernel(const uint16_t* __restrict__ h16, const uint8_
 
 int launch_f32_to_split(const float* x, Split y, int64_t rows, int C, int Cpad, Half16 t, cudaStream_t s) {
     if (y.l8) {
-        f32_to_f8c_kernel<<<(int)std::min<int64_t>(ceil_div64(rows * Cpad, 256), 148 * 32), 256, 0, s>>>(x, y.hi, y.l8, y.h8, rows, C, Cpad);
+        f32_to_f8c_kernel<<<(int)std::min<int64_t>(ceil_div64(rows * Cpad, 256), 132 * 32), 256, 0, s>>>(x, y.hi, y.l8, y.h8, rows, C, Cpad);
         H3D_CHECK_LAUNCH();
         return H3D_OK;
     }
-    const int blocks = (int)std::min<int64_t>(ceil_div64(rows * Cpad, 256), 148 * 32);
+    const int blocks = (int)std::min<int64_t>(ceil_div64(rows * Cpad, 256), 132 * 32);
     if (t == Half16::FP16) f32_to_split_kernel<true><<<blocks, 256, 0, s>>>(x, y.hi, y.lo, rows, C, Cpad);
     else f32_to_split_kernel<false><<<blocks, 256, 0, s>>>(x, y.hi, y.lo, rows, C, Cpad);
     H3D_CHECK_LAUNCH();
@@ -284,11 +284,11 @@ int launch_f32_to_split(const float* x, Split y, int64_t rows, int C, int Cpad, 
 }
 int launch_split_to_f32(Split x, float* y, int64_t rows, int C, int Cpad, Half16 t, cudaStream_t s) {
     if (x.l8) {
-        f8c_to_f32_kernel<<<(int)std::min<int64_t>(ceil_div64(rows * C, 256), 148 * 32), 256, 0, s>>>(x.hi, x.l8, y, rows, C, Cpad);
+        f8c_to_f32_kernel<<<(int)std::min<int64_t>(ceil_div64(rows * C, 256), 132 * 32), 256, 0, s>>>(x.hi, x.l8, y, rows, C, Cpad);
         H3D_CHECK_LAUNCH();
         return H3D_OK;
     }
-    const int blocks = (int)std::min<int64_t>(ceil_div64(rows * C, 256), 148 * 32);
+    const int blocks = (int)std::min<int64_t>(ceil_div64(rows * C, 256), 132 * 32);
     if (t == Half16::FP16) split_to_f32_kernel<true><<<blocks, 256, 0, s>>>(x.hi, x.lo, y, rows, C, Cpad);
     else split_to_f32_kernel<false><<<blocks, 256, 0, s>>>(x.hi, x.lo, y, rows, C, Cpad);
     H3D_CHECK_LAUNCH();
@@ -303,7 +303,7 @@ __global__ void copy_channels_kernel(const float* __restrict__ src, float* __res
     }
 }
 int launch_copy_channels(const float* src, float* dst, int64_t rows, int C, int dst_total, int dst_off, cudaStream_t s) {
-    copy_channels_kernel<<<(int)std::min<int64_t>(ceil_div64(rows * C, 256), 148 * 8), 256, 0, s>>>(src, dst, rows, C, dst_total, dst_off);
+    copy_channels_kernel<<<(int)std::min<int64_t>(ceil_div64(rows * C, 256), 132 * 8), 256, 0, s>>>(src, dst, rows, C, dst_total, dst_off);
     H3D_CHECK_LAUNCH();
     return H3D_OK;
 }
@@ -562,8 +562,8 @@ int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scrat
     uint32_t* det = (uint32_t*)((char*)scratch + align_up((int64_t)B * 8, 256));
     H3D_CUDA(cudaMemsetAsync(key, 0, (size_t)B * 8, s));
     const int words = H * Ww;
-    // about one resident wave of 256-thread CTAs (148 SMs x 8), split over the images
-    dim3 grid(std::max(1, std::min(ceil_div(words, 8), ceil_div(148 * 8, B))), B);
+    // about one resident wave of 256-thread CTAs (132 SMs x 8), split over the images
+    dim3 grid(std::max(1, std::min(ceil_div(words, 8), ceil_div(132 * 8, B))), B);
     if (low && !(LH == H && LW == W))
         seg_prob_kernel<true><<<grid, 256, 0, s>>>((const float2*)low, (float2*)const_cast<float*>(logits), LH, LW, (float)LH / (float)H,
                                                    (float)LW / (float)W, H, W, Ww, key, det);
@@ -658,8 +658,8 @@ crop_image_kernel(const float* __restrict__ image, const float* __restrict__ cen
 int launch_crop_image(const float* image, const float* center, const float* scale, float* out, int B, int H, int W, int C,
                       int crop, cudaStream_t s) {
     const int total = crop * crop;
-    // about one resident wave: 148 SMs x 8 CTAs of 256 threads, split over the images (at least 1, at most one CTA per 256 pixels)
-    const int per_image = std::max(1, std::min(ceil_div(total, 256), ceil_div(148 * 8, std::max(1, B))));
+    // about one resident wave: 132 SMs x 8 CTAs of 256 threads, split over the images (at least 1, at most one CTA per 256 pixels)
+    const int per_image = std::max(1, std::min(ceil_div(total, 256), ceil_div(132 * 8, std::max(1, B))));
     crop_image_kernel<<<dim3((unsigned)per_image, B), 256, 0, s>>>(image, center, scale, out, B, H, W, C, crop);
     H3D_CHECK_LAUNCH();
     return H3D_OK;
@@ -882,7 +882,7 @@ int launch_resize_argmax21(const float* x, float* y, int B, int H, int W, int oh
         return H3D_OK;
     }
     const int P = 256 / C;
-    dim3 grid(std::max(1, std::min(ceil_div(oh * ow, P * 8), 4 * 148 / std::max(1, std::min(B, 4)))), B);
+    dim3 grid(std::max(1, std::min(ceil_div(oh * ow, P * 8), 4 * 132 / std::max(1, std::min(B, 4)))), B);
     resize_argmax_kernel<C><<<grid, P * C, (size_t)P * C * 8, s>>>(x, y, H, W, oh, ow, (float)H / (float)oh, (float)W / (float)ow, P, key);
     H3D_CHECK_LAUNCH();
     argmax_decode_kernel<<<ceil_div(B * C, 256), 256, 0, s>>>(key, B * C, ow, uv);
@@ -940,7 +940,7 @@ int launch_decode_records(const uint8_t* rec, int64_t record_bytes, int header_f
                           int64_t mask_off, int tail_bytes, float* header, float* image, uint8_t* mask, uint8_t* tail, int B,
                           cudaStream_t s) {
     const int64_t total = (int64_t)B * (H / step) * (W / step) * 3;
-    decode_records_kernel<<<(int)std::min<int64_t>(ceil_div64(total, 256), 148 * 16), 256, 0, s>>>(
+    decode_records_kernel<<<(int)std::min<int64_t>(ceil_div64(total, 256), 132 * 16), 256, 0, s>>>(
         rec, record_bytes, header_floats, image_off, H, W, step, mask_off, tail_bytes, header, image, mask, tail, B);
     H3D_CHECK_LAUNCH();
     return H3D_OK;
@@ -1165,7 +1165,7 @@ __global__ void leaky_relu_kernel(const float* __restrict__ x, float* __restrict
 }
 int launch_leaky_relu(const float* x, float* y, int64_t n, cudaStream_t s) {
     H3D_REQUIRE((((uintptr_t)x | (uintptr_t)y) & 15) == 0, "leaky_relu: pointers must be 16-byte aligned");
-    leaky_relu_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(ceil_div64(n / 4 + 1, 256), 148 * 16)), 256, 0, s>>>(x, y, n);
+    leaky_relu_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(ceil_div64(n / 4 + 1, 256), 132 * 16)), 256, 0, s>>>(x, y, n);
     H3D_CHECK_LAUNCH();
     return H3D_OK;
 }

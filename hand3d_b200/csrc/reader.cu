@@ -197,7 +197,7 @@ __global__ void gaussian_map_kernel(const float* __restrict__ coords_hw, const u
 int launch_gaussian_map(const float* coords_hw, const uint8_t* valid, int B, int N, int H, int W, float sigma, float* out, cudaStream_t s) {
     H3D_REQUIRE(N >= 1 && N <= kMaxGaussKp && ((W * N) & 3) == 0, "gaussian_scoremap: N must be in [1,64] and W * N a multiple of 4");
     const int64_t total = (int64_t)H * (W * N / 4);
-    dim3 grid((unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div64(total, 256), 148 * 8 / std::max(1, std::min(B, 8)))), B);
+    dim3 grid((unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div64(total, 256), 132 * 8 / std::max(1, std::min(B, 8)))), B);
     gaussian_map_kernel<<<grid, 256, 0, s>>>(coords_hw, valid, N, H, W, sigma * sigma, out);
     H3D_CHECK_LAUNCH();
     return H3D_OK;

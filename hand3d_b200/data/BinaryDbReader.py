@@ -1,4 +1,4 @@
-"""BinaryDbReader / BinaryDbReaderSTB -- B200-native mirrors of the reference's dataset readers for the EVALUATION drivers
+"""BinaryDbReader / BinaryDbReaderSTB -- H100-native mirrors of the reference's dataset readers for the EVALUATION drivers
 (data/BinaryDbReader.py:21-412, data/BinaryDbReaderSTB.py:21-330): same constructor arguments, `num_samples`, and `get()`
 returning the same dictionary keys, but eager: every get() call uploads the next `batch_size` fixed-length records as bytes and
 produces the raw and derived items on the GPU (h3d_decode_records, h3d_rhd_reader_items / h3d_stb_reader_items,

@@ -1,7 +1,7 @@
-"""ColorHandPose3DNetwork -- B200-native forward pass behind the reference's Python API
+"""ColorHandPose3DNetwork -- H100-native forward pass behind the reference's Python API
 (nets/ColorHandPose3DNetwork.py:28-384): same class / method names, argument order, NHWC float32
 tensors and return-tuple order, eager over torch CUDA tensors.  All arithmetic runs in
-libhand3d_b200.so (hand-written sm_100a kernels); there is no TF session and no CPU fallback.
+libhand3d_b200.so (hand-written sm_90a kernels); there is no TF session and no CPU fallback.
 """
 from __future__ import annotations
 

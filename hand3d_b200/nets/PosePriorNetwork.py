@@ -1,6 +1,6 @@
 """PosePriorNetwork -- lifting 2D score maps to 3D behind the reference's API
 (nets/PosePriorNetwork.py:29-159).  All five variants ('direct', 'bottleneck', 'local',
-'local_w_xyz_loss', 'proposed') run on the same sm_100a kernels as ColorHandPose3DNetwork; the 'local*' variants add
+'local_w_xyz_loss', 'proposed') run on the same sm_90a kernels as ColorHandPose3DNetwork; the 'local*' variants add
 the forward-kinematics kernel that replaces bone_rel_trafo_inv (utils/relative_trafo.py:243-295).
 """
 from __future__ import annotations

@@ -39,7 +39,7 @@ class Context:
     def __init__(self, device=None, precision="bf16x3"):
         self.lib = _lib.load()
         if not torch.cuda.is_available():
-            raise RuntimeError("hand3d_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("hand3d_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
         h = C.c_void_p()
         _lib.check(self.lib.h3d_create(C.byref(h), self.device.index), "h3d_create")

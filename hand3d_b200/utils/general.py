@@ -1,6 +1,6 @@
-"""B200-native mirror of the reference's utils/general.py hot-path helpers (same names, argument
+"""H100-native mirror of the reference's utils/general.py hot-path helpers (same names, argument
 order, NHWC layouts and return conventions), eager over torch CUDA tensors and backed by the
-hand-written sm_100a kernels behind the C ABI (include/hand3d_b200.h).
+hand-written sm_90a kernels behind the C ABI (include/hand3d_b200.h).
 
 Reference: utils/general.py:26-65,113-148 (NetworkOps), :163 crop_image_from_xy, :199 find_max_location,
 :233 single_obj_scoremap, :271 calc_center_bb, :331 detect_keypoints, :347 trafo_coords.

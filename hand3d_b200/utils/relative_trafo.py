@@ -1,4 +1,4 @@
-"""B200-native mirror of utils/relative_trafo.py's inference-time entry point.
+"""H100-native mirror of utils/relative_trafo.py's inference-time entry point.
 
 bone_rel_trafo_inv (reference :243-295) assembles bone-relative coordinates (length, angle_x, angle_y per bone
 of the 21-node kinematic chain) back into xyz coordinates; it is the only function of that module on the forward

@@ -1,5 +1,5 @@
 /*
- * hand3d_b200 -- C ABI of the B200-native ColorHandPose3D forward pass.
+ * hand3d_b200 -- C ABI of the H100-native ColorHandPose3D forward pass.
  *
  * The reference (lmb-freiburg/hand3d) has no FFI boundary: its hot path sits behind the Python API
  * of nets/ColorHandPose3DNetwork.py / nets/PosePriorNetwork.py / utils/general.py and resolves to
@@ -18,7 +18,7 @@
  *   - return 0 on success, negative H3D_E* on failure; h3d_last_error() gives a thread-local message;
  *   - one h3d_ctx per device, used from one host thread at a time (one rank <-> one GPU); every entry makes the context's device
  *     current for the duration of the call and restores the caller's device;
- *   - there is NO CPU fallback: without a usable sm_100a device every compute call fails with
+ *   - there is NO CPU fallback: without a usable sm_90a device every compute call fails with
  *     H3D_ENODEVICE.
  */
 #ifndef HAND3D_B200_H_
@@ -46,11 +46,11 @@ extern "C" {
 
 /* Arithmetic of the tensor-core convolution layers. */
 #define H3D_PREC_FP32_FFMA 0  /* all layers on CUDA cores in fp32 (validation yard-stick)             */
-#define H3D_PREC_BF16X3 1     /* tcgen05, bf16 hi/lo split, 3 MMA passes, fp32 accumulate (fp32 parity) */
-#define H3D_PREC_FP16X3 2     /* tcgen05, fp16 hi/lo split, 3 MMA passes, fp32 accumulate (fp32 parity) */
-#define H3D_PREC_FP16 3       /* tcgen05, fp16 single pass, fp32 accumulate (BASELINE config 5, 1e-2)   */
-#define H3D_PREC_BF16 4       /* tcgen05, bf16 single pass                                              */
-#define H3D_PREC_FP16_F8C 5   /* tcgen05, fp16 main pass + two fp8 (e4m3) correction passes, fp32 accumulate (fp32 parity) */
+#define H3D_PREC_BF16X3 1     /* wgmma,   bf16 hi/lo split, 3 MMA passes, fp32 accumulate (fp32 parity) */
+#define H3D_PREC_FP16X3 2     /* wgmma,   fp16 hi/lo split, 3 MMA passes, fp32 accumulate (fp32 parity) */
+#define H3D_PREC_FP16 3       /* wgmma,   fp16 single pass, fp32 accumulate (BASELINE config 5, 1e-2)   */
+#define H3D_PREC_BF16 4       /* wgmma,   bf16 single pass                                              */
+#define H3D_PREC_FP16_F8C 5   /* wgmma,   fp16 main pass + two fp8 (e4m3) correction passes, fp32 accumulate (fp32 parity) */
 
 /* PosePriorNetwork variants (nets/PosePriorNetwork.py:64-93). */
 #define H3D_VARIANT_DIRECT 0
@@ -72,23 +72,23 @@ H3D_API int h3d_set_precision(h3d_ctx* ctx, int precision);
 H3D_API int h3d_get_precision(const h3d_ctx* ctx);
 /* Kernel-selection switches for A/B measurements and forced-variant tests (process-wide; initialised ONCE from the H3D_*
  * environment variables when the library is first used, never read on a launch path).  Keys: "tc_2cta" (-1 policy / 0 / 1),
- * "tc_bn" (0 policy / 64 / 128 / 256), "tc_c64", "tc_c64x2", "tc_pair128", "tc_stack", "tc_chunk_kb", "no_side_stream",
- * "no_pool_fusion", "lift_direct", "c3_ffma", "c3_tma", "pdl", "fc_chain", "c64_tma_out", "tc_chain" (layer chains: 0 off / 1 tile
- * tickets + per-image dependencies / 2 tickets only), "tc_small_split" (narrow tiles for small batches), "fuse_c1" (conv1_1 inside
- * conv1_2's kernel), "no_seg_fusion".  ctx may be NULL; when given, its cached layer plans are dropped (never while a CUDA graph
- * captured from this context is alive: graphs hold plan-owned pointers). */
+ * "tc_bn" (0 policy / 64 / 128), "tc_c64", "tc_c64x2", "tc_pair128", "tc_stack", "tc_chunk_kb", "no_side_stream",
+ * "no_pool_fusion", "lift_direct", "c3_ffma", "c3_tma", "pdl", "fc_chain", "c64_tma_out", "tc_chain", "tc_small_split", "fuse_c1",
+ * "no_seg_fusion".  "tc_2cta", "tc_c64", "tc_c64x2", "tc_pair128", "tc_stack", "c3_tma", "c64_tma_out", "tc_chain", "tc_small_split"
+ * and "fuse_c1" select nothing in the sm_90a build (one convolution kernel family) and are accepted for compatibility.
+ * ctx may be NULL; when given, its cached layer plans are dropped (never while a CUDA graph captured from this context is alive:
+ * graphs hold plan-owned pointers). */
 H3D_API int h3d_set_tuning(h3d_ctx* ctx, const char* key, int value);
-/* Device-side error word (pinned host memory, survives a trapped kernel): 0 = none; 1-5 = a bounded mbarrier wait of a tcgen05
- * convolution kernel timed out (1 TMA producer / free stage, 2 MMA issuer / drained accumulator, 3 MMA issuer / TMA stage,
- * 4 epilogue / finished accumulator, 5 MMA issuer / resident weights or tile-ticket ring, 6 ticket ring consumer, 7 per-image
- * dependency of a chained layer, 11-15 fused first-layer pipeline) and the kernel trapped; 100 + r = h3d_gather_records_p2p
+/* Device-side error word (pinned host memory, survives a trapped kernel): 0 = none; 1-5 = a bounded mbarrier wait of a tensor-core
+ * convolution kernel timed out (1 TMA producer waiting for a free stage, 3 wgmma warpgroup waiting for a loaded stage) and the
+ * kernel trapped; 100 + r = h3d_gather_records_p2p
  * never saw peer rank r's records.  Returns H3D_OK or H3D_ECUDA (message in h3d_last_error); *code (optional) = the word. */
 H3D_API int h3d_check_errors(h3d_ctx* ctx, int* code);
 /* Number of kernels this library launched through `ctx` since creation (bench "gpu_launches"). */
 H3D_API int64_t h3d_launch_count(const h3d_ctx* ctx);
 
 /* Per-kernel-class device timing for bench.py's roofline: between begin and end every plan step is
- * bracketed by CUDA events on its launch stream.  Classes: 0 = tcgen05 conv, 1 = CUDA-core conv,
+ * bracketed by CUDA events on its launch stream.  Classes: 0 = tensor-core conv, 1 = CUDA-core conv,
  * 2 = fully connected, 3 = other.  end() synchronises and fills three arrays of length 4. */
 H3D_API int h3d_profile_begin(h3d_ctx* ctx);
 H3D_API int h3d_profile_end(h3d_ctx* ctx, double* ms_by_kind, int64_t* flops_by_kind, int64_t* launches_by_kind);
@@ -147,7 +147,7 @@ H3D_API int h3d_pose2d_forward(h3d_ctx* ctx, const float* image_crop, int B, int
  * fp32 CUDA-core kernel; x [B,H,W,Cin], w HWIO [k,k,Cin,Cout] (device), y [B,ceil(H/s),ceil(W/s),Cout]. */
 H3D_API int h3d_conv2d_f32(h3d_ctx* ctx, const float* x, const float* w_hwio, const float* bias, float* y,
                    int B, int H, int W, int Cin, int Cout, int ksize, int stride, int leaky, void* stream);
-/* Same op on the tcgen05 tensor-core path (stride 1, Cin and Cout multiples of 64 after internal padding;
+/* Same op on the wgmma tensor-core path (stride 1, Cin and Cout multiples of 64 after internal padding;
  * ksize in {1,3,5,7}); host_w_hwio / host_bias are HOST pointers: this convenience entry packs, uploads and frees the weights
  * around the call (allocates, and the free waits for the kernel) -- use h3d_pack_conv_weights + h3d_conv2d_tc_packed on a hot path. */
 H3D_API int h3d_conv2d_tc(h3d_ctx* ctx, const float* x, const float* host_w_hwio, const float* host_bias, float* y,

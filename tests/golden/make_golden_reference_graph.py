@@ -1,4 +1,4 @@
-"""Golden tensors produced by running the reference's own GRAPH-BUILDING code (unmodified, imported from /root/reference) over an
+"""Golden tensors produced by running the reference's own GRAPH-BUILDING code (unmodified, imported from a checkout of lmb-freiburg/hand3d ($H3D_REFERENCE)) over an
 eager numpy stand-in for `tensorflow` (oracle/tf1_eager.py).
 
 What this pins and what it does not: the layer lists, variable names and shapes, strides, pool positions, concat order, mask growing
@@ -8,7 +8,7 @@ oracle's restatement of the published TF 1.3 kernels (oracle/tf1_ops.py), becaus
 tensors pin oracle/hand3d_oracle.py's restatement of the GRAPH (and through it the CUDA path) to the reference source; the op
 semantics stay pinned by the known-answer tests only.
 
-    python tests/golden/make_golden_reference_graph.py        # only where /root/reference exists; ~1 minute of CPU
+    python tests/golden/make_golden_reference_graph.py        # H3D_REFERENCE=<checkout of lmb-freiburg/hand3d>; ~1 minute of CPU
 """
 import os
 import sys
@@ -18,7 +18,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = os.environ.get("H3D_REFERENCE", "/root/reference")
+REF = os.environ.get("H3D_REFERENCE", "")   # a checkout of lmb-freiburg/hand3d (needed only to regenerate)
 OUT = os.path.join(HERE, "golden_reference_graph.npz")
 
 

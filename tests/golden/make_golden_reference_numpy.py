@@ -4,11 +4,11 @@ TensorFlow 1.3 cannot be installed here, so the TF graph functions of the refere
 `utils/general.py` however also holds the host-side numpy code of the path -- `detect_keypoints` (:331-344), `trafo_coords`
 (:347-357), `EvalUtil` (:522-611) and `calc_auc` (:654-659) -- and the module only needs `import tensorflow` to succeed.  This script
 puts an EMPTY stand-in module named `tensorflow` into `sys.modules`, imports the reference file from where it lies
-(/root/reference, read-only, nothing is copied), runs those functions on seeded inputs and stores inputs + outputs in
+(a checkout of lmb-freiburg/hand3d named by $H3D_REFERENCE, read-only, nothing is copied), runs those functions on seeded inputs and stores inputs + outputs in
 `golden_reference_numpy.npz`.  tests/test_reference_numpy_golden.py pins the oracle, the host-side mirror and (on the GPU) the
 device kernels against it.
 
-    python tests/golden/make_golden_reference_numpy.py        # only where /root/reference exists
+    python tests/golden/make_golden_reference_numpy.py        # H3D_REFERENCE=<checkout of lmb-freiburg/hand3d>
 """
 import importlib.util
 import os
@@ -17,7 +17,7 @@ import types
 
 import numpy as np
 
-REF = os.environ.get("H3D_REFERENCE", "/root/reference")
+REF = os.environ.get("H3D_REFERENCE", "")   # a checkout of lmb-freiburg/hand3d (needed only to regenerate)
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden_reference_numpy.npz")
 
 

@@ -1,6 +1,6 @@
 """Golden vectors of the dataset readers' derived items, produced by running the reference's UNMODIFIED reader classes
 (data/BinaryDbReader.py, data/BinaryDbReaderSTB.py, with utils/canonical_trafo.py, utils/relative_trafo.py, utils/general.py
-underneath -- all imported from /root/reference) over the eager TF stand-in (oracle/tf1_eager.py) on seeded synthetic records
+underneath -- all imported from a checkout of lmb-freiburg/hand3d ($H3D_REFERENCE)) over the eager TF stand-in (oracle/tf1_eager.py) on seeded synthetic records
 (tests/golden/synth_records.py) written to the file names the readers insist on.
 
 Pins oracle/reader_oracle.py (and through it the CUDA generators of SURVEY.md 8(f) row 4) to the reference SOURCE: palm / wrist
@@ -8,10 +8,12 @@ substitution, dominant-hand rule, 21-key-point subsets, root-relative normalisat
 create_multiple_gaussian_map, scale_to_size, convert_kp, canonical_trafo.  The heavy TF ops underneath (crop_and_resize, legacy
 resize) are oracle/tf1_ops.py, pinned separately by tests/test_tf_published_vectors.py.
 
-    python tests/golden/make_golden_reference_reader.py       # only where /root/reference exists; ~1 minute of CPU
+    python tests/golden/make_golden_reference_reader.py       # H3D_REFERENCE=<checkout of lmb-freiburg/hand3d>; ~1 minute of CPU
 Large tensors (image, image_crop, scoremap) are stored as an 8x sub-sampled copy plus float64 sum / sum of squares.
 """
+import io
 import os
+import zipfile
 import sys
 import tempfile
 import types
@@ -20,7 +22,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = os.environ.get("H3D_REFERENCE", "/root/reference")
+REF = os.environ.get("H3D_REFERENCE", "")   # a checkout of lmb-freiburg/hand3d (needed only to regenerate)
 OUT = os.path.join(HERE, "golden_reference_reader.npz")
 sys.path.insert(0, HERE)
 import synth_records as SR  # noqa: E402
@@ -93,7 +95,12 @@ def main():
                     pack("%s/%d" % (name, i), stb.BinaryDbReaderSTB(**kw).get(), out)
         finally:
             os.chdir(cwd)
-    np.savez_compressed(OUT, **out)
+    # LZMA-compressed members (np.load reads them): the file stays below 1 MB
+    with zipfile.ZipFile(OUT, "w", compression=zipfile.ZIP_LZMA) as z:
+        for k, v in out.items():
+            b = io.BytesIO()
+            np.save(b, np.asarray(v))
+            z.writestr(k + ".npy", b.getvalue())
     print("wrote %s: %d arrays, %.1f KB" % (OUT, len(out), os.path.getsize(OUT) / 1024))
 
 

@@ -1,5 +1,5 @@
 """CPU-side checks of the boundary: the library loads without a GPU, exports every symbol that
-include/hand3d_b200.h declares, and refuses to compute (loudly) when no sm_100a device is present."""
+include/hand3d_b200.h declares, and refuses to compute (loudly) when no sm_90a device is present."""
 import ctypes as C
 import os
 import re

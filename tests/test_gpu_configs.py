@@ -1,8 +1,8 @@
 """GPU parity at the BASELINE.json configurations' own batch sizes, against the CPU oracle (never CUDA against CUDA):
 config 2 (PoseNet-only, 32 crops of 256x256), config 3 (inference2d, 64 images of 320x320), config 5 (single-pass fp16 full
 pipeline, 64 images, tolerance 1e-2) and the fp32-parity full pipeline over 64 images with its free-running mismatch rates.
-The thresholds on the rates are the rates measured on the B200 (profiles/r02_mismatch.json, scripts/mismatch_report.py) with a
-small margin; the continuous tolerances are BASELINE.json's (1e-3 fp32 parity, 1e-2 fp16)."""
+The thresholds on the rates are rates measured with scripts/mismatch_report.py plus a small margin; the continuous tolerances
+are BASELINE.json's (1e-3 fp32 parity, 1e-2 fp16)."""
 import os
 import sys
 

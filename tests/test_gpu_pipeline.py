@@ -57,9 +57,8 @@ def test_handsegnet_stage(net, ctx, seg_ref, prec):
 
 @pytest.mark.parametrize("knobs", [{"fuse_c1": 0}, {"fuse_c1": 0, "c3_tma": 0}, {"fuse_c1": 0, "c3_ffma": 1}], ids=["c3_tma", "c3_tc", "c3_ffma"])
 def test_first_layer_kernel_variants(net, ctx, seg_ref, knobs):
-    """conv1_1 has four implementations: fused into conv1_2's kernel (conv_c1f_kernel: default, covered by every other test), and as
-    its own launch on tensor cores with bulk-tensor-store epilogue (fuse_c1 = 0), with direct global stores (c3_tma = 0) or as the
-    register-tiled FFMA kernel (c3_ffma = 1); all must give the HandSegNet parity."""
+    """conv1_1 runs on the tensor cores (conv_c3_tc_kernel, default) or as the register-tiled FFMA kernel (c3_ffma = 1); fuse_c1 and
+    c3_tma are accepted without effect on sm_90a.  Every setting must give the HandSegNet parity."""
     img, ref = seg_ref
     ctx.set_precision("bf16x3")
     default = {"fuse_c1": 1, "c3_tma": 1, "c3_ffma": 0}
@@ -77,9 +76,8 @@ def test_first_layer_kernel_variants(net, ctx, seg_ref, knobs):
 @pytest.mark.parametrize("prec", ["bf16x3", "fp16x3"])
 @pytest.mark.parametrize("shape", [(3, 40, 40), (1, 24, 56), (2, 72, 48)])
 def test_handsegnet_small_odd_maps(net, ctx, wd, shape, prec, fused):
-    """Maps that are no multiple of the 16 x 8 pixel tile, odd numbers of tiles (the CTA pair's second tile falls outside the batch) and
-    tiles that lie entirely in conv1_2's zero padding: exercises the masking of the 64-channel pair kernel and of the fused
-    conv1_1 + conv1_2 kernel."""
+    """Maps that are no multiple of the pixel tile, odd numbers of tiles and tiles that lie entirely in conv1_2's zero padding:
+    exercises the masking of the first-layer and the implicit-GEMM kernels (with fuse_c1 set to 0 and 1)."""
     B, H, W = shape
     img = Wt.synthetic_images(B, H, W, seed=17)
     ctx.set_precision(prec)
@@ -94,7 +92,7 @@ def test_handsegnet_small_odd_maps(net, ctx, wd, shape, prec, fused):
 
 
 def test_fused_first_layers_full_pipeline(net, ctx, wd):
-    """The fused conv1_1 + conv1_2 kernel (default) against the two separate kernels through the whole pipeline: 1e-3 maps, identical crops."""
+    """The default first layers against fuse_c1 = 0 through the whole pipeline: 1e-3 maps, identical crops."""
     B = 4
     img = np.concatenate([Wt.synthetic_images(2, 320, 320, seed=51), Wt.synthetic_blob_images(2, 320, 320, seed=52)], 0)
     hs = Wt.synthetic_hand_side(B, seed=53)
@@ -136,7 +134,7 @@ def test_posenet_stage(net, ctx, pose_ref, prec):
         assert err < TOL[prec], "PoseNet %s stage %d: max abs err %.3e" % (prec, i, err)
 
 
-# fp32_ffma: fp32 CUDA-core pyramids; bf16x3 / fp16x3: tcgen05 pyramids (stride 2 = odd pixels of the stride-1 result), branches on two streams
+# fp32_ffma: fp32 CUDA-core pyramids; bf16x3 / fp16x3: wgmma pyramids (stride 2 = odd pixels of the stride-1 result), branches on two streams
 @pytest.mark.parametrize("prec", ["fp32_ffma", "bf16x3", "fp16x3"])
 @pytest.mark.parametrize("variant", ["proposed", "direct"])
 def test_lifting_stage(ctx, wd, variant, prec):

@@ -112,9 +112,9 @@ def test_cuda_graph_replay_matches_eager(ctx):
 
 @pytest.mark.parametrize("prec", ["bf16x3", "fp16"])
 def test_layer_chains_change_no_bit(ctx, prec):
-    """Layer chains (dynamic tile tickets + per-image dependencies between consecutive CTA-pair conv launches, conv_tc.cu) only
-    re-order WHEN a tile is computed: chain = 1 (default), 2 (tickets only) and 0 (static round-robin, griddepcontrol.wait) must
-    give bit-identical outputs, repeatedly (B = 32 and a ragged B = 7, back-to-back calls so that consecutive steps overlap too)."""
+    """The tc_chain switch (layer chains of an earlier build; no effect in the sm_90a build) must not change a bit: chain = 1
+    (default), 2 and 0 give bit-identical outputs, repeatedly (B = 32 and a ragged B = 7, back-to-back calls so that consecutive
+    steps overlap too)."""
     ctx.set_precision(prec)
     try:
         for B in (32, 7):

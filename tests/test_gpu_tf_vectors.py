@@ -34,7 +34,7 @@ def test_tf_conv2d_same_vectors_fp32_kernel(ctx, case):
 
 
 def test_tf_conv2d_1x1_vector_tensor_core_kernel(ctx):
-    """testConv2D1x1Filter through the tcgen05 implicit-GEMM kernel (channels zero-padded 3 -> 64 on both sides): small
+    """testConv2D1x1Filter through the wgmma implicit-GEMM kernel (channels zero-padded 3 -> 64 on both sides): small
     integers are exact in bf16 hi/lo split arithmetic."""
     _, xs, ws, _, expected = TF_CONV_SAME[0]
     y = ctx.conv2d_tc(_cuda(_seq(xs)), _seq(ws), np.zeros(ws[3], f32), leaky=False, precision="bf16x3").cpu().numpy()

@@ -2,7 +2,7 @@
 
 `tests/golden/golden_reference_graph.npz` was produced by tests/golden/make_golden_reference_graph.py: the UNMODIFIED
 nets/ColorHandPose3DNetwork.py, nets/PosePriorNetwork.py, utils/general.py and utils/relative_trafo.py of the reference, imported
-from /root/reference and executed function by function over an eager numpy stand-in for `tensorflow` (oracle/tf1_eager.py).  The
+from a checkout of lmb-freiburg/hand3d and executed function by function over an eager numpy stand-in for `tensorflow` (oracle/tf1_eager.py).  The
 structure of the computation (layers, names, strides, concat order, mask growing, crop arithmetic, Rodrigues / flip, kinematic
 chain, tuple orders) therefore comes from the reference source; the heavy ops underneath are the oracle's restatement of the TF 1.3
 kernels, so op-level semantics remain pinned by tests/test_oracle_kat.py only."""

@@ -1,7 +1,7 @@
 """Pins the oracle, the host-side API mirror and the device kernels against outputs of the UNMODIFIED reference.
 
 `tests/golden/golden_reference_numpy.npz` was produced by tests/golden/make_golden_reference_numpy.py, which imports
-/root/reference/utils/general.py (with an empty stand-in for the `tensorflow` import) and runs the reference's own numpy code of
+the reference's utils/general.py (with an empty stand-in for the `tensorflow` import) and runs the reference's own numpy code of
 the hot path: detect_keypoints (utils/general.py:331-344), trafo_coords (:347-357), EvalUtil (:522-611), calc_auc (:654-659).
 These are the only functions of the path that can execute without TensorFlow 1.3; for them parity is pinned to the reference
 itself, bit for bit (indices) / to 1e-12 (float64 arithmetic)."""
