@@ -116,6 +116,9 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, void* dst, u
         ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
+// Register reallocation between the warpgroups of a CTA (executed by all 128 threads of a warpgroup)
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
@@ -485,6 +488,12 @@ __device__ __forceinline__ void store_tile(const TcParams& p, const float* racc,
 }
 
 // ------------------------------------------------------------------------------------------ convolution kernel
+// Registers per thread after the reallocation at kernel start: __launch_bounds__(384, 1) gives every thread 168, which the BN = 128
+// consumers exceed (two fp32 fragments of 64 registers + descriptors: racc spilled to local memory), while the producer warpgroup
+// only walks the K loop.  2 * 128 * 232 + 128 * 40 <= 65536.  setmaxnreg.inc only redistributes what the CTA was given at launch, so
+// every instance must stay allocated at 168 per thread (ptxas does so for kernels with setmaxnreg; tests/test_build_registers.py).
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+
 template <int BN, int PASSES, bool FP16>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
@@ -518,20 +527,24 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_consta
     pdl_launch_dependents();
     pdl_wait();
 
-    if (warp == 0) {
-        // ================================ TMA producer (whole warp, one elected lane issues) ================================
-        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-            const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
-            const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h, tb = mt / (p.tiles_w * p.tiles_h);
-            const int w0 = tw * p.TW - p.pad, h0 = th * p.TH - p.pad, b0 = tb * p.TB, n0 = nt * BN;
-            int kcol = 0;
-            for (int kh = 0; kh < p.k; ++kh)
-                for (int kw = 0; kw < p.k; ++kw)
-                    for (int cc = 0; cc < p.cin_chunks; ++cc, kcol += BK)
-                        produce_kblock<BN, PASSES>(ring, &map_x_hi, &map_x_lo, &map_x_h8, &map_w_hi, &map_w_lo, &map_w_l8, cc * BK, w0 + kw,
-                                                   h0 + kh, b0, kcol, n0, p.err_flag);
+    if (wg == 0) {
+        setmaxnreg_dec<kProducerRegs>();
+        if (warp == 0) {
+            // ================================ TMA producer (whole warp, one elected lane issues) ================================
+            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+                const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
+                const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h, tb = mt / (p.tiles_w * p.tiles_h);
+                const int w0 = tw * p.TW - p.pad, h0 = th * p.TH - p.pad, b0 = tb * p.TB, n0 = nt * BN;
+                int kcol = 0;
+                for (int kh = 0; kh < p.k; ++kh)
+                    for (int kw = 0; kw < p.k; ++kw)
+                        for (int cc = 0; cc < p.cin_chunks; ++cc, kcol += BK)
+                            produce_kblock<BN, PASSES>(ring, &map_x_hi, &map_x_lo, &map_x_h8, &map_w_hi, &map_w_lo, &map_w_l8, cc * BK,
+                                                       w0 + kw, h0 + kh, b0, kcol, n0, p.err_flag);
+            }
         }
-    } else if (wg >= 1) {
+    } else {
+        setmaxnreg_inc<kConsumerRegs>();
         // ================================ wgmma + epilogue (warpgroups 1 and 2) ================================
         const int ct = threadIdx.x - 128;
         float racc[BN / 2];
