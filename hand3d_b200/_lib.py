@@ -47,8 +47,11 @@ SIGNATURES = {
     "h3d_pack_conv_weights": (_i, [_p, _p, _p, _i, _i, _i, _i, C.POINTER(_p)]),
     "h3d_free_packed_conv": (_i, [_p, _p]),
     "h3d_conv2d_tc_packed": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _p]),
+    "h3d_conv2d_tc_dev": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
+    "h3d_conv2d_tc_backward": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
     "h3d_leaky_relu_f32": (_i, [_p, _p, _p, _i64, _p]),
     "h3d_maxpool2x2_f32": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),
+    "h3d_maxpool2x2_backward_f32": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _p]),
     "h3d_fully_connected_f32": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _p]),
     "h3d_resize_bilinear_tf1": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _i, _p]),
     "h3d_avgpool8": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),

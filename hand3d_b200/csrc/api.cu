@@ -1374,22 +1374,24 @@ int h3d_free_packed_conv(h3d_ctx* ctx, h3d_packed_conv* packed) {
     return H3D_OK;
 }
 
-int h3d_conv2d_tc_packed(h3d_ctx* ctx, const float* x, const h3d_packed_conv* packed, float* y, int B, int H, int W, int stride,
-                         int leaky, void* stream) {
-    H3D_OP_PROLOGUE(ctx);
-    H3D_REQUIRE(x && packed && y && B > 0, "h3d_conv2d_tc_packed: bad argument");
-    const int ksize = packed->k, Cin = packed->Cin, Cout = packed->Cout, precision = packed->precision;
+// Body shared by h3d_conv2d_tc_packed and h3d_conv2d_tc_dev.  Operand planes are carved from the context's operator scratch:
+// [x hi | x lo / l8 h8 | y hi | y lo / l8 h8 | wbytes for the caller's weight planes]; pack(wbase, &pw) provides the packed weights
+// (enqueueing their packing when they live in the scratch) before x is split and the convolution runs.
+extern "C++" {   // a template inside the C ABI block
+template <class PackFn>
+static int conv_tc_run(h3d_ctx* ctx, const float* x, float* y, int B, int H, int W, int Cin, int Cout, int ksize, int stride, int leaky,
+                       int precision, int Cin_pad, int Cout_pad, int64_t wbytes, PackFn pack, cudaStream_t s) {
     H3D_REQUIRE(stride == 1 || (stride == 2 && H % 2 == 0 && W % 2 == 0 && ksize >= 3),
                 "h3d_conv2d_tc: stride must be 1, or 2 with even H and W and ksize >= 3 (for ksize 1 TF's 'SAME' samples the even pixels)");
     const Half16 half = half_of(precision);
     const int passes = passes_of(precision);
-    const int Cin_pad = packed->pw.Cin_pad, Cout_pad = packed->pw.Cout_pad;
     const int64_t rows = (int64_t)B * H * W, rows_out = rows / (stride * stride);
-    // operand planes carved from the context's operator scratch: [x hi | x lo / l8 h8 | y hi | y lo / l8 h8]
     const int64_t xb = align_up(rows * Cin_pad * 2, 1024), yb = align_up(rows_out * Cout_pad * 2, 1024);
     char* base = nullptr;
-    int rc = op_scratch(ctx, 2 * xb + 2 * yb, &base);
+    int rc = op_scratch(ctx, 2 * xb + 2 * yb + wbytes, &base);
     if (rc) return rc;
+    PackedW pw;
+    if ((rc = pack(base + 2 * xb + 2 * yb, &pw))) return rc;
     Split xs, ys;
     xs.hi = (uint16_t*)base; ys.hi = (uint16_t*)(base + 2 * xb);
     if (passes == 3) { xs.lo = (uint16_t*)(base + xb); ys.lo = (uint16_t*)(base + 2 * xb + yb); }
@@ -1399,9 +1401,9 @@ int h3d_conv2d_tc_packed(h3d_ctx* ctx, const float* x, const h3d_packed_conv* pa
     }
     if ((rc = launch_f32_to_split(x, xs, rows, Cin, Cin_pad, half, s))) return rc;
     TcConvDesc d;
-    d.x = xs; d.Cin_total = Cin_pad; d.Cin_pad = Cin_pad; d.w = packed->pw.w; d.bias = packed->pw.bias; d.Cout = Cout; d.Cout_pad = Cout_pad;
+    d.x = xs; d.Cin_total = Cin_pad; d.Cin_pad = Cin_pad; d.w = pw.w; d.bias = pw.bias; d.Cout = Cout; d.Cout_pad = Cout_pad;
     d.y = ys; d.Cy_total = Cout_pad; d.cy_off = 0; d.yf = nullptr; d.Cyf_total = 0; d.cyf_off = 0;
-    d.B = B; d.H = H; d.W = W; d.k = ksize; d.leaky = leaky; d.passes = passes; d.half = half; d.corr_scale = packed->pw.corr_scale;
+    d.B = B; d.H = H; d.W = W; d.k = ksize; d.leaky = leaky; d.passes = passes; d.half = half; d.corr_scale = pw.corr_scale;
     d.pool = stride == 2 ? 2 : 0;
     d.err_flag = ctx->err_flag;
     TcConvPlan* tp = tc_conv_plan_create(d);     // host-side only: tensor maps + launch geometry (passed to the kernel by value)
@@ -1411,6 +1413,113 @@ int h3d_conv2d_tc_packed(h3d_ctx* ctx, const float* x, const h3d_packed_conv* pa
     if (rc) return rc;
     if ((rc = launch_split_to_f32(ys, y, rows_out, Cout, Cout_pad, half, s))) return rc;
     ctx->launches += 3;
+    return H3D_OK;
+}
+}  // extern "C++"
+
+int h3d_conv2d_tc_packed(h3d_ctx* ctx, const float* x, const h3d_packed_conv* packed, float* y, int B, int H, int W, int stride,
+                         int leaky, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(x && packed && y && B > 0, "h3d_conv2d_tc_packed: bad argument");
+    return conv_tc_run(ctx, x, y, B, H, W, packed->Cin, packed->Cout, packed->k, stride, leaky, packed->precision, packed->pw.Cin_pad,
+                       packed->pw.Cout_pad, 0, [&](char*, PackedW* pw) { *pw = packed->pw; return (int)H3D_OK; }, s);
+}
+
+// Weight planes of a device-weight convolution in the operator scratch: [hi | lo | bias padded to Cout_pad]
+static int64_t dev_plane_bytes(int ksize, int Cin_pad, int Cout_pad) { return align_up((int64_t)Cout_pad * ksize * ksize * Cin_pad * 2, 1024); }
+
+int h3d_conv2d_tc_dev(h3d_ctx* ctx, const float* x, const float* w_hwio, const float* bias, float* y, int B, int H, int W, int Cin,
+                      int Cout, int ksize, int stride, int leaky, int precision, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(x && w_hwio && bias && y && B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0, "h3d_conv2d_tc_dev: bad argument");
+    H3D_REQUIRE(precision >= H3D_PREC_BF16X3 && precision <= H3D_PREC_BF16,
+                "h3d_conv2d_tc_dev: precision must be bf16x3, fp16x3, fp16 or bf16 (fp16_f8c derives its scales from host weights)");
+    H3D_REQUIRE(ksize == 1 || ksize == 3 || ksize == 5 || ksize == 7, "h3d_conv2d_tc_dev: ksize must be 1, 3, 5 or 7");
+    const int Cin_pad = (int)align_up(Cin, 64), Cout_pad = (int)align_up(Cout, 64);
+    const int64_t pb = dev_plane_bytes(ksize, Cin_pad, Cout_pad);
+    auto pack = [&](char* wbase, PackedW* pw) {
+        pw->w.hi = (uint16_t*)wbase;
+        if (passes_of(precision) == 3) pw->w.lo = (uint16_t*)(wbase + pb);
+        pw->bias = (float*)(wbase + 2 * pb);
+        pw->Cin_pad = Cin_pad; pw->Cout_pad = Cout_pad;
+        ctx->launches += 1;
+        return launch_pack_conv_w(w_hwio, bias, pw->w, pw->bias, ksize, Cin, Cout, Cin_pad, Cout_pad, false, half_of(precision), s);
+    };
+    return conv_tc_run(ctx, x, y, B, H, W, Cin, Cout, ksize, stride, leaky, precision, Cin_pad, Cout_pad, 2 * pb + align_up(Cout_pad * 4, 1024),
+                       pack, s);
+}
+
+int h3d_conv2d_tc_backward(h3d_ctx* ctx, const float* x, const float* y, const float* dy, const float* w_hwio, float* dx, float* dw_hwio,
+                           float* db, int B, int H, int W, int Cin, int Cout, int ksize, int stride, int leaky, int precision, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(dy && B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0, "h3d_conv2d_tc_backward: bad argument");
+    H3D_REQUIRE(precision == H3D_PREC_BF16X3 || precision == H3D_PREC_BF16,
+                "h3d_conv2d_tc_backward: precision must be bf16x3 or bf16 (fp16 planes have no range for small gradients without loss "
+                "scaling, fp16_f8c carries per-layer scale factors, fp32_ffma has no tensor-core backward)");
+    H3D_REQUIRE(ksize == 1 || ksize == 3 || ksize == 5 || ksize == 7, "h3d_conv2d_tc_backward: ksize must be 1, 3, 5 or 7");
+    H3D_REQUIRE(stride == 1 || (stride == 2 && H % 2 == 0 && W % 2 == 0 && ksize >= 3),
+                "h3d_conv2d_tc_backward: stride must be 1, or 2 with even H and W and ksize >= 3");
+    H3D_REQUIRE(Cout <= 1024, "h3d_conv2d_tc_backward: Cout must be <= 1024");
+    H3D_REQUIRE(!leaky || y, "h3d_conv2d_tc_backward: y (the forward output) is required with leaky");
+    H3D_REQUIRE(!dx || w_hwio, "h3d_conv2d_tc_backward: dx needs w_hwio");
+    H3D_REQUIRE(!dw_hwio || x, "h3d_conv2d_tc_backward: dw_hwio needs x");
+    if (!dx && !dw_hwio && !db) return H3D_OK;
+    const int passes = passes_of(precision);
+    const int Cin_pad = (int)align_up(Cin, 64), Cout_pad = (int)align_up(Cout, 64);
+    const int64_t rows = (int64_t)B * H * W;
+    int64_t ppb = 0;
+    const int nblk = conv_grad_prep_blocks(rows, &ppb);
+    // scratch: [dy' hi | dy' lo | x hi | x lo | W_d hi | W_d lo | zero bias | db partials | dW partials]
+    const int64_t gb = align_up(rows * Cout_pad * 2, 1024), xb = align_up(rows * Cin_pad * 2, 1024);
+    const int64_t wb = dev_plane_bytes(ksize, Cin_pad, Cout_pad), zb = align_up(Cin_pad * 4, 1024);
+    const int64_t dbb = align_up((int64_t)nblk * Cout_pad * 4, 1024);
+    const int64_t pwb = dw_hwio ? conv_wgrad_partial_floats(B, H, W, ksize, Cin_pad, Cout_pad) * 4 : 0;
+    char* base = nullptr;
+    int rc = op_scratch(ctx, 2 * gb + 2 * xb + 2 * wb + zb + dbb + pwb, &base);
+    if (rc) return rc;
+    char* const xbase = base + 2 * gb;
+    char* const wbase = xbase + 2 * xb;
+    float* const zbias = (float*)(wbase + 2 * wb);
+    float* const db_part = (float*)((char*)zbias + zb);
+    float* const wpart = (float*)((char*)db_part + dbb);
+    Split gs;
+    gs.hi = (uint16_t*)base;
+    if (passes == 3) gs.lo = (uint16_t*)(base + gb);
+    if ((rc = launch_conv_grad_prep(dy, leaky ? y : nullptr, gs, db ? db_part : nullptr, B, H, W, Cout, Cout_pad, stride, leaky, s))) return rc;
+    ctx->launches += 1;
+    if (db) {
+        if ((rc = launch_bias_grad_reduce(db_part, nblk, Cout, Cout_pad, db, s))) return rc;
+        ctx->launches += 1;
+    }
+    if (dx) {   // the stride-1 'SAME' convolution of dy' with the flipped, transposed kernel, on the forward kernel
+        Split wd;
+        wd.hi = (uint16_t*)wbase;
+        if (passes == 3) wd.lo = (uint16_t*)(wbase + wb);
+        if ((rc = launch_pack_conv_w(w_hwio, nullptr, wd, zbias, ksize, Cin, Cout, Cin_pad, Cout_pad, true, Half16::BF16, s))) return rc;
+        TcConvDesc d;
+        d.x = gs; d.Cin_total = Cout_pad; d.Cin_pad = Cout_pad; d.w = wd; d.bias = zbias; d.Cout = Cin; d.Cout_pad = Cin_pad;
+        d.y = Split(); d.Cy_total = 0; d.cy_off = 0; d.yf = dx; d.Cyf_total = Cin; d.cyf_off = 0;
+        d.B = B; d.H = H; d.W = W; d.k = ksize; d.leaky = 0; d.passes = passes; d.half = Half16::BF16; d.pool = 0;
+        d.err_flag = ctx->err_flag;
+        TcConvPlan* tp = tc_conv_plan_create(d);
+        if (!tp) return H3D_ECUDA;
+        rc = tc_conv_launch(tp, s);
+        tc_conv_plan_destroy(tp);
+        if (rc) return rc;
+        ctx->launches += 2;
+    }
+    if (dw_hwio) {
+        Split xs;
+        xs.hi = (uint16_t*)xbase;
+        if (passes == 3) xs.lo = (uint16_t*)(xbase + xb);
+        if ((rc = launch_f32_to_split(x, xs, rows, Cin, Cin_pad, Half16::BF16, s))) return rc;
+        WgradDesc d;
+        d.x = xs; d.dy = gs;
+        d.B = B; d.H = H; d.W = W; d.Cin = Cin; d.Cout = Cout; d.Cin_pad = Cin_pad; d.Cout_pad = Cout_pad; d.k = ksize; d.passes = passes;
+        d.partial = wpart; d.dw = dw_hwio; d.err_flag = ctx->err_flag;
+        if ((rc = launch_conv_wgrad(d, s))) return rc;
+        ctx->launches += 3;
+    }
     return H3D_OK;
 }
 
@@ -1433,6 +1542,13 @@ int h3d_conv2d_tc_strided(h3d_ctx* ctx, const float* x, const float* host_w_hwio
 int h3d_maxpool2x2_f32(h3d_ctx* ctx, const float* x, float* y, int B, int H, int W, int C, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     int rc = launch_maxpool_f32(x, y, B, H, W, C, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_maxpool2x2_backward_f32(h3d_ctx* ctx, const float* x, const float* dy, float* dx, int B, int H, int W, int C, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(x && dy && dx && B > 0 && H > 0 && W > 0 && C > 0, "h3d_maxpool2x2_backward_f32: bad argument");
+    int rc = launch_maxpool_backward_f32(x, dy, dx, B, H, W, C, s);
     if (!rc) ctx->launches += 1;
     return rc;
 }

@@ -89,6 +89,8 @@ struct LaunchCounter {
 // ---------------------------------------------------------------- kernels (elementwise.cu)
 int launch_resize_bilinear_tf1(const float* x, float* y, int B, int H, int W, int C, int oh, int ow, cudaStream_t s);
 int launch_maxpool_f32(const float* x, float* y, int B, int H, int W, int C, cudaStream_t s);
+// gradient of the 2x2 / 2 VALID max-pool: dy [B,H/2,W/2,C] -> dx [B,H,W,C], each window's gradient to its first maximum (row-major)
+int launch_maxpool_backward_f32(const float* x, const float* dy, float* dx, int B, int H, int W, int C, cudaStream_t s);
 int launch_maxpool_split(Split x, Split y, int B, int H, int W, int C, Half16 t, cudaStream_t s);
 int launch_avgpool8(const float* x, float* y, int B, int H, int W, int C, cudaStream_t s);
 int launch_f32_to_split(const float* x, Split y, int64_t rows, int C, int Cpad, Half16 t, cudaStream_t s);
@@ -237,5 +239,27 @@ int tc_conv_launch_image(const TcConvPlan* p, const float* image, cudaStream_t s
 bool tc_conv_can_fuse_first(int H, int W, int Cin, int Cout, int k, int passes, int pool);
 int64_t tc_conv_flops(const TcConvPlan* p);
 int tc_num_sms();
+
+// ---------------------------------------------------------------- kernels (conv_wgrad.cu): backward of the tensor-core convolution
+// HWIO fp32 device weights -> 16-bit hi (/ lo) planes: forward [Cout_pad][k][k][Cin_pad] (as pack_conv_weights) or, with dgrad, the
+// data-gradient operator [Cin_pad][k][k][Cout_pad] of the spatially flipped kernel; bias_pad [rows] = padded bias, or zeros with dgrad
+int launch_pack_conv_w(const float* w_hwio, const float* bias, Split out, float* bias_pad, int k, int Cin, int Cout, int Cin_pad,
+                       int Cout_pad, bool dgrad, Half16 half, cudaStream_t s);
+// dy' = dy * act'(y) (y may be null without leaky) as bf16 split planes [B,H,W,Cout_pad] at the input resolution (stride 2: odd pixels);
+// db_part (optional) [conv_grad_prep_blocks(B*H*W)][Cout_pad] per-block column sums for launch_bias_grad_reduce
+int conv_grad_prep_blocks(int64_t pixels, int64_t* pixels_per_block);
+int launch_conv_grad_prep(const float* dy, const float* y, Split out, float* db_part, int B, int H, int W, int Cout, int Cout_pad,
+                          int stride, int leaky, cudaStream_t s);
+int launch_bias_grad_reduce(const float* db_part, int nblk, int Cout, int Cout_pad, float* db, cudaStream_t s);
+struct WgradDesc {
+    Split x;        // input activations, split planes [B,H,W,Cin_pad]
+    Split dy;       // dy' split planes [B,H,W,Cout_pad] (launch_conv_grad_prep)
+    int B, H, W, Cin, Cout, Cin_pad, Cout_pad, k, passes;
+    float* partial;  // conv_wgrad_partial_floats(...) floats of scratch
+    float* dw;       // HWIO [k,k,Cin,Cout] fp32
+    int* err_flag;
+};
+int64_t conv_wgrad_partial_floats(int B, int H, int W, int k, int Cin_pad, int Cout_pad);
+int launch_conv_wgrad(const WgradDesc& d, cudaStream_t s);
 
 }  // namespace h3d

@@ -132,6 +132,41 @@ int launch_maxpool_f32(const float* x, float* y, int B, int H, int W, int C, cud
     return H3D_OK;
 }
 
+// Gradient of NetworkOps.max_pool: one thread per (window, channel) writes the window's four dx values; the gradient goes to the first
+// maximum in row-major window order (TF's CPU MaxPoolGrad).  Odd trailing rows / columns (dropped by VALID) are zeroed by the launcher.
+__global__ void maxpool_backward_f32_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ dx, int B, int H,
+                                            int W, int C) {
+    const int Ho = H >> 1, Wo = W >> 1;
+    const int64_t total = (int64_t)B * Ho * Wo * C;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int c = (int)(i % C);
+        const int ox = (int)((i / C) % Wo);
+        const int oy = (int)((i / ((int64_t)C * Wo)) % Ho);
+        const int b = (int)(i / ((int64_t)C * Wo * Ho));
+        const int64_t base = (((int64_t)b * H + 2 * oy) * W + 2 * ox) * C + c;
+        const int64_t offs[4] = {0, C, (int64_t)W * C, (int64_t)W * C + C};
+        int arg = 0;
+        float best = __ldg(x + base);
+#pragma unroll
+        for (int q = 1; q < 4; ++q) {
+            const float v = __ldg(x + base + offs[q]);
+            if (v > best) { best = v; arg = q; }
+        }
+        const float g = __ldg(dy + i);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) dx[base + offs[q]] = q == arg ? g : 0.f;
+    }
+}
+
+int launch_maxpool_backward_f32(const float* x, const float* dy, float* dx, int B, int H, int W, int C, cudaStream_t s) {
+    if ((H | W) & 1) H3D_CUDA(cudaMemsetAsync(dx, 0, (size_t)B * H * W * C * sizeof(float), s));
+    const int64_t total = (int64_t)B * (H / 2) * (W / 2) * C;
+    if (total == 0) return H3D_OK;
+    maxpool_backward_f32_kernel<<<(int)std::min<int64_t>(ceil_div64(total, 256), 132 * 32), 256, 0, s>>>(x, dy, dx, B, H, W, C);
+    H3D_CHECK_LAUNCH();
+    return H3D_OK;
+}
+
 template <bool FP16>
 __device__ __forceinline__ float h16_to_f32(uint16_t v) {
     if (FP16) return __half2float(__ushort_as_half(v));

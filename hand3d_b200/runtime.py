@@ -277,6 +277,42 @@ class Context:
                    "h3d_conv2d_tc_packed")
         return y
 
+    def conv2d_tc_dev(self, x, w, b, stride=1, leaky=False, precision="bf16x3"):
+        """Tensor-core convolution with DEVICE weights (w HWIO [k,k,Cin,Cout], b [Cout]): packed on the GPU every call, enqueue-only;
+        bit-identical to pack_conv + conv2d_tc_packed for the same weights."""
+        x = _chk_f32(x, "x", 4); w = _chk_f32(w, "w", 4); b = _chk_f32(b, "b", 1)
+        B, H, W, Cin = x.shape
+        k, _, wc, Cout = w.shape
+        if wc != Cin or b.shape[0] != Cout:
+            raise ValueError("conv2d_tc_dev: x %s, w %s and b %s do not match" % (tuple(x.shape), tuple(w.shape), tuple(b.shape)))
+        y = torch.empty((B, H // stride, W // stride, Cout), dtype=torch.float32, device=x.device)
+        _lib.check(self.lib.h3d_conv2d_tc_dev(self.h, _ptr(x), _ptr(w), _ptr(b), _ptr(y), B, H, W, Cin, Cout, k, stride, int(leaky),
+                                              PRECISIONS[precision], _stream()), "h3d_conv2d_tc_dev")
+        return y
+
+    def conv2d_tc_backward(self, x, y, dy, w, stride=1, leaky=False, precision="bf16x3", need_dx=True, need_dw=True, need_db=True):
+        """Gradients (dx, dw, db) of y = act(conv_SAME(x, w, stride) + b); outputs not needed come back as None.  y (the forward
+        output) is read only with leaky, x only for dw, w only for dx."""
+        dy = _chk_f32(dy, "dy", 4)
+        w = _chk_f32(w, "w", 4)
+        k, _, Cin, Cout = w.shape
+        B, Ho, Wo, _ = dy.shape
+        H, W = Ho * stride, Wo * stride
+        if need_dw:
+            x = _chk_f32(x, "x", 4)
+            if tuple(x.shape) != (B, H, W, Cin):
+                raise ValueError("conv2d_tc_backward: x %s does not match dy %s / w %s" % (tuple(x.shape), tuple(dy.shape), tuple(w.shape)))
+        if leaky:
+            y = _chk_f32(y, "y", 4)
+        f32 = dict(dtype=torch.float32, device=dy.device)
+        dx = torch.empty((B, H, W, Cin), **f32) if need_dx else None
+        dw = torch.empty((k, k, Cin, Cout), **f32) if need_dw else None
+        db = torch.empty((Cout,), **f32) if need_db else None
+        _lib.check(self.lib.h3d_conv2d_tc_backward(
+            self.h, _ptr(x if need_dw else None), _ptr(y if leaky else None), _ptr(dy), _ptr(w if need_dx else None), _ptr(dx), _ptr(dw),
+            _ptr(db), B, H, W, Cin, Cout, k, stride, int(leaky), PRECISIONS[precision], _stream()), "h3d_conv2d_tc_backward")
+        return dx, dw, db
+
     def leaky_relu(self, x):
         x = _chk_f32(x, "x")
         y = torch.empty_like(x)
@@ -316,6 +352,17 @@ class Context:
         y = torch.empty((B, H // 2, W // 2, Cc), dtype=torch.float32, device=x.device)
         _lib.check(self.lib.h3d_maxpool2x2_f32(self.h, _ptr(x), _ptr(y), B, H, W, Cc, _stream()), "h3d_maxpool2x2_f32")
         return y
+
+    def max_pool_backward(self, x, dy):
+        """Gradient of max_pool: x [B,H,W,C] (forward input), dy [B,H/2,W/2,C] -> dx [B,H,W,C] (first maximum of each window)."""
+        x = _chk_f32(x, "x", 4); dy = _chk_f32(dy, "dy", 4)
+        B, H, W, Cc = x.shape
+        if tuple(dy.shape) != (B, H // 2, W // 2, Cc):
+            raise ValueError("max_pool_backward: dy %s does not match x %s" % (tuple(dy.shape), tuple(x.shape)))
+        dx = torch.empty_like(x)
+        _lib.check(self.lib.h3d_maxpool2x2_backward_f32(self.h, _ptr(x), _ptr(dy), _ptr(dx), B, H, W, Cc, _stream()),
+                   "h3d_maxpool2x2_backward_f32")
+        return dx
 
     def fully_connected(self, x, w, b, leaky=False):
         x = _chk_f32(x, "x", 2); w = _chk_f32(w, "w", 2); b = _chk_f32(b, "b", 1)

@@ -166,10 +166,28 @@ H3D_API int h3d_free_packed_conv(h3d_ctx* ctx, h3d_packed_conv* packed);
  * operator scratch (no allocation, no synchronisation). */
 H3D_API int h3d_conv2d_tc_packed(h3d_ctx* ctx, const float* x, const h3d_packed_conv* packed, float* y, int B, int H, int W,
                                  int stride, int leaky, void* stream);
+/* The same forward with DEVICE weights (w_hwio [k,k,Cin,Cout], bias [Cout]), for weights that change every optimiser step: a kernel
+ * packs them into the context's operator scratch, so the call only enqueues work.  Bit-identical to h3d_pack_conv_weights +
+ * h3d_conv2d_tc_packed for the same weights.  precision: bf16x3, fp16x3, fp16 or bf16. */
+H3D_API int h3d_conv2d_tc_dev(h3d_ctx* ctx, const float* x, const float* w_hwio, const float* bias, float* y, int B, int H, int W,
+                              int Cin, int Cout, int ksize, int stride, int leaky, int precision, void* stream);
+/* Gradients of y = act(conv_SAME(x, w, stride) + b) (act: identity, or leaky ReLU 0.01 when leaky), the TF Conv2DBackpropInput,
+ * Conv2DBackpropFilter, BiasAddGrad and Maximum gradients that AdamOptimizer.minimize evaluates (training_posenet.py:67,
+ * training_handsegnet.py).  x [B,H,W,Cin], y and dy [B,H/stride,W/stride,Cout], w_hwio [k,k,Cin,Cout], all fp32 device tensors;
+ * outputs dx [B,H,W,Cin], dw_hwio [k,k,Cin,Cout], db [Cout], each may be NULL to skip it (a first layer needs no dx).  y is required
+ * with leaky (the slope is chosen where y >= 0, as TF's Maximum gradient does), x with dw_hwio, w_hwio with dx.  Same geometry as
+ * h3d_conv2d_tc_strided, Cout <= 1024; precision bf16x3 (fp32 parity) or bf16, the fp16 modes return H3D_EINVAL.  Enqueue-only
+ * (operator scratch), deterministic bit for bit; capturable into a CUDA graph once a first call has sized the scratch. */
+H3D_API int h3d_conv2d_tc_backward(h3d_ctx* ctx, const float* x, const float* y, const float* dy, const float* w_hwio, float* dx,
+                                   float* dw_hwio, float* db, int B, int H, int W, int Cin, int Cout, int ksize, int stride, int leaky,
+                                   int precision, void* stream);
 /* NetworkOps.leaky_relu (utils/general.py:31-33): y = max(x, 0.01 x), n elements, 16-byte aligned pointers. */
 H3D_API int h3d_leaky_relu_f32(h3d_ctx* ctx, const float* x, float* y, int64_t n, void* stream);
 /* NetworkOps.max_pool (utils/general.py:62-65): 2x2 / 2 VALID. */
 H3D_API int h3d_maxpool2x2_f32(h3d_ctx* ctx, const float* x, float* y, int B, int H, int W, int C, void* stream);
+/* Gradient of NetworkOps.max_pool (TF MaxPoolGrad under AdamOptimizer.minimize, training_posenet.py:67): x [B,H,W,C] (the forward
+ * input), dy [B,H/2,W/2,C] -> dx [B,H,W,C]; each window's gradient goes to its first maximum in row-major order, as TF's CPU kernel. */
+H3D_API int h3d_maxpool2x2_backward_f32(h3d_ctx* ctx, const float* x, const float* dy, float* dx, int B, int H, int W, int C, void* stream);
 /* NetworkOps.fully_connected(_relu) (utils/general.py:113-136): y = x[B,in] @ w[in,out] + b. */
 H3D_API int h3d_fully_connected_f32(h3d_ctx* ctx, const float* x, const float* w, const float* bias, float* y,
                             int B, int in_features, int out_features, int leaky, void* stream);
