@@ -86,7 +86,8 @@ static const std::map<std::string, VarShape>& known_vars() {
 
 // ------------------------------------------------------------------------------------------ context
 struct HostTensor { std::vector<float> data; std::vector<int64_t> shape; };
-struct PackedW { Split w; float* bias = nullptr; int Cin_pad = 0, Cout_pad = 0; float corr_scale = 0.f; };
+// w_scale: fp16 planes with passes 1 / 3, the per-channel shift factors 2^-s (split_fmt.cuh), stored after the padded bias
+struct PackedW { Split w; float* bias = nullptr; float* w_scale = nullptr; int Cin_pad = 0, Cout_pad = 0; float corr_scale = 0.f; };
 
 struct Arena {   // bump allocator over the caller-owned workspace (base == nullptr -> size query)
     char* base = nullptr; int64_t off = 0;
@@ -207,11 +208,12 @@ static float host_f32(uint16_t b, Half16 t) {
 }
 
 // Pack HWIO fp32 -> K-major [Cout_pad][kh][kw][Cin_pad] hi/lo planes.  perm[j] = source input channel of
-// packed channel j (or -1 for zero padding); empty perm = identity.
+// packed channel j (or -1 for zero padding); empty perm = identity.  fp16 planes (passes 1 / 3) carry the per-channel weight shift
+// of split_fmt.cuh; its factors 2^-s follow the padded bias in the same allocation ([bias | w_scale], 2 Cout_pad floats).
 static int pack_conv_weights(const float* w, const float* bias, int k, int Cin, int Cout, int Cin_pad, int Cout_pad,
                              const std::vector<int>& perm, Half16 t, int passes, PackedW* out) {
     const int64_t Ktot = (int64_t)k * k * Cin_pad;
-    const bool want_lo = passes == 3, f8c = passes == 4;
+    const bool want_lo = passes == 3, f8c = passes == 4, shifted = t == Half16::FP16 && !f8c;
     std::vector<uint16_t> hi((size_t)Cout_pad * Ktot, 0), lo;
     std::vector<uint8_t> h8, l8;
     if (want_lo) lo.assign((size_t)Cout_pad * Ktot, 0);
@@ -226,6 +228,13 @@ static int pack_conv_weights(const float* w, const float* bias, int k, int Cin, 
         h8.assign((size_t)Cout_pad * Ktot, 0); l8.assign((size_t)Cout_pad * Ktot, 0);
         out->corr_scale = std::ldexp(1.0f, -(kF8XLoShift + b));
     }
+    std::vector<int> sh((size_t)Cout_pad, 0);
+    if (shifted)
+        for (int co = 0; co < Cout; ++co) {
+            float mx = 0.f;
+            for (int64_t r = 0; r < (int64_t)k * k * Cin; ++r) mx = std::max(mx, std::fabs(w[r * Cout + co]));
+            sh[co] = fp16_w_shift(mx);
+        }
     for (int co = 0; co < Cout; ++co)
         for (int tap = 0; tap < k * k; ++tap)
             for (int cj = 0; cj < Cin_pad; ++cj) {
@@ -240,12 +249,15 @@ static int pack_conv_weights(const float* w, const float* bias, int k, int Cin, 
                     l8[idx] = f32_to_e4m3(std::ldexp(v - std::ldexp(host_f32(h, t), -(kF8XMainShift + b)), 12 + b));
                     continue;
                 }
-                const uint16_t h = host_h16(v, t);
+                const float vs = std::ldexp(v, sh[co]);
+                const uint16_t h = host_h16(vs, t);
                 hi[idx] = h;
-                if (want_lo) lo[idx] = host_h16(v - host_f32(h, t), t);
+                if (want_lo) lo[idx] = host_h16(vs - host_f32(h, t), t);
             }
     std::vector<float> bv((size_t)Cout_pad, 0.f);
     for (int co = 0; co < Cout; ++co) bv[co] = bias[co];
+    if (shifted)
+        for (int co = 0; co < Cout_pad; ++co) bv.push_back(std::ldexp(1.0f, -sh[co]));
     H3D_CUDA(cudaMalloc(&out->w.hi, hi.size() * 2));
     H3D_CUDA(cudaMemcpy(out->w.hi, hi.data(), hi.size() * 2, cudaMemcpyHostToDevice));
     if (want_lo) {
@@ -259,6 +271,7 @@ static int pack_conv_weights(const float* w, const float* bias, int k, int Cin, 
     }
     H3D_CUDA(cudaMalloc(&out->bias, bv.size() * 4));
     H3D_CUDA(cudaMemcpy(out->bias, bv.data(), bv.size() * 4, cudaMemcpyHostToDevice));
+    if (shifted) out->w_scale = out->bias + Cout_pad;
     out->Cin_pad = Cin_pad; out->Cout_pad = Cout_pad;
     return H3D_OK;
 }
@@ -446,7 +459,8 @@ static int add_tc(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, const L
     int rc = get_packed(ctx, scope, l, Cin_pad, perm, &pw, force_passes);
     if (rc) return rc;
     TcConvDesc d;
-    d.x = x; d.Cin_total = Cin_total; d.Cin_pad = Cin_pad; d.w = pw->w; d.bias = pw->bias; d.Cout = l.cout; d.Cout_pad = pw->Cout_pad;
+    d.x = x; d.Cin_total = Cin_total; d.Cin_pad = Cin_pad; d.w = pw->w; d.bias = pw->bias; d.w_scale = pw->w_scale; d.Cout = l.cout;
+    d.Cout_pad = pw->Cout_pad;
     d.y = y; d.Cy_total = Cy_total; d.cy_off = cy_off; d.yf = yf; d.Cyf_total = Cyf_total; d.cyf_off = cyf_off;
     d.B = B; d.H = H; d.W = W; d.k = l.k; d.leaky = l.leaky; d.passes = force_passes ? force_passes : passes_of(ctx->precision);
     d.half = half_of(ctx->precision);
@@ -789,7 +803,7 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
             if (rc2) return rc2;
             FcLayerDesc& d = cd.layer[cd.num_layers++];
             d.x = x.s; d.x_stride = x.stride; d.in_features = in_f;
-            d.w = pw->w; d.bias = pw->bias; d.out_features = out_f; d.out_pad = pw->Cout_pad;
+            d.w = pw->w; d.bias = pw->bias; d.w_scale = pw->w_scale; d.out_features = out_f; d.out_pad = pw->Cout_pad;
             d.y = y ? y->s : Split(); d.y_stride = y ? y->stride : 0; d.yf = yf; d.yf_stride = yf_stride; d.leaky = leaky;
             fl += 2ll * B * in_f * out_f;
             return H3D_OK;
@@ -1401,7 +1415,8 @@ static int conv_tc_run(h3d_ctx* ctx, const float* x, float* y, int B, int H, int
     }
     if ((rc = launch_f32_to_split(x, xs, rows, Cin, Cin_pad, half, s))) return rc;
     TcConvDesc d;
-    d.x = xs; d.Cin_total = Cin_pad; d.Cin_pad = Cin_pad; d.w = pw.w; d.bias = pw.bias; d.Cout = Cout; d.Cout_pad = Cout_pad;
+    d.x = xs; d.Cin_total = Cin_pad; d.Cin_pad = Cin_pad; d.w = pw.w; d.bias = pw.bias; d.w_scale = pw.w_scale; d.Cout = Cout;
+    d.Cout_pad = Cout_pad;
     d.y = ys; d.Cy_total = Cout_pad; d.cy_off = 0; d.yf = nullptr; d.Cyf_total = 0; d.cyf_off = 0;
     d.B = B; d.H = H; d.W = W; d.k = ksize; d.leaky = leaky; d.passes = passes; d.half = half; d.corr_scale = pw.corr_scale;
     d.pool = stride == 2 ? 2 : 0;
@@ -1425,7 +1440,7 @@ int h3d_conv2d_tc_packed(h3d_ctx* ctx, const float* x, const h3d_packed_conv* pa
                        packed->pw.Cout_pad, 0, [&](char*, PackedW* pw) { *pw = packed->pw; return (int)H3D_OK; }, s);
 }
 
-// Weight planes of a device-weight convolution in the operator scratch: [hi | lo | bias padded to Cout_pad]
+// Weight planes of a device-weight convolution in the operator scratch: [hi | lo | bias padded to Cout_pad | fp16: w_scale [Cout_pad]]
 static int64_t dev_plane_bytes(int ksize, int Cin_pad, int Cout_pad) { return align_up((int64_t)Cout_pad * ksize * ksize * Cin_pad * 2, 1024); }
 
 int h3d_conv2d_tc_dev(h3d_ctx* ctx, const float* x, const float* w_hwio, const float* bias, float* y, int B, int H, int W, int Cin,
@@ -1441,11 +1456,12 @@ int h3d_conv2d_tc_dev(h3d_ctx* ctx, const float* x, const float* w_hwio, const f
         pw->w.hi = (uint16_t*)wbase;
         if (passes_of(precision) == 3) pw->w.lo = (uint16_t*)(wbase + pb);
         pw->bias = (float*)(wbase + 2 * pb);
+        if (half_of(precision) == Half16::FP16) pw->w_scale = pw->bias + Cout_pad;
         pw->Cin_pad = Cin_pad; pw->Cout_pad = Cout_pad;
-        ctx->launches += 1;
-        return launch_pack_conv_w(w_hwio, bias, pw->w, pw->bias, ksize, Cin, Cout, Cin_pad, Cout_pad, false, half_of(precision), s);
+        ctx->launches += pw->w_scale ? 2 : 1;
+        return launch_pack_conv_w(w_hwio, bias, pw->w, pw->bias, pw->w_scale, ksize, Cin, Cout, Cin_pad, Cout_pad, false, half_of(precision), s);
     };
-    return conv_tc_run(ctx, x, y, B, H, W, Cin, Cout, ksize, stride, leaky, precision, Cin_pad, Cout_pad, 2 * pb + align_up(Cout_pad * 4, 1024),
+    return conv_tc_run(ctx, x, y, B, H, W, Cin, Cout, ksize, stride, leaky, precision, Cin_pad, Cout_pad, 2 * pb + align_up(Cout_pad * 8, 1024),
                        pack, s);
 }
 
@@ -1495,7 +1511,7 @@ int h3d_conv2d_tc_backward(h3d_ctx* ctx, const float* x, const float* y, const f
         Split wd;
         wd.hi = (uint16_t*)wbase;
         if (passes == 3) wd.lo = (uint16_t*)(wbase + wb);
-        if ((rc = launch_pack_conv_w(w_hwio, nullptr, wd, zbias, ksize, Cin, Cout, Cin_pad, Cout_pad, true, Half16::BF16, s))) return rc;
+        if ((rc = launch_pack_conv_w(w_hwio, nullptr, wd, zbias, nullptr, ksize, Cin, Cout, Cin_pad, Cout_pad, true, Half16::BF16, s))) return rc;
         TcConvDesc d;
         d.x = gs; d.Cin_total = Cout_pad; d.Cin_pad = Cout_pad; d.w = wd; d.bias = zbias; d.Cout = Cin; d.Cout_pad = Cin_pad;
         d.y = Split(); d.Cy_total = 0; d.cy_off = 0; d.yf = dx; d.Cyf_total = Cin; d.cyf_off = 0;

@@ -174,6 +174,7 @@ struct TcConvDesc {
     // packed weights: [Cout_pad][k*k*Cin_pad] K-major 16-bit planes
     Split w;
     const float* bias;  // [Cout_pad] fp32
+    const float* w_scale = nullptr;   // fp16 planes with passes 1 / 3: [Cout_pad] 2^-s un-doing the per-channel weight shift (split_fmt.cuh)
     int Cout, Cout_pad;
     // outputs: split planes at channel offset (16-byte aligned) and/or fp32
     Split y;
@@ -216,6 +217,7 @@ int tc_set_tuning(const char* key, int value);
 struct FcLayerDesc {
     Split x; int x_stride, in_features;      // input planes [B, x_stride], K = in_features rounded up to 64
     Split w; const float* bias; int out_features, out_pad;   // packed weights [out_pad][K] (pack_conv_weights with k = 1)
+    const float* w_scale = nullptr;           // fp16 planes: per-output shifts (TcConvDesc::w_scale)
     Split y; int y_stride;                    // output planes (hidden layers) ...
     float* yf; int yf_stride;                 // ... or fp32 output (last layer)
     int leaky;
@@ -242,9 +244,10 @@ int tc_num_sms();
 
 // ---------------------------------------------------------------- kernels (conv_wgrad.cu): backward of the tensor-core convolution
 // HWIO fp32 device weights -> 16-bit hi (/ lo) planes: forward [Cout_pad][k][k][Cin_pad] (as pack_conv_weights) or, with dgrad, the
-// data-gradient operator [Cin_pad][k][k][Cout_pad] of the spatially flipped kernel; bias_pad [rows] = padded bias, or zeros with dgrad
-int launch_pack_conv_w(const float* w_hwio, const float* bias, Split out, float* bias_pad, int k, int Cin, int Cout, int Cin_pad,
-                       int Cout_pad, bool dgrad, Half16 half, cudaStream_t s);
+// data-gradient operator [Cin_pad][k][k][Cout_pad] of the spatially flipped kernel; bias_pad [rows] = padded bias, or zeros with dgrad.
+// w_scale [Cout_pad] (forward fp16 planes, else nullptr): the per-channel shift factors 2^-s of split_fmt.cuh, as the host packer
+int launch_pack_conv_w(const float* w_hwio, const float* bias, Split out, float* bias_pad, float* w_scale, int k, int Cin, int Cout,
+                       int Cin_pad, int Cout_pad, bool dgrad, Half16 half, cudaStream_t s);
 // dy' = dy * act'(y) (y may be null without leaky) as bf16 split planes [B,H,W,Cout_pad] at the input resolution (stride 2: odd pixels);
 // db_part (optional) [conv_grad_prep_blocks(B*H*W)][Cout_pad] per-block column sums for launch_bias_grad_reduce
 int conv_grad_prep_blocks(int64_t pixels, int64_t* pixels_per_block);

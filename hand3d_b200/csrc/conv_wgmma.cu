@@ -11,8 +11,12 @@
 // * B tiles are 2-D TMA boxes {64, BN} of the pre-packed K-major weights [Cout][kh][kw][Cin].
 // * fp32 parity on 16-bit tensor cores: activations and weights are stored as two 16-bit planes
 //   x = hi + lo; each K block issues hi*hi + hi*lo + lo*hi (3 passes) into the same fp32 register
-//   accumulator (dropped lo*lo term ~2^-18 relative for bf16, ~2^-24 for fp16).  PASSES == 1 is the
-//   plain 16-bit path; PASSES == 4 is one fp16 pass plus two e4m3 correction passes (split_fmt.cuh).
+//   accumulator.  Per operand the split keeps 16 (bf16) or 22 (fp16) significant bits, so the dropped lo*lo term is ~2^-16
+//   (bf16) or ~2^-22 (fp16) of a product -- as long as lo stays a normal number.  bf16 has fp32's exponent range; fp16's
+//   ends at 2^-14, so fp16 weight planes are packed with a per-output-channel power-of-two shift that the epilogue un-does
+//   (split_fmt.cuh), and fp16 activations keep the full split only for |x| >= ~2^-3 (below, lo is subnormal and the error
+//   grows towards single-pass fp16's; DESIGN.md section 6.1 gives the measured ranges).  PASSES == 1 is the plain 16-bit
+//   path; PASSES == 4 is one fp16 pass plus two e4m3 correction passes (split_fmt.cuh).
 // * Warp-specialised persistent CTAs of three warpgroups: warpgroup 0 is the TMA producer (one elected lane of
 //   its first warp issues), warpgroups 1 and 2 each own 64 rows of the 128-pixel tile and issue wgmma.mma_async
 //   on them.  A ring of shared-memory stages with full / empty mbarriers decouples the two sides.
@@ -68,13 +72,16 @@ struct TcParams {
     int chunk_kb;   // K blocks accumulated inside the tensor core before the partial sum is folded into the fp32 registers
     int leaky;
     int* err_flag;
+    const float* w_scale;   // fp16 weight planes (PASSES 1 / 3): [Cout_pad] 2^-s per output channel (split_fmt.cuh)
 };
 
-// bias + leaky ReLU + store of 32 consecutive output channels [n, n+32) of one pixel (fp32 and / or hi-lo split planes)
+// bias + leaky ReLU + store of 32 consecutive output channels [n, n+32) of one pixel (fp32 and / or hi-lo split planes).
+// w_scale (fp16 weight planes): [n, n+32) per-channel factors 2^-s that un-do the weight shift, in global memory (read through the
+// read-only path, as the bias) or, with SMEM_SCALE, in shared memory.
 // With p.pool the 2x2 max-pool partners of a pixel are lanes (lane ^ 1) and (lane ^ TW) of the same warp (tile rows are
 // ordered w-fastest and TW <= 16), so pooling is two warp shuffles per value; the lane with even (w, h) stores.
-template <int PASSES, bool FP16>
-__device__ __forceinline__ void epilogue_store32(const TcParams& p, const float* a, int64_t pix, int n, bool valid) {
+template <int PASSES, bool FP16, bool SMEM_SCALE = false>
+__device__ __forceinline__ void epilogue_store32(const TcParams& p, const float* a, int64_t pix, int n, bool valid, const float* w_scale) {
     float f[32];
     const float4* bp = reinterpret_cast<const float4*>(p.bias + n);
 #pragma unroll
@@ -85,6 +92,12 @@ __device__ __forceinline__ void epilogue_store32(const TcParams& p, const float*
             f[4 * q + 1] = fmaf(a[4 * q + 1], p.corr_scale, bv.y);
             f[4 * q + 2] = fmaf(a[4 * q + 2], p.corr_scale, bv.z);
             f[4 * q + 3] = fmaf(a[4 * q + 3], p.corr_scale, bv.w);
+        } else if (FP16) {   // un-do the per-channel weight shift (exact power of two)
+            const float4 sv = SMEM_SCALE ? reinterpret_cast<const float4*>(w_scale + n)[q] : __ldg(reinterpret_cast<const float4*>(w_scale + n) + q);
+            f[4 * q + 0] = fmaf(a[4 * q + 0], sv.x, bv.x);
+            f[4 * q + 1] = fmaf(a[4 * q + 1], sv.y, bv.y);
+            f[4 * q + 2] = fmaf(a[4 * q + 2], sv.z, bv.z);
+            f[4 * q + 3] = fmaf(a[4 * q + 3], sv.w, bv.w);
         } else {
             f[4 * q + 0] = a[4 * q + 0] + bv.x;
             f[4 * q + 1] = a[4 * q + 1] + bv.y;
@@ -293,8 +306,9 @@ __device__ __forceinline__ void mma_tile(Ring& r, int kblocks, int chunk_kb, flo
 // Epilogue of one tile: the two warpgroups' fragments go through the staging buffer (64 channels per round); consumer thread ct
 // (0..255) then owns tile row ct % 128 and channels [32 (ct / 128), +32) of the round, so the 2x2 pooling partners of a pixel are
 // lanes of one warp as epilogue_store32 requires.  pix_of(row, &pix, &valid) maps a tile row to its output pixel.
-template <int BN, int PASSES, bool FP16, class PixOf>
-__device__ __forceinline__ void store_tile(const TcParams& p, const float* racc, float* stg, int ct, int n0, PixOf pix_of) {
+template <int BN, int PASSES, bool FP16, class PixOf, bool SMEM_SCALE = false>
+__device__ __forceinline__ void store_tile(const TcParams& p, const float* racc, float* stg, int ct, int n0, PixOf pix_of,
+                                           const float* w_scale) {
     const int wg = ct >> 7, tt = ct & 127;
     const int r0 = wg * 64 + (tt >> 5) * 16 + ((tt & 31) >> 2);
     const int cq = 2 * (tt & 3);
@@ -316,7 +330,7 @@ __device__ __forceinline__ void store_tile(const TcParams& p, const float* racc,
         float f[32];
 #pragma unroll
         for (int q = 0; q < 32; ++q) f[q] = stg[row * STG_PITCH + half * 32 + q];
-        epilogue_store32<PASSES, FP16>(p, f, pix, n0 + rnd * STG_COLS + half * 32, valid);
+        epilogue_store32<PASSES, FP16, SMEM_SCALE>(p, f, pix, n0 + rnd * STG_COLS + half * 32, valid, w_scale);
     }
 }
 
@@ -396,7 +410,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_consta
                     valid = valid && ((w & 1) == par) && ((h & 1) == par);
                     pix = ((int64_t)b * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1);
                 }
-            });
+            }, p.w_scale);
         }
     }
 }
@@ -406,14 +420,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_consta
 // operand is BUILT in shared memory: the CTA stages the 18 x 10 x 3 input patch of a 16 x 8 pixel tile, then each of 128 threads
 // writes the 27 neighbourhood values of "its" pixel (+ 5 zeros) as hi / lo 16-bit rows in the K-major SWIZZLE_128B layout (rows
 // keep the 128-byte pitch of the other kernels, only the first 64 bytes = 32 K values are read).  The 64 x 27 weights are
-// converted and stored the same way once per CTA ([W_hi ; W_lo]: 128 rows).  Per tile each warpgroup runs 2 K steps x 3 passes of
+// converted and stored the same way once per CTA ([W_hi ; W_lo]: 128 rows); fp16 weights with the per-channel shift of
+// split_fmt.cuh, whose factors 2^-s the CTA keeps in shared memory for the epilogue.  Per tile each warpgroup runs 2 K steps x 3 passes of
 // wgmma (64 pixels x 64 channels) and the shared epilogue.  Two CTAs per SM overlap one CTA's build with the other's stores.
 constexpr int C3_TW = 16, C3_TH = 8;
 constexpr int C3T_THREADS = 256;
 constexpr int C3T_B_BYTES = 128 * BK * 2;
 constexpr int C3T_PW = C3_TW + 2, C3T_PH = C3_TH + 2;
 constexpr int C3T_PATCH_FLOATS = C3T_PH * C3T_PW * 3;   // 540
-constexpr int C3T_SMEM = C3T_B_BYTES + 2 * A_TILE_BYTES + STG_BYTES + C3T_PATCH_FLOATS * 4 + 1024 /*align*/;
+constexpr int C3T_SMEM = C3T_B_BYTES + 2 * A_TILE_BYTES + STG_BYTES + C3T_PATCH_FLOATS * 4 + 64 * 4 + 1024 /*align*/;
 
 template <bool FP16>
 __global__ void __launch_bounds__(C3T_THREADS, 2)
@@ -424,16 +439,25 @@ conv_c3_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, cons
     uint8_t* asm_ = smem + C3T_B_BYTES;                    // A_hi | A_lo, 128 rows x 128 B each
     float* stg = reinterpret_cast<float*>(asm_ + 2 * A_TILE_BYTES);
     float* patch = stg + BM * STG_PITCH;                   // [PH][PW][3]
+    float* w_scale = patch + C3T_PATCH_FLOATS;             // [64] fp16 weight shifts 2^-s (16-byte aligned)
 
     const int t = threadIdx.x, wg = t >> 7;
     if (t < 128) {   // weights: row n = output channel (t < 64: hi plane, t >= 64: lo plane of channel t - 64), k = (kh*3 + kw)*3 + ci
         const int co = t & 63;
+        int sh = 0;
+        if (FP16) {
+            float mx = 0.f;
+            for (int k = 0; k < 27; ++k) mx = fmaxf(mx, fabsf(__ldg(w + k * 64 + co)));
+            sh = fp16_w_shift(mx);
+            if (t < 64) w_scale[co] = ldexpf(1.f, -sh);
+        }
         uint32_t pk[16];
 #pragma unroll
         for (int k2 = 0; k2 < 16; ++k2) {
             float v0 = 0.f, v1 = 0.f;
             if (2 * k2 < 27) v0 = __ldg(w + (2 * k2) * 64 + co);
             if (2 * k2 + 1 < 27) v1 = __ldg(w + (2 * k2 + 1) * 64 + co);
+            if (FP16) { v0 = ldexpf(v0, sh); v1 = ldexpf(v1, sh); }
             const uint32_t h = pack_hi2<FP16>(v0, v1);
             if (t < 64) pk[k2] = h;
             else { const float2 r = unpack2<FP16>(h); pk[k2] = pack_hi2<FP16>(v0 - r.x, v1 - r.y); }
@@ -502,8 +526,8 @@ conv_c3_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, cons
             valid = (wx < p.W) && (hy < p.H);
             pix = ((int64_t)b * p.H + hy) * p.W + wx;
         };
-        if (p.y_lo) store_tile<64, 3, FP16>(p, acc, stg, t, 0, pix_of);
-        else store_tile<64, 1, FP16>(p, acc, stg, t, 0, pix_of);
+        if (p.y_lo) store_tile<64, 3, FP16, decltype(pix_of), true>(p, acc, stg, t, 0, pix_of, w_scale);
+        else store_tile<64, 1, FP16, decltype(pix_of), true>(p, acc, stg, t, 0, pix_of, w_scale);
     }
 }
 
@@ -593,7 +617,7 @@ fc_chain_kernel(const __grid_constant__ FcChainParams P) {
                 store_tile<BN, PASSES, FP16>(L.p, racc, stg, ct, nt * BN, [&](int row, int64_t& pix, bool& valid) {
                     pix = (int64_t)mt * BM + row;
                     valid = pix < P.B;
-                });
+                }, L.p.w_scale);
             }
         }
         fc_layer_sync();
@@ -828,6 +852,7 @@ TcConvPlan* tc_conv_plan_create(const TcConvDesc& d) {
         set_error("tc_conv: fp8-correction mode needs fp16 + e4m3 l8/h8 planes for activations and weights and a correction scale");
         return nullptr;
     }
+    if (d.half == Half16::FP16 && d.passes != 4 && !d.w_scale) { set_error("tc_conv: fp16 weight planes need their per-channel scales"); return nullptr; }
     if (d.passes == 4 && d.y.hi && (!d.y.l8 || !d.y.h8)) { set_error("tc_conv: fp8-correction mode needs l8/h8 output planes"); return nullptr; }
     if (d.passes == 4 && d.y.hi && ((d.Cy_total % 16) || (d.cy_off % 16))) { set_error("tc_conv: fp8 planes need 16-channel aligned offsets"); return nullptr; }
     if (d.pool && ((d.H | d.W) & 1)) { set_error("tc_conv: fused max-pool / stride 2 needs even H and W"); return nullptr; }
@@ -860,6 +885,7 @@ TcConvPlan* tc_conv_plan_create(const TcConvDesc& d) {
     p.n_valid = d.Cout;
     p.pool = d.pool;
     p.err_flag = d.err_flag;
+    p.w_scale = d.w_scale;
     // <= ~108 accumulating tensor-core steps per partial sum (9 K blocks x 4 K steps x 3 passes)
     p.chunk_kb = d.passes >= 3 ? 9 : 27;
     if (tune.chunk_kb > 0) p.chunk_kb = tune.chunk_kb;
@@ -959,7 +985,8 @@ FcChainPlan* fc_chain_plan_create(const FcChainDesc* chains, int num_chains, int
             const FcLayerDesc& d = cd.layer[l];
             FcLayer& L = P.chain[c].layer[l];
             const int Kpad = (int)align_up(d.in_features, BK);
-            if (!d.x.hi || !d.x.lo || !d.w.hi || !d.w.lo || d.out_pad % 64 || d.x_stride < Kpad || (d.y.hi && (d.y_stride % 8))) {
+            if (!d.x.hi || !d.x.lo || !d.w.hi || !d.w.lo || d.out_pad % 64 || d.x_stride < Kpad || (d.y.hi && (d.y_stride % 8)) ||
+                (half == Half16::FP16 && !d.w_scale)) {
                 set_error("fc_chain: bad layer %d of chain %d", l, c); delete pl; return nullptr;
             }
             bool ok = encode_act_map(&L.map_x_hi, d.x.hi, d.x_stride, Kpad, 1, 1, B, 1, 1, BM) &&
@@ -971,7 +998,7 @@ FcChainPlan* fc_chain_plan_create(const FcChainDesc* chains, int num_chains, int
             p.bias = d.bias; p.y_hi = d.y.hi; p.y_lo = d.y.lo; p.Cy_total = d.y_stride; p.cy_off = 0; p.corr_scale = 1.f;
             p.yf = d.yf; p.Cyf_total = d.yf_stride; p.cyf_off = 0;
             p.B = B; p.H = 1; p.W = 1; p.k = 1; p.TW = 1; p.TH = 1; p.TB = BM;
-            p.n_valid = d.out_features; p.pool = 0; p.leaky = d.leaky; p.err_flag = err_flag;
+            p.n_valid = d.out_features; p.pool = 0; p.leaky = d.leaky; p.err_flag = err_flag; p.w_scale = d.w_scale;
         }
     }
     return pl;

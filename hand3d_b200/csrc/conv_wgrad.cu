@@ -20,6 +20,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "split_fmt.cuh"
 #include "wgmma_common.cuh"
 
 namespace h3d {
@@ -216,17 +217,19 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ partial, float* __
 //   forward:       [Cout_pad][k][k][Cin_pad],  element w[kh][kw][ci][co]
 //   data gradient: [Cin_pad][k][k][Cout_pad],  element w[k-1-kh][k-1-kw][ci][co]
 // bias_pad [rows] = the bias zero-padded to the row count (forward), or zeros (data gradient: the transposed convolution has no bias).
+// w_scale (forward fp16 planes, else nullptr): the per-channel factors 2^-s of conv_w_shift_kernel; w / 2^-s is exact.
 template <bool FP16>
 __global__ void pack_conv_w_kernel(const float* __restrict__ w, const float* __restrict__ bias, uint16_t* __restrict__ hi,
-                                   uint16_t* __restrict__ lo, float* __restrict__ bias_pad, int k, int Cin, int Cout, int Cin_pad,
-                                   int Cout_pad, int dgrad) {
+                                   uint16_t* __restrict__ lo, float* __restrict__ bias_pad, const float* __restrict__ w_scale, int k,
+                                   int Cin, int Cout, int Cin_pad, int Cout_pad, int dgrad) {
     const int kk = k * k;
     const int rows = dgrad ? Cin_pad : Cout_pad, cols = dgrad ? Cout_pad : Cin_pad;
     const int64_t total = (int64_t)rows * kk * cols;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int c = (int)(i % cols), tap = (int)((i / cols) % kk), r = (int)(i / ((int64_t)cols * kk));
         const int co = dgrad ? c : r, ci = dgrad ? r : c, src_tap = dgrad ? kk - 1 - tap : tap;
-        const float v = (co < Cout && ci < Cin) ? __ldg(w + ((int64_t)src_tap * Cin + ci) * Cout + co) : 0.f;
+        float v = (co < Cout && ci < Cin) ? __ldg(w + ((int64_t)src_tap * Cin + ci) * Cout + co) : 0.f;
+        if (w_scale) v = __fdiv_rn(v, w_scale[co]);
         uint16_t h;
         float hf;
         if (FP16) { h = __half_as_ushort(__float2half_rn(v)); hf = __half2float(__ushort_as_half(h)); }
@@ -235,6 +238,18 @@ __global__ void pack_conv_w_kernel(const float* __restrict__ w, const float* __r
         if (lo) lo[i] = FP16 ? __half_as_ushort(__float2half_rn(v - hf)) : __bfloat16_as_ushort(__float2bfloat16_rn(v - hf));
         if (i < rows) bias_pad[i] = (!dgrad && bias && i < Cout) ? bias[i] : 0.f;
     }
+}
+
+// fp16 weight shifts (split_fmt.cuh): w_scale[co] = 2^-s(co) from max_k |w[k, co]|, 1 for the padding columns; one warp per column
+__global__ void conv_w_shift_kernel(const float* __restrict__ w, float* __restrict__ w_scale, int K, int Cout, int Cout_pad) {
+    const int co = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32, lane = threadIdx.x & 31;
+    if (co >= Cout_pad) return;
+    float mx = 0.f;
+    if (co < Cout)
+        for (int r = lane; r < K; r += 32) mx = fmaxf(mx, fabsf(__ldg(w + (int64_t)r * Cout + co)));
+#pragma unroll
+    for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xFFFFFFFFu, mx, o));
+    if (lane == 0) w_scale[co] = ldexpf(1.f, -fp16_w_shift(mx));
 }
 
 // dy' = dy * act'(y) as bf16 split planes [B,H,W,Cout_pad] (input resolution; stride 2: dy' at the odd pixels, zeros elsewhere).
@@ -365,14 +380,21 @@ int launch_conv_wgrad(const WgradDesc& d, cudaStream_t s) {
     return H3D_OK;
 }
 
-int launch_pack_conv_w(const float* w_hwio, const float* bias, Split out, float* bias_pad, int k, int Cin, int Cout, int Cin_pad,
-                       int Cout_pad, bool dgrad, Half16 half, cudaStream_t s) {
+int launch_pack_conv_w(const float* w_hwio, const float* bias, Split out, float* bias_pad, float* w_scale, int k, int Cin, int Cout,
+                       int Cin_pad, int Cout_pad, bool dgrad, Half16 half, cudaStream_t s) {
+    H3D_REQUIRE(!w_scale || (half == Half16::FP16 && !dgrad), "pack_conv_w: weight shifts belong to forward fp16 planes");
     const int64_t total = (int64_t)Cin_pad * Cout_pad * k * k;
     const int blocks = (int)std::min<int64_t>(ceil_div64(total, 256), 132 * 32);
+    if (w_scale) {
+        conv_w_shift_kernel<<<ceil_div(Cout_pad, 8), 256, 0, s>>>(w_hwio, w_scale, k * k * Cin, Cout, Cout_pad);
+        H3D_CHECK_LAUNCH();
+    }
     if (half == Half16::FP16)
-        pack_conv_w_kernel<true><<<blocks, 256, 0, s>>>(w_hwio, bias, out.hi, out.lo, bias_pad, k, Cin, Cout, Cin_pad, Cout_pad, dgrad ? 1 : 0);
+        pack_conv_w_kernel<true><<<blocks, 256, 0, s>>>(w_hwio, bias, out.hi, out.lo, bias_pad, w_scale, k, Cin, Cout, Cin_pad, Cout_pad,
+                                                        dgrad ? 1 : 0);
     else
-        pack_conv_w_kernel<false><<<blocks, 256, 0, s>>>(w_hwio, bias, out.hi, out.lo, bias_pad, k, Cin, Cout, Cin_pad, Cout_pad, dgrad ? 1 : 0);
+        pack_conv_w_kernel<false><<<blocks, 256, 0, s>>>(w_hwio, bias, out.hi, out.lo, bias_pad, w_scale, k, Cin, Cout, Cin_pad, Cout_pad,
+                                                         dgrad ? 1 : 0);
     H3D_CHECK_LAUNCH();
     return H3D_OK;
 }
