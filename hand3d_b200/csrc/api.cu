@@ -335,6 +335,17 @@ static int dev_weight(h3d_ctx* ctx, const std::string& name, const float** out) 
 // ------------------------------------------------------------------------------------------ workspace layout
 static int64_t slot_elems_seg(int B, int H, int W) { return (int64_t)B * H * W * 64; }
 
+// FC split-K scratch of one lifting branch on the CUDA-core path: the maximum of fc_scratch_floats over the stage's FC shapes.
+// fc_ksplit chooses each layer's split count from its tile count, so the widest layer is not always the one that needs the most
+// (fc_vp0, 4098 -> 256, needs more than fc_rel0, 2050 -> 512, at B = 33 ... 64 for example).
+static int64_t lift_fc_scratch_floats(int B) {
+    static const int shapes[][2] = {{2050, 512}, {512, 512}, {512, 30}, {512, 63}, {30, 63},   // PosePrior, incl. the bottleneck
+                                    {4098, 256}, {256, 128}, {128, 3}};                         // ViewpointNet, fused ux | uy | uz heads
+    int64_t m = 0;
+    for (const auto& sh : shapes) m = std::max(m, fc_scratch_floats(B, sh[0], sh[1]));
+    return m;
+}
+
 static void layout(h3d_ctx::Layout& L, char* base, int B, int H, int W) {
     Arena a; a.base = base;
     L.B = B; L.H = H; L.W = W;
@@ -357,7 +368,7 @@ static void layout(h3d_ctx::Layout& L, char* base, int B, int H, int W) {
     a.off = align_up(a.off, 1024); L.lift_off = a.off;
     // lifting: input planes + two ping-pong slots per branch (PosePrior, ViewpointNet), FC buffers and scratch per branch
     a.off += 5 * align_up((int64_t)B * 32 * 32 * 64 * 4, 1024) + 2 * 5 * align_up((int64_t)B * 4100 * 4, 1024) +
-             2 * align_up(fc_scratch_floats(B, 4098, 512) * 4, 1024) + 2 * align_up(kConvSplitKScratchFloats * 4, 1024) + 65536;
+             2 * align_up(lift_fc_scratch_floats(B) * 4, 1024) + 2 * align_up(kConvSplitKScratchFloats * 4, 1024) + 65536;
     L.total = align_up(a.off, 1024);
 }
 
@@ -688,12 +699,13 @@ static int ensure_vp_heads(h3d_ctx* ctx) {
     return H3D_OK;
 }
 
-static int add_fc(h3d_ctx* ctx, StagePlan* pl, const std::string& name, const float* x, float* y, float* scratch, int B, int in_f, int out_f, int leaky) {
+static int add_fc(h3d_ctx* ctx, StagePlan* pl, const std::string& name, const float* x, float* y, float* scratch, int64_t scratch_floats,
+                  int B, int in_f, int out_f, int leaky) {
     const float *w, *b;
     int rc;
     if ((rc = dev_weight(ctx, name + "/weights", &w))) return rc;
     if ((rc = dev_weight(ctx, name + "/biases", &b))) return rc;
-    pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_fc(x, w, b, y, scratch, B, in_f, out_f, leaky, in_f, s); });
+    pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_fc(x, w, b, y, scratch, scratch_floats, B, in_f, out_f, leaky, in_f, s); });
     pl->launches.push_back(2);
     pl->flops += 2ll * B * in_f * out_f;
     tag(pl, KIND_FC, 2ll * B * in_f * out_f);
@@ -715,12 +727,13 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
     const bool tc_lift = is_tc(ctx->precision) && passes_of(ctx->precision) != 4 && !tc_tuning().lift_direct;
     const int64_t slot_bytes = align_up((int64_t)B * 32 * 32 * 64 * 4, 1024);
     char* slot_in = a.alloc<char>(slot_bytes);
+    const int64_t fcs_floats = lift_fc_scratch_floats(B);
     struct Branch { char* slot[2]; float *xcat, *t1, *t2, *t3, *fcs, *cvs; } br[2];
     for (auto& b : br) {
         b.slot[0] = a.alloc<char>(slot_bytes); b.slot[1] = a.alloc<char>(slot_bytes);
         b.xcat = a.alloc<float>((int64_t)B * 4100);
         b.t1 = a.alloc<float>((int64_t)B * 512); b.t2 = a.alloc<float>((int64_t)B * 512); b.t3 = a.alloc<float>((int64_t)B * 64);
-        b.fcs = a.alloc<float>(fc_scratch_floats(B, 4098, 512));   // upper bound over all FC layers of the stage
+        b.fcs = a.alloc<float>(fcs_floats);
         b.cvs = a.alloc<float>(kConvSplitKScratchFloats);
     }
     float* can = a.alloc<float>((int64_t)B * 63);
@@ -888,13 +901,13 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
         float* xcat = b.xcat;
         pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_concat_handside(feat, e.hand_side, xcat, B, 2048, s); });
         pl->launches.push_back(1);
-        if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_rel0", b.xcat, b.t1, b.fcs, B, 2050, 512, 1))) return rc2;
-        if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_rel1", b.t1, b.t2, b.fcs, B, 512, 512, 1))) return rc2;
+        if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_rel0", b.xcat, b.t1, b.fcs, fcs_floats, B, 2050, 512, 1))) return rc2;
+        if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_rel1", b.t1, b.t2, b.fcs, fcs_floats, B, 512, 512, 1))) return rc2;
         if (bott) {
-            if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_bottleneck", b.t2, b.t3, b.fcs, B, 512, 30, 0))) return rc2;
-            if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_xyz", b.t3, can, b.fcs, B, 30, 63, 0))) return rc2;
+            if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_bottleneck", b.t2, b.t3, b.fcs, fcs_floats, B, 512, 30, 0))) return rc2;
+            if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_xyz", b.t3, can, b.fcs, fcs_floats, B, 30, 63, 0))) return rc2;
         } else {
-            if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_xyz", b.t2, can, b.fcs, B, 512, 63, 0))) return rc2;
+            if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_xyz", b.t2, can, b.fcs, fcs_floats, B, 512, 63, 0))) return rc2;
         }
         return H3D_OK;
     };
@@ -917,12 +930,12 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
             float* xcat = b.xcat;
             pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_concat_handside(feat, e.hand_side, xcat, B, 4096, s); });
             pl->launches.push_back(1);
-            if ((rc = add_fc(ctx, pl.get(), "ViewpointNet/fc_vp0", b.xcat, b.t1, b.fcs, B, 4098, 256, 1))) return rc;
-            if ((rc = add_fc(ctx, pl.get(), "ViewpointNet/fc_vp1", b.t1, b.t2, b.fcs, B, 256, 128, 1))) return rc;
+            if ((rc = add_fc(ctx, pl.get(), "ViewpointNet/fc_vp0", b.xcat, b.t1, b.fcs, fcs_floats, B, 4098, 256, 1))) return rc;
+            if ((rc = add_fc(ctx, pl.get(), "ViewpointNet/fc_vp1", b.t1, b.t2, b.fcs, fcs_floats, B, 256, 128, 1))) return rc;
         }
         const float* hw = ctx->vp_head_w; const float* hb = ctx->vp_head_b;
         float* t2 = b.t2; float* fcs = b.fcs;
-        pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_fc(t2, hw, hb, uxyz, fcs, B, 128, 3, 0, 128, s); });
+        pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_fc(t2, hw, hb, uxyz, fcs, fcs_floats, B, 128, 3, 0, 128, s); });
         pl->launches.push_back(2);
         tag(pl.get(), KIND_FC, 2ll * B * 128 * 3);
         pl->seal();
@@ -1572,9 +1585,10 @@ int h3d_fully_connected_f32(h3d_ctx* ctx, const float* x, const float* w, const 
                             int out_features, int leaky, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     char* scratch = nullptr;
-    int rc = op_scratch(ctx, fc_scratch_floats(B, in_features, out_features) * 4, &scratch);
+    const int64_t scratch_floats = fc_scratch_floats(B, in_features, out_features);
+    int rc = op_scratch(ctx, scratch_floats * 4, &scratch);
     if (rc) return rc;
-    rc = launch_fc(x, w, bias, y, (float*)scratch, B, in_features, out_features, leaky, in_features, s);
+    rc = launch_fc(x, w, bias, y, (float*)scratch, scratch_floats, B, in_features, out_features, leaky, in_features, s);
     if (!rc) ctx->launches += 2;
     return rc;
 }

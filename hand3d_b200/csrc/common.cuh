@@ -153,10 +153,11 @@ struct DirectConvArgs {
 constexpr int64_t kConvSplitKScratchFloats = 600ll * 64 * 64;   // upper bound used by launch_conv_direct's split-K policy
 int launch_conv_direct(const DirectConvArgs& a, cudaStream_t s);
 int conv_direct_num_launches(const DirectConvArgs& a);   // 1, or 2 when the split-K policy applies
-// scratch: fc_scratch_floats(B, in_f, out_f) floats (split-K partial sums); two kernels per call
+// scratch: fc_scratch_floats(B, in_f, out_f) floats (split-K partial sums); two kernels per call.  scratch_floats is the capacity
+// of the scratch buffer: a call that would need more returns H3D_EINVAL and launches nothing.
 int64_t fc_scratch_floats(int B, int in_f, int out_f);
-int launch_fc(const float* x, const float* w, const float* bias, float* y, float* scratch, int B, int in_f, int out_f, int leaky,
-              int x_stride, cudaStream_t s);
+int launch_fc(const float* x, const float* w, const float* bias, float* y, float* scratch, int64_t scratch_floats, int B, int in_f,
+              int out_f, int leaky, int x_stride, cudaStream_t s);
 // gathers [conv_feat(b, :feat) , hand_side(b, :2)] -> xcat [B, feat+2]
 int launch_concat_handside(const float* feat, const float* hand_side, float* out, int B, int feat_n, cudaStream_t s);
 // same as 16-bit split planes [B, Kpad] (Kpad % 64 == 0, zero padded): input of the tensor-core FC stack

@@ -444,9 +444,11 @@ int fc_ksplit(int B, int in_f, int out_f) {
 }
 int64_t fc_scratch_floats(int B, int in_f, int out_f) { return (int64_t)fc_ksplit(B, in_f, out_f) * B * out_f; }
 
-int launch_fc(const float* x, const float* w, const float* bias, float* y, float* scratch, int B, int in_f, int out_f, int leaky,
-              int x_stride, cudaStream_t s) {
+int launch_fc(const float* x, const float* w, const float* bias, float* y, float* scratch, int64_t scratch_floats, int B, int in_f,
+              int out_f, int leaky, int x_stride, cudaStream_t s) {
     const int ksplit = fc_ksplit(B, in_f, out_f);
+    H3D_REQUIRE((int64_t)ksplit * B * out_f <= scratch_floats, "fully_connected %d -> %d at B=%d: split-K needs %lld scratch floats, have %lld",
+                in_f, out_f, B, (long long)ksplit * B * out_f, (long long)scratch_floats);
     const int k_per_split = (int)align_up(ceil_div(in_f, ksplit), FCK);
     dim3 grid(ceil_div(out_f, FCN), ksplit, ceil_div(B, FCB));
     fc_splitk_kernel<<<grid, 256, 0, s>>>(x, w, scratch, B, in_f, out_f, x_stride, k_per_split);

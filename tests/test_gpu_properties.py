@@ -29,17 +29,17 @@ CONV = ["hand_scoremap", "keypoints_scoremap"]
 
 
 def test_batch_independence_and_sharding_b32(ctx):
-    """Full batch of 32 (BASELINE config 4 per-GPU shard) == two shards of 16 == ragged shards 7 + 25, bit for bit
-    (3-D coordinates: within 2e-6 -- the split-K FC / lifting kernels pick their reduction split from the batch size)."""
+    """Full batch of 32 (BASELINE config 4 per-GPU shard) == two shards of 16 == ragged shards 7 + 25, bit for bit, 3-D coordinates
+    included: in bf16x3 the lifting's pyramids run on conv_tc_kernel, whose arithmetic does not depend on B, and the FC chain computes
+    each row on its own (no split-K on the tensor-core path)."""
     B = 32
     img = Wt.synthetic_images(B, 320, 320, seed=21)
     hs = Wt.synthetic_hand_side(B, seed=22)
     full = _run(ctx, img, hs)
     for cuts in ([0, 16, 32], [0, 7, 32], [0, 1, 2, 32]):
         parts = [_run(ctx, img[a:b], hs[a:b]) for a, b in zip(cuts[:-1], cuts[1:])]
-        for k in DISCRETE + CONV:
+        for k in DISCRETE + CONV + ["keypoint_coord3d"]:
             np.testing.assert_array_equal(np.concatenate([p[k] for p in parts], 0), full[k], err_msg="%s, cuts %s" % (k, cuts))
-        np.testing.assert_allclose(np.concatenate([p["keypoint_coord3d"] for p in parts], 0), full["keypoint_coord3d"], atol=2e-6)
 
 
 def test_determinism(ctx):
