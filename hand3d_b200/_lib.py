@@ -71,7 +71,16 @@ SIGNATURES = {
     "h3d_bone_rel_trafo_inv": (_i, [_p, _p, _p, _i, _p]),
     "h3d_rotate_canonical": (_i, [_p, _p, _p, _p, _i, _p, _p, _p]),
     "h3d_flip_right_hand": (_i, [_p, _p, _p, _i, _p, _p]),
+    "h3d_resize_bilinear_tf1_backward": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _i, _p]),
+    "h3d_scoremap_loss_forward": (_i, [_p, _p, _p, _p, _i, _i, _i, _p, _p, _p]),
+    "h3d_scoremap_loss_backward": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _p]),
+    "h3d_softmax_xent_forward": (_i, [_p, _p, _p, _i64, _p, _p]),
+    "h3d_softmax_xent_backward": (_i, [_p, _p, _p, _p, _i64, _p, _p]),
+    "h3d_adam_state_set": (_i, [_p, _p, _f, _f, _f, _p]),
+    "h3d_adam_set_lr": (_i, [_p, _p, _f, _p]),
+    "h3d_adam_step": (_i, [_p, _p, _i, _p, _f, _f, _f, _p]),
 }
+ADAM_STATE_WORDS = 4   # H3D_ADAM_STATE_WORDS
 
 _lib = None
 

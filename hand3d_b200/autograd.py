@@ -7,6 +7,12 @@ input's device; there is no CPU path.
 
     y = conv2d(x, w, b, stride=1, leaky=True)    # NetworkOps.conv_relu (leaky=False: NetworkOps.conv)
     p = max_pool(y)                              # NetworkOps.max_pool
+    u = resize_bilinear(s, 256, 256)             # tf.image.resize_images
+    L = scoremap_loss(u, target, vis)            # training_posenet.py:61, one map
+    L = softmax_xent_loss(logits, labels)        # training_handsegnet.py:60
+
+The backward of every function reads the incoming gradient on the device: no .item(), no host synchronisation, so a whole training
+step can be captured into a CUDA graph.
 """
 from __future__ import annotations
 
@@ -53,6 +59,60 @@ class _MaxPool(torch.autograd.Function):
     def backward(ctx, dy):
         (x,) = ctx.saved_tensors
         return _ctx(dy).max_pool_backward(x, dy)
+
+
+class _Resize(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, out_h, out_w):
+        ctx.in_hw = (x.shape[1], x.shape[2])
+        return _ctx(x).resize_bilinear(x, out_h, out_w)
+
+    @staticmethod
+    def backward(ctx, dy):
+        return _ctx(dy).resize_bilinear_backward(dy, *ctx.in_hw), None, None
+
+
+class _ScoremapLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, pred, target, vis):
+        loss, rms = _ctx(pred).scoremap_loss(pred, target, vis)
+        ctx.save_for_backward(pred, target, vis, rms)
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        pred, target, vis, rms = ctx.saved_tensors
+        return _ctx(g).scoremap_loss_backward(pred, target, vis, rms, g), None, None
+
+
+class _SoftmaxXent(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, labels):
+        ctx.save_for_backward(logits, labels)
+        return _ctx(logits).softmax_xent(logits, labels)
+
+    @staticmethod
+    def backward(ctx, g):
+        logits, labels = ctx.saved_tensors
+        return _ctx(g).softmax_xent_backward(logits, labels, g), None
+
+
+def resize_bilinear(x, out_h, out_w):
+    """tf.image.resize_images (bilinear, align_corners=False, TF1 legacy) of x [B,H,W,C]; the backward is the forward's exact adjoint
+    (ResizeBilinearGrad)."""
+    return _Resize.apply(x, int(out_h), int(out_w))
+
+
+def scoremap_loss(pred, target, vis):
+    """training_posenet.py:61 for one map: sum vis sqrt(mean_hw (pred - target)^2) / (sum vis + 0.001); pred, target [B,H,W,21],
+    vis [B,21] (any dtype, cast to fp32).  Only pred receives a gradient; it is 0 where a (b, k) map matches its target exactly."""
+    return _ScoremapLoss.apply(pred, target.detach(), vis.detach().to(torch.float32))
+
+
+def softmax_xent_loss(logits, labels):
+    """training_handsegnet.py:60: reduce_mean(softmax_cross_entropy_with_logits(logits, labels)) over every [..., 2] row; labels fp32
+    (not necessarily one-hot).  Only logits receive a gradient."""
+    return _SoftmaxXent.apply(logits, labels.detach().to(torch.float32))
 
 
 def conv2d(x, w, b, stride=1, leaky=True, precision="bf16x3"):

@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libhand3d_b200.so")
 STAMP = os.path.join(HERE, ".libhand3d_b200.stamp")
-SOURCES = ["api.cu", "elementwise.cu", "reader.cu", "conv_direct.cu", "conv_wgmma.cu", "conv_wgrad.cu"]
+SOURCES = ["api.cu", "elementwise.cu", "reader.cu", "conv_direct.cu", "conv_wgmma.cu", "conv_wgrad.cu", "train.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--cudart=static", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",

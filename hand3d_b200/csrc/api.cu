@@ -1759,4 +1759,88 @@ int h3d_flip_right_hand(h3d_ctx* ctx, const float* coords_xyz, const uint8_t* co
     return rc;
 }
 
+// ---------------------------------------------------------------------------------------------- training (train.cu)
+int h3d_resize_bilinear_tf1_backward(h3d_ctx* ctx, const float* dy, float* dx, int B, int H, int W, int C, int out_h, int out_w,
+                                     void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(dy && dx, "h3d_resize_bilinear_tf1_backward: dy and dx are required");
+    H3D_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && out_h > 0 && out_w > 0,
+                "h3d_resize_bilinear_tf1_backward: bad shape B=%d H=%d W=%d C=%d out=%dx%d", B, H, W, C, out_h, out_w);
+    char* scratch = nullptr;
+    int rc = op_scratch(ctx, std::max<int64_t>(4, resize_grad_scratch_floats(B, H, W, C, out_h, out_w) * 4), &scratch);
+    if (rc) return rc;
+    int nl = 0;
+    rc = launch_resize_bilinear_tf1_grad(dy, dx, (float*)scratch, B, H, W, C, out_h, out_w, s, &nl);
+    ctx->launches += nl;
+    return rc;
+}
+int h3d_scoremap_loss_forward(h3d_ctx* ctx, const float* pred, const float* target, const float* vis, int B, int H, int W, float* loss,
+                              float* rms, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(pred && target && vis && loss && rms, "h3d_scoremap_loss_forward: pred, target, vis, loss and rms are required");
+    H3D_REQUIRE(B > 0 && H > 0 && W > 0 && (int64_t)H * W <= (1 << 30), "h3d_scoremap_loss_forward: bad shape B=%d H=%d W=%d", B, H, W);
+    char* scratch = nullptr;
+    int rc = op_scratch(ctx, scoremap_loss_scratch_floats(B, H, W) * 4, &scratch);
+    if (rc) return rc;
+    rc = launch_scoremap_loss(pred, target, vis, (float*)scratch, B, H, W, loss, rms, s);
+    if (!rc) ctx->launches += 2;
+    return rc;
+}
+int h3d_scoremap_loss_backward(h3d_ctx* ctx, const float* pred, const float* target, const float* vis, const float* rms,
+                               const float* grad_loss, int B, int H, int W, float* dpred, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(pred && target && vis && rms && dpred, "h3d_scoremap_loss_backward: pred, target, vis, rms and dpred are required");
+    H3D_REQUIRE(B > 0 && H > 0 && W > 0 && (int64_t)H * W <= (1 << 30), "h3d_scoremap_loss_backward: bad shape B=%d H=%d W=%d", B, H, W);
+    int rc = launch_scoremap_loss_grad(pred, target, vis, rms, grad_loss, dpred, B, H, W, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_softmax_xent_forward(h3d_ctx* ctx, const float* logits, const float* labels, int64_t rows, float* loss, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(logits && labels && loss, "h3d_softmax_xent_forward: logits, labels and loss are required");
+    H3D_REQUIRE(rows > 0, "h3d_softmax_xent_forward: rows must be positive, got %lld", (long long)rows);
+    H3D_REQUIRE(((uintptr_t)logits | (uintptr_t)labels) % 8 == 0, "h3d_softmax_xent_forward: logits and labels must be 8-byte aligned");
+    char* scratch = nullptr;
+    int rc = op_scratch(ctx, softmax_xent_scratch_floats(rows) * 4, &scratch);
+    if (rc) return rc;
+    rc = launch_softmax_xent(logits, labels, (float*)scratch, rows, loss, s);
+    if (!rc) ctx->launches += 2;
+    return rc;
+}
+int h3d_softmax_xent_backward(h3d_ctx* ctx, const float* logits, const float* labels, const float* grad_loss, int64_t rows, float* dlogits,
+                              void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(logits && labels && dlogits, "h3d_softmax_xent_backward: logits, labels and dlogits are required");
+    H3D_REQUIRE(rows > 0, "h3d_softmax_xent_backward: rows must be positive, got %lld", (long long)rows);
+    H3D_REQUIRE(((uintptr_t)logits | (uintptr_t)labels | (uintptr_t)dlogits) % 8 == 0,
+                "h3d_softmax_xent_backward: logits, labels and dlogits must be 8-byte aligned");
+    int rc = launch_softmax_xent_grad(logits, labels, grad_loss, dlogits, rows, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_adam_state_set(h3d_ctx* ctx, float* state, float lr, float beta1_power, float beta2_power, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(state && ((uintptr_t)state % 16) == 0, "h3d_adam_state_set: state must be a 16-byte aligned device pointer");
+    int rc = launch_adam_state_set(state, 7, lr, beta1_power, beta2_power, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_adam_set_lr(h3d_ctx* ctx, float* state, float lr, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(state && ((uintptr_t)state % 16) == 0, "h3d_adam_set_lr: state must be a 16-byte aligned device pointer");
+    int rc = launch_adam_state_set(state, 1, lr, 0.f, 0.f, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_adam_step(h3d_ctx* ctx, const h3d_adam_tensor* table, int num_tensors, float* state, float beta1, float beta2, float epsilon,
+                  void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(table && state && ((uintptr_t)state % 16) == 0, "h3d_adam_step: table and a 16-byte aligned state are required");
+    H3D_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && epsilon >= 0.f,
+                "h3d_adam_step: need 0 <= beta1, beta2 < 1 and epsilon >= 0");
+    int rc = launch_adam_step(table, num_tensors, state, beta1, beta2, epsilon, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+
 }  // extern "C"

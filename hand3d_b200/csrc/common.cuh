@@ -266,4 +266,21 @@ struct WgradDesc {
 int64_t conv_wgrad_partial_floats(int B, int H, int W, int k, int Cin_pad, int Cout_pad);
 int launch_conv_wgrad(const WgradDesc& d, cudaStream_t s);
 
+// ---------------------------------------------------------------- kernels (train.cu): resize gradient, training losses, Adam
+// scratch: resize_grad_scratch_floats(...) floats (the column pass's [B,oh,W,C] when both dimensions change); *n_launch kernels
+int64_t resize_grad_scratch_floats(int B, int H, int W, int C, int oh, int ow);
+int launch_resize_bilinear_tf1_grad(const float* dy, float* dx, float* scratch, int B, int H, int W, int C, int oh, int ow, cudaStream_t s,
+                                    int* n_launch);
+int64_t scoremap_loss_scratch_floats(int B, int H, int W);   // two kernels
+int launch_scoremap_loss(const float* P, const float* T, const float* vis, float* scratch, int B, int H, int W, float* loss, float* rms,
+                         cudaStream_t s);
+int launch_scoremap_loss_grad(const float* P, const float* T, const float* vis, const float* rms, const float* grad, float* dP, int B,
+                              int H, int W, cudaStream_t s);
+int64_t softmax_xent_scratch_floats(int64_t rows);           // two kernels
+int launch_softmax_xent(const float* logits, const float* labels, float* scratch, int64_t rows, float* loss, cudaStream_t s);
+int launch_softmax_xent_grad(const float* logits, const float* labels, const float* grad, float* dlogits, int64_t rows, cudaStream_t s);
+int launch_adam_step(const h3d_adam_tensor* table, int n, float* state, float beta1, float beta2, float epsilon, cudaStream_t s);
+// mask bit 0: lr, bit 1: beta1_power, bit 2: beta2_power; the ticket is always cleared
+int launch_adam_state_set(float* state, int mask, float lr, float beta1_power, float beta2_power, cudaStream_t s);
+
 }  // namespace h3d

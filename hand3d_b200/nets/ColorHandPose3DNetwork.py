@@ -9,11 +9,56 @@ import os
 
 import torch
 
-from .. import runtime, weights as _weights
+from .. import _lib, arch, autograd as A, runtime, weights as _weights
 
 
 def _truthy(x):
     return bool(x.item()) if torch.is_tensor(x) else bool(x)
+
+
+_TRAIN_PRECISIONS = {_lib.PRECISIONS["bf16x3"]: "bf16x3", _lib.PRECISIONS["bf16"]: "bf16"}
+
+
+def _train_scope(scope):
+    """(context, variables of scope, precision name) of a train=True graph; the convolution backward runs in bf16x3 or bf16 only."""
+    ctx = runtime.default_context()
+    prec = _TRAIN_PRECISIONS.get(ctx.precision)
+    if prec is None:
+        name = [k for k, v in _lib.PRECISIONS.items() if v == ctx.precision]
+        raise ValueError("train=True needs the context precision 'bf16x3' or 'bf16' (the convolution backward runs in these two), "
+                         "got %r" % (name[0] if name else ctx.precision))
+    return ctx, ctx.variables(scope), prec
+
+
+def _train_layers(x, v, scope, layers, pool_after, prec):
+    """The conv_relu / max_pool chain of nets/ColorHandPose3DNetwork.py:150-157 (HandSegNet) and :189-199 (PoseNet2D)."""
+    for name, k, stride, _, _, leaky in layers:
+        x = A.conv2d(x, v["%s/%s/weights" % (scope, name)], v["%s/%s/biases" % (scope, name)], stride, leaky, prec)
+        if name in pool_after:
+            x = A.max_pool(x)
+    return x
+
+
+def _train_detection(image):
+    ctx, v, prec = _train_scope("HandSegNet")
+    image = image.to(torch.float32).contiguous()
+    scoremap = _train_layers(image, v, "HandSegNet", arch.HANDSEGNET, arch.HANDSEGNET_POOL_AFTER, prec)
+    return A.resize_bilinear(scoremap, image.shape[1], image.shape[2])       # :165-166
+
+
+def _train_pose2d(image_crop, num_kp):
+    ctx, v, prec = _train_scope("PoseNet2D")
+    layers = {l[0]: l for l in arch.POSENET2D}
+    trunk = [layers[n] for n in ("conv1_1", "conv1_2", "conv2_1", "conv2_2", "conv3_1", "conv3_2", "conv3_3", "conv3_4", "conv4_1",
+                                 "conv4_2", "conv4_3", "conv4_4", "conv4_5", "conv4_6", "conv4_7")]
+    encoding = _train_layers(image_crop.to(torch.float32).contiguous(), v, "PoseNet2D", trunk, arch.POSENET2D_POOL_AFTER, prec)
+    scoremap_list = [_train_layers(encoding, v, "PoseNet2D", [layers["conv5_1"], layers["conv5_2"]], (), prec)]    # :202-204
+    for pass_id in range(2):                                                                                      # :207-215
+        x = torch.cat([scoremap_list[-1], encoding], 3)      # 21 + 128 = 149 channels: a plain copy, as tf.concat
+        unit = [layers["conv%d_%d" % (pass_id + 6, i)] for i in range(1, 8)]
+        scoremap_list.append(_train_layers(x, v, "PoseNet2D", unit, (), prec))
+    assert all(s.shape[3] == num_kp for s in scoremap_list)
+    return scoremap_list
 
 
 class ColorHandPose3DNetwork(object):
@@ -72,15 +117,23 @@ class ColorHandPose3DNetwork(object):
 
     @staticmethod
     def inference_detection(image, train=False):
-        """ HandSegNet (reference :131-168): image [B,H,W,3] -> list of one [B,H,W,2] logits tensor. """
+        """ HandSegNet (reference :131-168): image [B,H,W,3] -> list of one [B,H,W,2] logits tensor.
+
+            train=True builds the same graph from hand3d_b200.autograd over ctx.variables('HandSegNet'), so that a loss of its
+            output back-propagates into those Parameters (training_handsegnet.py:47); H and W must be multiples of 8.
+        """
         if train:
-            raise NotImplementedError("forward pass only: train must be False")
+            return [_train_detection(image)]
         return [runtime.default_context().handsegnet(image)]
 
     def inference_pose2d(self, image_crop, train=False):
-        """ PoseNet (reference :170-219): image_crop [B,256,256,3] -> list of three [B,32,32,21] score maps. """
+        """ PoseNet (reference :170-219): image_crop [B,256,256,3] -> list of three [B,32,32,21] score maps.
+
+            train=True builds the same graph from hand3d_b200.autograd over ctx.variables('PoseNet2D') (training_posenet.py:47);
+            the maps are then [B,H/8,W/8,21] for crops whose sides are multiples of 8.
+        """
         if train:
-            raise NotImplementedError("forward pass only: train must be False")
+            return _train_pose2d(image_crop, self.num_kp)
         return runtime.default_context().posenet(image_crop)
 
     def _inference_pose3d(self, keypoints_scoremap, hand_side, evaluation=True, train=False):

@@ -105,6 +105,10 @@ class Context:
             _lib.check(rc, "h3d_load_weight(%s)" % name)
             self.weights[name] = a
             self.__dict__.get("_dev_w", {}).pop(name, None)    # the operator-level device copy follows the reload
+            var = self.__dict__.get("_variables", {}).get(name.split("/")[0])
+            if var is not None and name in var:   # so do the trainable variables: in place, so an optimiser over them stays valid
+                with torch.no_grad():
+                    var[name].copy_(torch.from_numpy(a))
 
     def scope_ready(self, scope):
         return bool(self.lib.h3d_scope_ready(self.h, scope.encode()))
@@ -378,6 +382,103 @@ class Context:
         _lib.check(self.lib.h3d_resize_bilinear_tf1(self.h, _ptr(x), _ptr(y), B, H, W, Cc, out_h, out_w, _stream()),
                    "h3d_resize_bilinear_tf1")
         return y
+
+    # ---- training (h3d_resize_bilinear_tf1_backward, the two losses, Adam) ----------------------
+    def variables(self, scope):
+        """Ordered {reference variable name: torch.nn.Parameter} of "HandSegNet" or "PoseNet2D" (layer order of the reference graph,
+        weights before biases): fp32 device copies of the host arrays load_weights keeps, created once per context and then shared by
+        every train=True graph, so an optimiser over them trains the network in place.
+
+        The inference path (train=False, pipeline(), the stage entries) keeps the weights last loaded, not these Parameters: call
+        commit_variables(scope) to make it use the trained values.  A later load_weights of the scope writes the loaded values into
+        the same Parameters in place, so an optimiser built over them keeps working (its m / v slots are not reset)."""
+        from . import arch
+        layers = {"HandSegNet": arch.HANDSEGNET, "PoseNet2D": arch.POSENET2D}
+        if scope not in layers:
+            raise ValueError("variables(): scope must be 'HandSegNet' or 'PoseNet2D', got %r" % (scope,))
+        cache = self.__dict__.setdefault("_variables", {})
+        if scope not in cache:
+            names = ["%s/%s/%s" % (scope, l[0], what) for l in layers[scope] for what in ("weights", "biases")]
+            missing = [n for n in names if n not in self.weights]
+            if missing:
+                raise ValueError("variables(%r): the scope was not loaded (%d of %d variables missing, e.g. %s); call "
+                                 "ColorHandPose3DNetwork().init() first" % (scope, len(missing), len(names), missing[0]))
+            cache[scope] = {n: torch.nn.Parameter(torch.from_numpy(self.weights[n].copy()).to(self.device)) for n in names}
+        return cache[scope]
+
+    def commit_variables(self, scope):
+        """Loads the current values of variables(scope) as the inference weights of the scope (as load_weights does with a pickle),
+        so that train=False graphs, pipeline() and the stage entries use the trained network.  Reads the Parameters on the host."""
+        self.load_weights({n: p.detach().cpu().numpy() for n, p in self.variables(scope).items()})
+
+    def resize_bilinear_backward(self, dy, H, W):
+        """Gradient of resize_bilinear(x [B,H,W,C], out_h, out_w): dy [B,out_h,out_w,C] -> dx [B,H,W,C]."""
+        dy = _chk_f32(dy, "dy", 4)
+        B, oh, ow, Cc = dy.shape
+        dx = torch.empty((B, int(H), int(W), Cc), dtype=torch.float32, device=dy.device)
+        _lib.check(self.lib.h3d_resize_bilinear_tf1_backward(self.h, _ptr(dy), _ptr(dx), B, int(H), int(W), Cc, oh, ow, _stream()),
+                   "h3d_resize_bilinear_tf1_backward")
+        return dx
+
+    def _scoremap_args(self, pred, target, vis):
+        pred = _chk_f32(pred, "pred", 4); target = _chk_f32(target, "target", 4)
+        B, H, W, K = pred.shape
+        if K != 21 or tuple(target.shape) != tuple(pred.shape):
+            raise ValueError("scoremap loss: pred and target must both be [B,H,W,21], got %s and %s" % (tuple(pred.shape), tuple(target.shape)))
+        vis = _chk_f32(vis.to(torch.float32).reshape(B, 21), "vis")
+        return pred, target, vis, B, H, W
+
+    def scoremap_loss(self, pred, target, vis):
+        """training_posenet.py:61 for one map -> (loss, a 0-d device tensor; rms [B,21])."""
+        pred, target, vis, B, H, W = self._scoremap_args(pred, target, vis)
+        loss = torch.empty((), dtype=torch.float32, device=pred.device)
+        rms = torch.empty((B, 21), dtype=torch.float32, device=pred.device)
+        _lib.check(self.lib.h3d_scoremap_loss_forward(self.h, _ptr(pred), _ptr(target), _ptr(vis), B, H, W, _ptr(loss), _ptr(rms), _stream()),
+                   "h3d_scoremap_loss_forward")
+        return loss, rms
+
+    def scoremap_loss_backward(self, pred, target, vis, rms, grad_loss=None):
+        """dL/dpred for the incoming gradient grad_loss (a device scalar, None = 1)."""
+        pred, target, vis, B, H, W = self._scoremap_args(pred, target, vis)
+        rms = _chk_f32(rms, "rms", 2)
+        g = _chk_f32(grad_loss.reshape(()), "grad_loss") if grad_loss is not None else None
+        dpred = torch.empty_like(pred)
+        _lib.check(self.lib.h3d_scoremap_loss_backward(self.h, _ptr(pred), _ptr(target), _ptr(vis), _ptr(rms), _ptr(g), B, H, W, _ptr(dpred),
+                                                       _stream()), "h3d_scoremap_loss_backward")
+        return dpred
+
+    def _xent_args(self, logits, labels):
+        logits = _chk_f32(logits, "logits"); labels = _chk_f32(labels, "labels")
+        if logits.shape[-1] != 2 or tuple(labels.shape) != tuple(logits.shape):
+            raise ValueError("softmax_xent: logits and labels must both be [..., 2], got %s and %s" % (tuple(logits.shape), tuple(labels.shape)))
+        return logits, labels, logits.numel() // 2
+
+    def softmax_xent(self, logits, labels):
+        """training_handsegnet.py:60: mean softmax cross-entropy of [..., 2] logits and labels -> 0-d device tensor."""
+        logits, labels, rows = self._xent_args(logits, labels)
+        loss = torch.empty((), dtype=torch.float32, device=logits.device)
+        _lib.check(self.lib.h3d_softmax_xent_forward(self.h, _ptr(logits), _ptr(labels), rows, _ptr(loss), _stream()), "h3d_softmax_xent_forward")
+        return loss
+
+    def softmax_xent_backward(self, logits, labels, grad_loss=None):
+        logits, labels, rows = self._xent_args(logits, labels)
+        g = _chk_f32(grad_loss.reshape(()), "grad_loss") if grad_loss is not None else None
+        d = torch.empty_like(logits)
+        _lib.check(self.lib.h3d_softmax_xent_backward(self.h, _ptr(logits), _ptr(labels), _ptr(g), rows, _ptr(d), _stream()),
+                   "h3d_softmax_xent_backward")
+        return d
+
+    def adam_state_set(self, state, lr, beta1_power, beta2_power):
+        _lib.check(self.lib.h3d_adam_state_set(self.h, _ptr(state), C.c_float(lr), C.c_float(beta1_power), C.c_float(beta2_power), _stream()),
+                   "h3d_adam_state_set")
+
+    def adam_set_lr(self, state, lr):
+        _lib.check(self.lib.h3d_adam_set_lr(self.h, _ptr(state), C.c_float(lr), _stream()), "h3d_adam_set_lr")
+
+    def adam_step(self, table, n, state, beta1, beta2, epsilon):
+        """table: int64 device tensor [n, 5] of h3d_adam_tensor rows (param, grad, m, v pointers, numel)."""
+        _lib.check(self.lib.h3d_adam_step(self.h, _ptr(table), int(n), _ptr(state), C.c_float(beta1), C.c_float(beta2), C.c_float(epsilon),
+                                          _stream()), "h3d_adam_step")
 
     def avg_pool8(self, x):
         x = _chk_f32(x, "x", 4)

@@ -5,8 +5,9 @@ hand-written sm_90a kernels behind the C ABI (include/hand3d_b200.h).
 Reference: utils/general.py:26-65,113-148 (NetworkOps), :163 crop_image_from_xy, :199 find_max_location,
 :233 single_obj_scoremap, :271 calc_center_bb, :331 detect_keypoints, :347 trafo_coords.
 EvalUtil (:522-611) is mirrored with a batched device path (SURVEY.md 8(f) row 3).
+LearningRateScheduler (:480-519) is mirrored as a host function of an integer step.
 Not mirrored (dead code in every graph / out of scope, SURVEY.md section 2): upconv*, spatial_dropout,
-plot helpers, LearningRateScheduler, load_weights_from_snapshot.
+plot helpers, load_weights_from_snapshot.
 """
 from __future__ import annotations
 
@@ -163,6 +164,33 @@ def trafo_coords(keypoints_crop_coords, centers, scale, crop_size):
         scale = scale.reshape(-1, 1, 1)
         centers = centers.reshape(-1, 1, 2)
     return k / scale + centers
+
+
+class LearningRateScheduler:
+    """ Multistep learning-rate schedule (utils/general.py:480-519) evaluated on the host for an integer step.
+
+        get_lr(step) returns the value TF's graph yields, as a float32, with the reference's branch quirks:
+        one value: constant; two values: values[1] where step > steps[0] (strict), else values[0];
+        n > 2 values: the sum of the values whose condition holds, the conditions being step < steps[0],
+        steps[i] <= step < steps[i+1] and step >= steps[-1].
+    """
+    def __init__(self, steps, values):
+        self.steps = steps
+        self.values = values
+
+        assert len(steps)+1 == len(values), "There must be one more element in value as step."
+
+    def get_lr(self, global_step):
+        step = int(global_step)
+        vals = [np.float32(v) for v in self.values]
+        if len(vals) == 1:
+            return vals[0]
+        if len(vals) == 2:
+            return vals[1] if step > self.steps[0] else vals[0]
+        conds = [step < self.steps[0]]
+        conds += [self.steps[i] <= step < self.steps[i + 1] for i in range(len(self.steps) - 1)]
+        conds.append(step >= self.steps[-1])
+        return np.sum(np.where(conds, np.array(vals, np.float32), np.float32(0)), dtype=np.float32)
 
 
 class EvalUtil:

@@ -58,6 +58,21 @@ def load_weight_files(weight_files, exclude_var_list=None, verbose=True):
     return merged
 
 
+def save_weight_file(path, variables):
+    """Writes a snapshot in the reference's pickle layout ({variable_name: float32 ndarray}, pickle protocol 2), which
+    ColorHandPose3DNetwork().init(weight_files=[path]) loads back.  variables: {name: ndarray or tensor}, e.g. ctx.variables(scope)."""
+    out = {}
+    for name, v in variables.items():
+        if hasattr(v, "detach"):
+            v = v.detach().cpu().numpy()
+        out[name] = np.ascontiguousarray(v, dtype=np.float32)
+    tmp = path + ".tmp"
+    with open(tmp, "wb") as f:
+        pickle.dump(out, f, protocol=2)
+    os.replace(tmp, path)
+    return path
+
+
 def validate(weight_dict, known=None):
     """Unknown names raise (as tf.contrib.framework.assign_from_values does); shapes must match."""
     known = known or {**arch.variable_shapes(False), **arch.variable_shapes(True)}

@@ -283,6 +283,59 @@ H3D_API int h3d_rotate_canonical(h3d_ctx* ctx, const float* coord_can, const flo
 /* _flip_right_hand (nets/ColorHandPose3DNetwork.py:336-361): out = coords with z negated where cond_right[b] != 0 (u8 [B]). */
 H3D_API int h3d_flip_right_hand(h3d_ctx* ctx, const float* coords_xyz, const uint8_t* cond_right, int B, float* out, void* stream);
 
+/* ---- Training of HandSegNet and PoseNet2D (training_posenet.py, training_handsegnet.py) ----
+ * Like h3d_conv2d_tc_backward: enqueue-only (operator scratch), no float atomics, every sum in an order fixed by the shapes, so the
+ * results are bit-reproducible; capturable into a CUDA graph once a first call has sized the scratch.  grad_loss is the incoming
+ * gradient of a loss as a DEVICE scalar (NULL = 1), so a backward never reads a value on the host. */
+
+/* Gradient of tf.image.resize_images (TF ResizeBilinearGrad: bilinear, align_corners = False, TF1 legacy) between the networks and
+ * their losses (training_posenet.py:49, nets/ColorHandPose3DNetwork.py:166): dy [B,out_h,out_w,C] -> dx [B,H,W,C], the exact adjoint
+ * of h3d_resize_bilinear_tf1 (source indices and weights from the forward's own fp32 operations), any ratio, up or down; equal sizes
+ * copy.  Sums gather in ascending output order. */
+H3D_API int h3d_resize_bilinear_tf1_backward(h3d_ctx* ctx, const float* dy, float* dx, int B, int H, int W, int C, int out_h, int out_w,
+                                             void* stream);
+/* PoseNet score-map loss for one predicted map (training_posenet.py:58-61):
+ *   loss = sum_{b,k} vis[b,k] sqrt(mean_{h,w} (pred - target)^2) / (sum_{b,k} vis + 0.001)
+ * pred, target [B,H,W,21], vis [B,21] fp32 (0 / 1, any value is accepted) -> loss (device scalar) and rms [B,21] =
+ * sqrt(mean (pred - target)^2), which the backward reuses.  fp32 with separate multiply and add. */
+H3D_API int h3d_scoremap_loss_forward(h3d_ctx* ctx, const float* pred, const float* target, const float* vis, int B, int H, int W,
+                                      float* loss, float* rms, void* stream);
+/* Its gradient: dpred [B,H,W,21] = grad_loss vis[b,k] / S (pred - target) / (H W rms[b,k]), S = sum vis + 0.001; 0 where
+ * rms[b,k] == 0 (TF's SqrtGrad gives NaN there). */
+H3D_API int h3d_scoremap_loss_backward(h3d_ctx* ctx, const float* pred, const float* target, const float* vis, const float* rms,
+                                       const float* grad_loss, int B, int H, int W, float* dpred, void* stream);
+/* HandSegNet loss (training_handsegnet.py:56-60): reduce_mean(softmax_cross_entropy_with_logits(logits, labels)) over `rows` rows of 2
+ * classes.  logits, labels [rows,2] fp32 (8-byte aligned; labels need not be one-hot) -> loss (device scalar).  Per row as TF's
+ * SoftmaxXentWithLogits: m = max, s = sum exp(x - m), loss = sum labels (log s - (x - m)). */
+H3D_API int h3d_softmax_xent_forward(h3d_ctx* ctx, const float* logits, const float* labels, int64_t rows, float* loss, void* stream);
+/* Its gradient: dlogits [rows,2] = grad_loss / rows (softmax(logits) - labels). */
+H3D_API int h3d_softmax_xent_backward(h3d_ctx* ctx, const float* logits, const float* labels, const float* grad_loss, int64_t rows,
+                                      float* dlogits, void* stream);
+
+/* tf.train.AdamOptimizer (TF 1.3 ApplyAdam, training_posenet.py:67).  The optimiser state is H3D_ADAM_STATE_WORDS 32-bit words of
+ * DEVICE memory owned by the caller: [lr, beta1_power, beta2_power (fp32), ticket (uint32, 0 between steps)].  Keeping the learning
+ * rate and the beta powers on the device lets a captured CUDA graph replay the step. */
+#define H3D_ADAM_STATE_WORDS 4
+typedef struct h3d_adam_tensor {   /* one variable: param, its gradient and the slots m, v, all fp32 [numel] device arrays */
+    float* param;
+    const float* grad;
+    float* m;
+    float* v;
+    int64_t numel;
+} h3d_adam_tensor;
+/* Writes the state: lr, beta1_power and beta2_power (a fresh optimiser: beta1_power = beta1, beta2_power = beta2, as TF creates the
+ * accumulators) and clears the ticket.  Enqueued on `stream`. */
+H3D_API int h3d_adam_state_set(h3d_ctx* ctx, float* state, float lr, float beta1_power, float beta2_power, void* stream);
+/* Writes the learning rate only (LearningRateScheduler.get_lr's value for this step). */
+H3D_API int h3d_adam_set_lr(h3d_ctx* ctx, float* state, float lr, void* stream);
+/* One Adam step over every tensor of `table` (a DEVICE array of num_tensors <= 1024 entries) in one launch.  Per element, in this order
+ * and in fp32 without contraction: alpha = lr sqrt(1 - beta2_power) / (1 - beta1_power) (once per call), m += (g - m)(1 - beta1),
+ * v += (g^2 - v)(1 - beta2), param -= m alpha / (sqrt(v) + epsilon): TF's epsilon-hat form, which differs from torch.optim.Adam for
+ * small gradients.  After every element has used them, the last block multiplies beta1_power by beta1 and beta2_power by beta2 (fp32),
+ * as AdamOptimizer._finish does.  The reference's defaults are beta1 0.9, beta2 0.999, epsilon 1e-8. */
+H3D_API int h3d_adam_step(h3d_ctx* ctx, const h3d_adam_tensor* table, int num_tensors, float* state, float beta1, float beta2,
+                          float epsilon, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
