@@ -79,6 +79,11 @@ SIGNATURES = {
     "h3d_adam_state_set": (_i, [_p, _p, _f, _f, _f, _p]),
     "h3d_adam_set_lr": (_i, [_p, _p, _f, _p]),
     "h3d_adam_step": (_i, [_p, _p, _i, _p, _f, _f, _f, _p]),
+    "h3d_rotate_canonical_backward": (_i, [_p, _p, _p, _p, _p, _p, _i, _p, _p, _p]),
+    "h3d_bone_rel_trafo_inv_backward": (_i, [_p, _p, _p, _p, _i, _p]),
+    "h3d_bone_rel_trafo": (_i, [_p, _p, _p, _i, _p]),
+    "h3d_mse_loss_forward": (_i, [_p, _p, _p, _i64, _p, _p]),
+    "h3d_mse_loss_backward": (_i, [_p, _p, _p, _p, _i64, _p, _p]),
 }
 ADAM_STATE_WORDS = 4   # H3D_ADAM_STATE_WORDS
 

@@ -10,6 +10,10 @@ input's device; there is no CPU path.
     u = resize_bilinear(s, 256, 256)             # tf.image.resize_images
     L = scoremap_loss(u, target, vis)            # training_posenet.py:61, one map
     L = softmax_xent_loss(logits, labels)        # training_handsegnet.py:60
+    y = fully_connected(x, w, b, leaky=True)     # ops.fully_connected_relu, on the 1x1 tensor-core convolution
+    R, out = rotate_canonical(can, uxyz, hs)     # PosePriorNetwork 'proposed': Rodrigues, flip, rotate
+    xyz = bone_rel_trafo_inv(rel)                # the 'local*' variants' forward kinematics
+    L = mse_loss(pred, target)                   # training_lifting.py:63-76
 
 The backward of every function reads the incoming gradient on the device: no .item(), no host synchronisation, so a whole training
 step can be captured into a CUDA graph.
@@ -95,6 +99,70 @@ class _SoftmaxXent(torch.autograd.Function):
     def backward(ctx, g):
         logits, labels = ctx.saved_tensors
         return _ctx(g).softmax_xent_backward(logits, labels, g), None
+
+
+class _RotateCanonical(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, can, uxyz, hand_side):
+        ctx.set_materialize_grads(False)        # an unused output passes None, and the kernel skips its term
+        ctx.save_for_backward(can, uxyz, hand_side)
+        return _ctx(can).rotate_canonical(can, uxyz, hand_side)
+
+    @staticmethod
+    def backward(ctx, d_rot, d_out):
+        can, uxyz, hand_side = ctx.saved_tensors
+        if d_rot is None and d_out is None:
+            return None, None, None
+        d_can, d_u = _ctx(can).rotate_canonical_backward(can, uxyz, hand_side, d_out, d_rot)
+        return d_can, d_u, None
+
+
+class _BoneRelTrafoInv(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, rel):
+        ctx.save_for_backward(rel)
+        return _ctx(rel).bone_rel_trafo_inv(rel)
+
+    @staticmethod
+    def backward(ctx, d_xyz):
+        (rel,) = ctx.saved_tensors
+        return _ctx(d_xyz).bone_rel_trafo_inv_backward(rel, d_xyz).reshape(rel.shape)
+
+
+class _MseLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, pred, target):
+        ctx.save_for_backward(pred, target)
+        return _ctx(pred).mse_loss(pred, target)
+
+    @staticmethod
+    def backward(ctx, g):
+        pred, target = ctx.saved_tensors
+        return _ctx(g).mse_loss_backward(pred, target, g), None
+
+
+def fully_connected(x, w, b, leaky=True, precision="bf16x3"):
+    """ops.fully_connected(_relu) (utils/general.py:113-137): act(x w + b) for x [B,in], w [in,out], b [out], run as the 1x1
+    tensor-core convolution of x viewed as [B,1,1,in] (the layout the inference FC layers use); leaky=False is the plain layer."""
+    B, n_in = x.shape
+    y = conv2d(x.contiguous().view(B, 1, 1, n_in), w.view(1, 1, *w.shape), b, 1, leaky, precision)
+    return y.view(B, w.shape[1])
+
+
+def rotate_canonical(can, uxyz, hand_side):
+    """The end of the 'proposed' lifting (nets/PosePriorNetwork.py:82-91): R = Rodrigues(uxyz) [B,3,3], out = flip(can) R [B,21,3],
+    z mirrored where argmax(hand_side) == 1.  Returns (R, out); can and uxyz receive gradients from either output."""
+    return _RotateCanonical.apply(can.contiguous(), uxyz.contiguous(), hand_side.detach().to(torch.float32).contiguous())
+
+
+def bone_rel_trafo_inv(coords_rel):
+    """utils/relative_trafo.py:243-295 with its adjoint: coords_rel [B,21,3] (length, angle_x, angle_y) -> xyz [B,21,3]."""
+    return _BoneRelTrafoInv.apply(coords_rel.contiguous())
+
+
+def mse_loss(pred, target):
+    """tf.reduce_mean(tf.square(pred - target)) (training_lifting.py:63-76) over any shape; only pred receives a gradient."""
+    return _MseLoss.apply(pred.contiguous(), target.detach().to(torch.float32).contiguous())
 
 
 def resize_bilinear(x, out_h, out_w):

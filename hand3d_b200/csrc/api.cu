@@ -1843,4 +1843,52 @@ int h3d_adam_step(h3d_ctx* ctx, const h3d_adam_tensor* table, int num_tensors, f
     return rc;
 }
 
+// ---------------------------------------------------------------------------------------------- lifting training (train_lift.cu)
+int h3d_rotate_canonical_backward(h3d_ctx* ctx, const float* coord_can, const float* uxyz, const float* hand_side, const float* d_out,
+                                  const float* d_rot_mat, int B, float* d_can, float* d_uxyz, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(coord_can && uxyz && hand_side && d_can && d_uxyz,
+                "h3d_rotate_canonical_backward: coord_can, uxyz, hand_side, d_can and d_uxyz are required");
+    H3D_REQUIRE(B > 0, "h3d_rotate_canonical_backward: bad shape B=%d", B);
+    int rc = launch_rotate_canonical_backward(coord_can, uxyz, hand_side, d_out, d_rot_mat, B, d_can, d_uxyz, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_bone_rel_trafo_inv_backward(h3d_ctx* ctx, const float* coords_rel, const float* d_xyz, float* d_rel, int B, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(coords_rel && d_xyz && d_rel, "h3d_bone_rel_trafo_inv_backward: coords_rel, d_xyz and d_rel are required");
+    H3D_REQUIRE(B > 0, "h3d_bone_rel_trafo_inv_backward: bad shape B=%d", B);
+    int rc = launch_bone_rel_trafo_inv_backward(coords_rel, d_xyz, d_rel, B, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_bone_rel_trafo(h3d_ctx* ctx, const float* coords_xyz, float* coords_rel, int B, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(coords_xyz && coords_rel, "h3d_bone_rel_trafo: coords_xyz and coords_rel are required");
+    H3D_REQUIRE(B > 0, "h3d_bone_rel_trafo: bad shape B=%d", B);
+    int rc = launch_bone_rel_trafo(coords_xyz, coords_rel, B, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_mse_loss_forward(h3d_ctx* ctx, const float* pred, const float* target, int64_t n, float* loss, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(pred && target && loss, "h3d_mse_loss_forward: pred, target and loss are required");
+    H3D_REQUIRE(n > 0, "h3d_mse_loss_forward: n must be positive, got %lld", (long long)n);
+    char* scratch = nullptr;
+    int rc = op_scratch(ctx, mse_scratch_floats(n) * 4, &scratch);
+    if (rc) return rc;
+    rc = launch_mse(pred, target, (float*)scratch, n, loss, s);
+    if (!rc) ctx->launches += 2;
+    return rc;
+}
+int h3d_mse_loss_backward(h3d_ctx* ctx, const float* pred, const float* target, const float* grad_loss, int64_t n, float* dpred,
+                          void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(pred && target && dpred, "h3d_mse_loss_backward: pred, target and dpred are required");
+    H3D_REQUIRE(n > 0, "h3d_mse_loss_backward: n must be positive, got %lld", (long long)n);
+    int rc = launch_mse_grad(pred, target, grad_loss, dpred, n, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+
 }  // extern "C"

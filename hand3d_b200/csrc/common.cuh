@@ -283,4 +283,13 @@ int launch_adam_step(const h3d_adam_tensor* table, int n, float* state, float be
 // mask bit 0: lr, bit 1: beta1_power, bit 2: beta2_power; the ticket is always cleared
 int launch_adam_state_set(float* state, int mask, float lr, float beta1_power, float beta2_power, cudaStream_t s);
 
+// ---------------------------------------------------------------- kernels (train_lift.cu): the lifting stage's adjoints and its loss
+int launch_rotate_canonical_backward(const float* can, const float* uxyz, const float* hand_side, const float* d_out, const float* d_R,
+                                     int B, float* d_can, float* d_uxyz, cudaStream_t s);
+int launch_bone_rel_trafo_inv_backward(const float* rel, const float* d_xyz, float* d_rel, int B, cudaStream_t s);
+int launch_bone_rel_trafo(const float* xyz, float* rel, int B, cudaStream_t s);
+int64_t mse_scratch_floats(int64_t n);                        // two kernels
+int launch_mse(const float* p, const float* q, float* scratch, int64_t n, float* loss, cudaStream_t s);
+int launch_mse_grad(const float* p, const float* q, const float* grad, float* dp, int64_t n, cudaStream_t s);
+
 }  // namespace h3d

@@ -81,6 +81,7 @@ class BinaryDbReader(object):
         right = it["hand_side"][:, 1] > 0.5
         can, _, rot_inv = ctx.canonical_trafo(it["keypoint_xyz21_normed"], right)
         d["keypoint_xyz21_can"], d["rot_mat"] = can, rot_inv
+        d["keypoint_xyz21_local"] = ctx.bone_rel_trafo(it["keypoint_xyz21_normed"])      # :245-247, the 'local' lifting target
         size = self.image_size
         if self.hand_crop:
             d["crop_scale"] = it["crop_scale"]
@@ -131,6 +132,7 @@ class BinaryDbReaderSTB(object):
              "hand_side": torch.tensor([1.0, 0.0], device=dev).expand(B, 2).contiguous()}
         can, _, rot_inv = ctx.canonical_trafo(it["keypoint_xyz21_normed"], None)
         d["keypoint_xyz21_can"], d["rot_mat"] = can, rot_inv
+        d["keypoint_xyz21_local"] = ctx.bone_rel_trafo(it["keypoint_xyz21_normed"])      # :199-202
         if self.with_scoremap:             # 480 x 640 x 21 targets (26 MB per sample): training only, off by default
             hw21 = torch.stack([it["keypoint_uv21"][..., 1], it["keypoint_uv21"][..., 0]], -1).contiguous()
             d["scoremap"] = ctx.gaussian_scoremap(hw21, self.image_size, self.sigma, it["keypoint_vis21"])

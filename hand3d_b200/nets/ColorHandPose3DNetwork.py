@@ -61,6 +61,59 @@ def _train_pose2d(image_crop, num_kp):
     return scoremap_list
 
 
+def _train_evaluation(evaluation):
+    if not _truthy(evaluation):
+        raise NotImplementedError("train=True needs evaluation=True: dropout is not implemented (training_lifting.py never feeds "
+                                  "`evaluation`, so its dropout is the identity too)")
+
+
+def _train_lift_input(pooled, hand_side):
+    return pooled.to(torch.float32).contiguous(), hand_side.to(torch.float32).contiguous()
+
+
+def _train_fc_stack(x, hand_side, v, scope, names, prec):
+    """Flatten (NHWC order, as tf.reshape), concat hand_side, then the leaky FC layers `names` (nets/PosePriorNetwork.py:110-114)."""
+    x = torch.cat([x.reshape(x.shape[0], -1), hand_side], 1)
+    for name in names:
+        x = A.fully_connected(x, v["%s/%s/weights" % (scope, name)], v["%s/%s/biases" % (scope, name)], True, prec)
+    return x
+
+
+def _train_pose3d_can(pooled, hand_side, bottleneck=False):
+    """PosePrior (nets/PosePriorNetwork.py:97-122) over ctx.variables('PosePrior'): [B,32,32,21], [B,2] -> [B,21,3].  Dropout is the
+    identity: training_lifting.py never feeds `evaluation`, whose default is True."""
+    _, v, prec = _train_scope("PosePrior")
+    has_bn = "PosePrior/fc_bottleneck/weights" in v
+    if bottleneck != has_bn:
+        raise ValueError("the %s PosePrior needs %s fc_bottleneck layer in the loaded weights" % (
+            "'bottleneck'" if bottleneck else "non-bottleneck", "an" if bottleneck else "no"))
+    pooled, hand_side = _train_lift_input(pooled, hand_side)
+    x = _train_layers(pooled, v, "PosePrior", arch.POSEPRIOR[:6], (), prec)
+    x = _train_fc_stack(x, hand_side, v, "PosePrior", ("fc_rel0", "fc_rel1"), prec)
+    if bottleneck:
+        x = A.fully_connected(x, v["PosePrior/fc_bottleneck/weights"], v["PosePrior/fc_bottleneck/biases"], False, prec)
+    x = A.fully_connected(x, v["PosePrior/fc_xyz/weights"], v["PosePrior/fc_xyz/biases"], False, prec)
+    return x.view(x.shape[0], 21, 3)
+
+
+def _train_viewpoint_u(pooled, hand_side):
+    """ViewpointNet (nets/PosePriorNetwork.py:136-159) over ctx.variables('ViewpointNet') -> uxyz [B,3].  The three 128 -> 1 heads
+    run as one 128 -> 3 layer whose weights are the concatenation of the three variables."""
+    _, v, prec = _train_scope("ViewpointNet")
+    pooled, hand_side = _train_lift_input(pooled, hand_side)
+    x = _train_layers(pooled, v, "ViewpointNet", arch.VIEWPOINT[:6], (), prec)
+    x = _train_fc_stack(x, hand_side, v, "ViewpointNet", ("fc_vp0", "fc_vp1"), prec)
+    heads = ["ViewpointNet/fc_vp_u%s" % a for a in "xyz"]
+    w = torch.cat([v[h + "/weights"] for h in heads], 1)
+    b = torch.cat([v[h + "/biases"] for h in heads], 0)
+    return A.fully_connected(x, w, b, False, prec)
+
+
+def _train_rotate(can, u, hand_side):
+    """(R, out) of the 'proposed' lifting: Rodrigues, right-hand flip, out = flip(can) R."""
+    return A.rotate_canonical(can, u, hand_side.to(torch.float32))
+
+
 class ColorHandPose3DNetwork(object):
     """ Network performing 3D pose estimation of a human hand from a single color image. """
     def __init__(self):
@@ -137,17 +190,32 @@ class ColorHandPose3DNetwork(object):
         return runtime.default_context().posenet(image_crop)
 
     def _inference_pose3d(self, keypoints_scoremap, hand_side, evaluation=True, train=False):
-        """ PosePrior + Viewpoint (reference :221-247): [B,32,32,21], [B,2] -> [B,21,3]. """
-        if not _truthy(evaluation) or train:
-            raise NotImplementedError("forward pass only")
+        """ PosePrior + Viewpoint (reference :221-247): [B,32,32,21], [B,2] -> [B,21,3].
+
+            train=True builds the graph from hand3d_b200.autograd over ctx.variables('PosePrior') and ctx.variables('ViewpointNet').
+            evaluation=False (dropout) is not supported.
+        """
+        if not _truthy(evaluation):
+            raise NotImplementedError("forward pass only: evaluation must be True (dropout is the identity)")
+        if train:
+            can = _train_pose3d_can(keypoints_scoremap, hand_side)
+            return _train_rotate(can, _train_viewpoint_u(keypoints_scoremap, hand_side), hand_side)[1]
         return runtime.default_context().lifting(keypoints_scoremap, hand_side, "proposed")[0]
 
     def _inference_pose3d_can(self, keypoints_scoremap, hand_side, evaluation=True, train=False):
         """ Canonical coordinates (reference :249-272). """
+        if train:
+            _train_evaluation(evaluation)
+            return _train_pose3d_can(keypoints_scoremap, hand_side)
         return runtime.default_context().lifting(keypoints_scoremap, hand_side, "proposed")[1]
 
     def _inference_viewpoint(self, keypoints_scoremap, hand_side, evaluation=True, train=False):
         """ Viewpoint rotation matrix (reference :274-283). """
+        if train:
+            _train_evaluation(evaluation)
+            u = _train_viewpoint_u(keypoints_scoremap, hand_side)
+            zeros = torch.zeros((u.shape[0], 21, 3), dtype=torch.float32, device=u.device)
+            return _train_rotate(zeros, u, hand_side)[0]
         return runtime.default_context().lifting(keypoints_scoremap, hand_side, "proposed")[2]
 
     def _get_rot_mat(self, ux_b, uy_b, uz_b):

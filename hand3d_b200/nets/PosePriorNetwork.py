@@ -9,7 +9,7 @@ import os
 
 import torch
 
-from .. import runtime, weights as _weights
+from .. import autograd as A, runtime, weights as _weights
 
 
 class PosePriorNetwork(object):
@@ -35,16 +35,22 @@ class PosePriorNetwork(object):
                 ctx.load_weights(wd)
                 print('Loaded %d variables from %s' % (len(wd), file_name))
 
-    def inference(self, scoremap, hand_side, evaluation=True):
+    def inference(self, scoremap, hand_side, evaluation=True, train=False):
         """ Infere 3D coordinates from 2D scoremaps (reference :59-95).
 
             scoremap [B,256,256,21] -> avg_pool 8x8 -> variant.  Returns (coord_xyz_rel_normed, coord3d, R).
+
+            train=True builds the graph from hand3d_b200.autograd over ctx.variables('PosePrior') (and ctx.variables('ViewpointNet')
+            for 'proposed'), as the reference's own inference() does with trainable variables (training_lifting.py:54): a loss of
+            coord3d, R or coord_xyz_rel_normed back-propagates into those Parameters.  The 8x8 average pool takes no gradient.
         """
         ev = bool(evaluation.item()) if torch.is_tensor(evaluation) else bool(evaluation)
         if not ev:
             raise NotImplementedError("forward pass only: evaluation must be True")
         ctx = runtime.default_context()
         scoremap_pooled = ctx.avg_pool8(scoremap)                       # :61
+        if train:
+            return self._train_inference(scoremap_pooled, hand_side)
         if self.variant in ('direct', 'bottleneck'):
             c, _, _ = ctx.lifting(scoremap_pooled, hand_side, self.variant)
             return c, c, None
@@ -54,6 +60,21 @@ class PosePriorNetwork(object):
             return normed, rel, None
         elif self.variant == 'proposed':
             out, can, R = ctx.lifting(scoremap_pooled, hand_side, 'proposed')
+            return out, can, R
+        else:
+            assert 0, "Unknown variant."
+
+    def _train_inference(self, scoremap_pooled, hand_side):
+        from .ColorHandPose3DNetwork import _train_pose3d_can, _train_rotate, _train_viewpoint_u
+        if self.variant in ('direct', 'bottleneck'):
+            c = _train_pose3d_can(scoremap_pooled, hand_side, bottleneck=self.variant == 'bottleneck')
+            return c, c, None
+        elif self.variant in ('local', 'local_w_xyz_loss'):
+            rel = _train_pose3d_can(scoremap_pooled, hand_side)
+            return A.bone_rel_trafo_inv(rel), rel, None
+        elif self.variant == 'proposed':
+            can = _train_pose3d_can(scoremap_pooled, hand_side)
+            R, out = _train_rotate(can, _train_viewpoint_u(scoremap_pooled, hand_side), hand_side)
             return out, can, R
         else:
             assert 0, "Unknown variant."

@@ -105,7 +105,11 @@ class Context:
             _lib.check(rc, "h3d_load_weight(%s)" % name)
             self.weights[name] = a
             self.__dict__.get("_dev_w", {}).pop(name, None)    # the operator-level device copy follows the reload
-            var = self.__dict__.get("_variables", {}).get(name.split("/")[0])
+            scope = name.split("/")[0]
+            var = self.__dict__.get("_variables", {}).get(scope)
+            if var is not None and name in var and tuple(var[name].shape) != a.shape:
+                del self._variables[scope]    # fc_xyz changed between 512 x 63 and 30 x 63 (fc_bottleneck): new Parameters next time
+                var = None
             if var is not None and name in var:   # so do the trainable variables: in place, so an optimiser over them stays valid
                 with torch.no_grad():
                     var[name].copy_(torch.from_numpy(a))
@@ -385,17 +389,21 @@ class Context:
 
     # ---- training (h3d_resize_bilinear_tf1_backward, the two losses, Adam) ----------------------
     def variables(self, scope):
-        """Ordered {reference variable name: torch.nn.Parameter} of "HandSegNet" or "PoseNet2D" (layer order of the reference graph,
-        weights before biases): fp32 device copies of the host arrays load_weights keeps, created once per context and then shared by
+        """Ordered {reference variable name: torch.nn.Parameter} of "HandSegNet", "PoseNet2D", "PosePrior" (with fc_bottleneck when
+        the loaded fc_xyz is 30 x 63) or "ViewpointNet" (layer order of the reference graph, weights before biases): fp32 device copies of the host arrays load_weights keeps, created once per context and then shared by
         every train=True graph, so an optimiser over them trains the network in place.
 
         The inference path (train=False, pipeline(), the stage entries) keeps the weights last loaded, not these Parameters: call
         commit_variables(scope) to make it use the trained values.  A later load_weights of the scope writes the loaded values into
         the same Parameters in place, so an optimiser built over them keeps working (its m / v slots are not reset)."""
         from . import arch
-        layers = {"HandSegNet": arch.HANDSEGNET, "PoseNet2D": arch.POSENET2D}
+        layers = {"HandSegNet": arch.HANDSEGNET, "PoseNet2D": arch.POSENET2D, "PosePrior": list(arch.POSEPRIOR),
+                  "ViewpointNet": arch.VIEWPOINT}
         if scope not in layers:
-            raise ValueError("variables(): scope must be 'HandSegNet' or 'PoseNet2D', got %r" % (scope,))
+            raise ValueError("variables(): scope must be 'HandSegNet', 'PoseNet2D', 'PosePrior' or 'ViewpointNet', got %r" % (scope,))
+        xyz = self.weights.get("PosePrior/fc_xyz/weights")
+        if scope == "PosePrior" and xyz is not None and xyz.shape[0] == 30:      # the 'bottleneck' variant: 512 -> 30 -> 63
+            layers["PosePrior"].insert(8, arch.POSEPRIOR_BOTTLENECK)
         cache = self.__dict__.setdefault("_variables", {})
         if scope not in cache:
             names = ["%s/%s/%s" % (scope, l[0], what) for l in layers[scope] for what in ("weights", "biases")]
@@ -626,6 +634,69 @@ class Context:
         _lib.check(self.lib.h3d_rotate_canonical(self.h, _ptr(coord_can), _ptr(uxyz), _ptr(hand_side), B, _ptr(rot), _ptr(out),
                                                  _stream()), "h3d_rotate_canonical")
         return rot, out
+
+    # ---- lifting training (h3d_rotate_canonical_backward, h3d_bone_rel_trafo*, h3d_mse_loss_*) --------------------------------
+    def rotate_canonical_backward(self, coord_can, uxyz, hand_side, d_out=None, d_rot=None):
+        """Gradient of rotate_canonical -> (d_can [B,21,3], d_uxyz [B,3]); d_out [B,21,3] and d_rot [B,3,3] may be None (= 0)."""
+        coord_can = _chk_f32(coord_can, "coord_can", 3); uxyz = _chk_f32(uxyz, "uxyz", 2); hand_side = _chk_f32(hand_side, "hand_side", 2)
+        B = coord_can.shape[0]
+        if tuple(coord_can.shape) != (B, 21, 3) or tuple(uxyz.shape) != (B, 3) or tuple(hand_side.shape) != (B, 2):
+            raise ValueError("rotate_canonical_backward: expects can [B,21,3], uxyz [B,3], hand_side [B,2], got %s, %s, %s"
+                             % (tuple(coord_can.shape), tuple(uxyz.shape), tuple(hand_side.shape)))
+        d_out = _chk_f32(d_out.reshape(B, 21, 3), "d_out") if d_out is not None else None
+        d_rot = _chk_f32(d_rot.reshape(B, 3, 3), "d_rot") if d_rot is not None else None
+        d_can = torch.empty((B, 21, 3), dtype=torch.float32, device=coord_can.device)
+        d_u = torch.empty((B, 3), dtype=torch.float32, device=coord_can.device)
+        _lib.check(self.lib.h3d_rotate_canonical_backward(self.h, _ptr(coord_can), _ptr(uxyz), _ptr(hand_side), _ptr(d_out), _ptr(d_rot), B,
+                                                          _ptr(d_can), _ptr(d_u), _stream()), "h3d_rotate_canonical_backward")
+        return d_can, d_u
+
+    def _rel_arg(self, t, name):
+        t = _chk_f32(t, name)
+        if t.dim() == 2:
+            t = t.unsqueeze(0)
+        if t.dim() != 3 or tuple(t.shape[1:]) != (21, 3):
+            raise ValueError("%s must be [B,21,3] (or [21,3]), got %s" % (name, tuple(t.shape)))
+        return t
+
+    def bone_rel_trafo_inv_backward(self, coords_rel, d_xyz):
+        """Gradient of bone_rel_trafo_inv: coords_rel (its input), d_xyz [B,21,3] -> d_rel [B,21,3]."""
+        coords_rel = self._rel_arg(coords_rel, "coords_rel")
+        d_xyz = self._rel_arg(d_xyz, "d_xyz")
+        if d_xyz.shape != coords_rel.shape:
+            raise ValueError("bone_rel_trafo_inv_backward: d_xyz %s does not match coords_rel %s" % (tuple(d_xyz.shape), tuple(coords_rel.shape)))
+        d_rel = torch.empty_like(coords_rel)
+        _lib.check(self.lib.h3d_bone_rel_trafo_inv_backward(self.h, _ptr(coords_rel), _ptr(d_xyz), _ptr(d_rel), coords_rel.shape[0], _stream()),
+                   "h3d_bone_rel_trafo_inv_backward")
+        return d_rel
+
+    def bone_rel_trafo(self, coords_xyz):
+        """utils/relative_trafo.py:184-240: xyz [B,21,3] -> (length, angle_x, angle_y) [B,21,3]."""
+        coords_xyz = self._rel_arg(coords_xyz, "coords_xyz")
+        rel = torch.empty_like(coords_xyz)
+        _lib.check(self.lib.h3d_bone_rel_trafo(self.h, _ptr(coords_xyz), _ptr(rel), coords_xyz.shape[0], _stream()), "h3d_bone_rel_trafo")
+        return rel
+
+    def _mse_args(self, pred, target):
+        pred = _chk_f32(pred, "pred"); target = _chk_f32(target, "target")
+        if tuple(pred.shape) != tuple(target.shape) or pred.numel() == 0:
+            raise ValueError("mse_loss: pred and target must have one non-empty shape, got %s and %s" % (tuple(pred.shape), tuple(target.shape)))
+        return pred, target
+
+    def mse_loss(self, pred, target):
+        """reduce_mean(square(pred - target)) -> 0-d device tensor."""
+        pred, target = self._mse_args(pred, target)
+        loss = torch.empty((), dtype=torch.float32, device=pred.device)
+        _lib.check(self.lib.h3d_mse_loss_forward(self.h, _ptr(pred), _ptr(target), pred.numel(), _ptr(loss), _stream()), "h3d_mse_loss_forward")
+        return loss
+
+    def mse_loss_backward(self, pred, target, grad_loss=None):
+        pred, target = self._mse_args(pred, target)
+        g = _chk_f32(grad_loss.reshape(()), "grad_loss") if grad_loss is not None else None
+        d = torch.empty_like(pred)
+        _lib.check(self.lib.h3d_mse_loss_backward(self.h, _ptr(pred), _ptr(target), _ptr(g), pred.numel(), _ptr(d), _stream()),
+                   "h3d_mse_loss_backward")
+        return d
 
 
 class PackedConv:

@@ -37,6 +37,25 @@ def synthetic_weights(seed: int = 0, bottleneck: bool = False, dtype=np.float32,
     return out
 
 
+def xavier_weights(seed: int = 0, scopes=("PosePrior", "ViewpointNet"), bottleneck: bool = False, dtype=np.float32):
+    """The reference's initialisers (utils/general.py:36-137), for a run that starts from tf.global_variables_initializer() as
+    training_lifting.py does: weights Xavier-uniform, U(-l, l) with l = sqrt(6 / (fan_in + fan_out)) (xavier_initializer_conv2d:
+    fan_in = k k Cin, fan_out = k k Cout; xavier_initializer: the FC's in and out sizes), biases 1e-4.  Only the distributions match:
+    the values come from numpy's generator seeded with `seed`, not from TF's random stream, which cannot be reproduced here."""
+    rng = np.random.default_rng(seed)
+    out = {}
+    for name, shape in arch.variable_shapes(bottleneck).items():
+        if name.split("/")[0] not in scopes:
+            continue
+        if name.endswith("/weights"):
+            rf = int(np.prod(shape[:-2])) if len(shape) > 2 else 1
+            limit = np.sqrt(6.0 / (rf * shape[-2] + rf * shape[-1]))
+            out[name] = rng.uniform(-limit, limit, size=shape).astype(dtype)
+        else:
+            out[name] = np.full(shape, 1e-4, dtype)
+    return out
+
+
 def load_weight_files(weight_files, exclude_var_list=None, verbose=True):
     """nets/ColorHandPose3DNetwork.py:42-59 (same asserts / messages, no TF session)."""
     if exclude_var_list is None:

@@ -336,6 +336,25 @@ H3D_API int h3d_adam_set_lr(h3d_ctx* ctx, float* state, float lr, void* stream);
 H3D_API int h3d_adam_step(h3d_ctx* ctx, const h3d_adam_tensor* table, int num_tensors, float* state, float beta1, float beta2,
                           float epsilon, void* stream);
 
+/* ---- Training of the lifting stage (training_lifting.py); the same conventions as the section above ---- */
+
+/* Adjoint of h3d_rotate_canonical (out = flip_z(can) R, R = Rodrigues(uxyz), the flip where argmax(hand_side) == 1): can [B,21,3],
+ * uxyz [B,3], hand_side [B,2], and the incoming gradients d_out [B,21,3] and d_R [B,3,3], either of which may be NULL (= 0) ->
+ * d_can [B,21,3], d_uxyz [B,3].  R is recomputed with the forward's own fp32 operations; the sum over the 21 key-points for dR runs
+ * in ascending order. */
+H3D_API int h3d_rotate_canonical_backward(h3d_ctx* ctx, const float* coord_can, const float* uxyz, const float* hand_side,
+                                          const float* d_out, const float* d_rot_mat, int B, float* d_can, float* d_uxyz, void* stream);
+/* Adjoint of h3d_bone_rel_trafo_inv: coords_rel [B,21,3] (the forward's input), d_xyz [B,21,3] -> d_rel [B,21,3]. */
+H3D_API int h3d_bone_rel_trafo_inv_backward(h3d_ctx* ctx, const float* coords_rel, const float* d_xyz, float* d_rel, int B, void* stream);
+/* bone_rel_trafo (utils/relative_trafo.py:184-240): xyz [B,21,3] -> (length, angle_x, angle_y) [B,21,3] per bone, with the reference's
+ * own atan2 (atan(y / (x + 1e-8)) plus quadrant corrections).  The 'local' variant's training target. */
+H3D_API int h3d_bone_rel_trafo(h3d_ctx* ctx, const float* coords_xyz, float* coords_rel, int B, void* stream);
+/* reduce_mean(square(pred - target)) over n elements -> loss (device scalar). */
+H3D_API int h3d_mse_loss_forward(h3d_ctx* ctx, const float* pred, const float* target, int64_t n, float* loss, void* stream);
+/* Its gradient: dpred [n] = (grad_loss / n) (2 (pred - target)). */
+H3D_API int h3d_mse_loss_backward(h3d_ctx* ctx, const float* pred, const float* target, const float* grad_loss, int64_t n, float* dpred,
+                                  void* stream);
+
 #ifdef __cplusplus
 }
 #endif
