@@ -4,6 +4,7 @@ on-device decode (BinaryDbReader mirror) -> inference_detection(train=True) -> s
 with TF 1.3 semantics, loss prints every show_loss_freq and pickled snapshots every snapshot_freq iterations.
 
     python examples/train_handsegnet_demo.py [--db data/bin/rhd_training.bin] [--weights handsegnet.pickle] [--iters 30]
+                                             [--augment [--seed S]]
 
 Without --db it trains on a few synthetic records (examples/_synthetic_db.py) and without --weights from synthetic_weights(0): the
 TF checkpoint the reference starts from (load_weights_from_snapshot, :73-75) is not read here.  Snapshots are in the reference's
@@ -38,6 +39,9 @@ if __name__ == '__main__':
     ap.add_argument("--show-loss-freq", type=int, default=5)
     ap.add_argument("--snapshot-freq", type=int, default=0, help="0: only the final snapshot")
     ap.add_argument("--snapshot-dir", default=train_para['snapshot_dir'])
+    ap.add_argument("--augment", action="store_true",
+                    help="read as training_handsegnet.py does: shuffled, hue augmentation, random 256x256 crops")
+    ap.add_argument("--seed", type=int, default=None, help="seed of the reader's shuffle and augmentation (default: OS entropy)")
     ap.add_argument("--advance-global-step", action="store_true",
                     help="advance the global step so that the learning-rate schedule takes effect (the reference never does)")
     args = ap.parse_args()
@@ -46,10 +50,15 @@ if __name__ == '__main__':
 
     path, tmp = db_path(args.db, "rhd", 16)
     try:
-        # training_handsegnet.py:37-39 reads with shuffle=True, hue_aug=True and random_crop_to_size=True.  Shuffling and augmentation
-        # are refused by the reader mirror (TF's random streams cannot be matched anyway), so this driver reads whole 320x320 images
-        # in file order.
-        dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=False, path_to_db=path)
+        # training_handsegnet.py:37-39 reads with shuffle=True, hue_aug=True and random_crop_to_size=True; --augment does the same
+        # (seeded draws, not TF's streams).  The default reads whole 320x320 images in file order, which the losses recorded in
+        # DESIGN.md section 6 were measured with.
+        if args.augment:
+            dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=True, hue_aug=True, random_crop_to_size=True, path_to_db=path,
+                                     seed=args.seed)
+            print('Reader seed:', dataset.seed)
+        else:
+            dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=False, path_to_db=path)
 
         net = ColorHandPose3DNetwork()
         if args.weights:

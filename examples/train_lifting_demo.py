@@ -5,7 +5,7 @@ PosePriorNetwork(variant).inference(train=True) -> the variant's MSE loss -> Ada
 show_loss_freq and pickled snapshots every snapshot_freq iterations.
 
     python examples/train_lifting_demo.py --variant {direct,bottleneck,local,local_w_xyz_loss,proposed} [--db rhd_training.bin]
-                                          [--iters 30]
+                                          [--iters 30] [--augment] [--seed S]
 
 Like the reference, it starts from the initialisers (weights.xavier_weights: Xavier-uniform weights, biases 1e-4; the same
 distributions as tf.global_variables_initializer(), not TF's random values), not from a pickle.  Without --db it trains on a few
@@ -39,7 +39,9 @@ if __name__ == '__main__':
     ap = argparse.ArgumentParser()
     ap.add_argument("--variant", default="proposed", choices=["direct", "bottleneck", "local", "local_w_xyz_loss", "proposed"])
     ap.add_argument("--db", default=None)
-    ap.add_argument("--seed", type=int, default=0, help="seed of the initialisers")
+    ap.add_argument("--seed", type=int, default=0, help="seed of the initialisers and, with --augment, of the reader")
+    ap.add_argument("--augment", action="store_true",
+                    help="read as training_lifting.py does: shuffled, with the coordinate and the three crop noises")
     ap.add_argument("--iters", type=int, default=30)
     ap.add_argument("--show-loss-freq", type=int, default=5)
     ap.add_argument("--snapshot-freq", type=int, default=0, help="0: only the final snapshot")
@@ -53,10 +55,13 @@ if __name__ == '__main__':
 
     path, tmp = db_path(args.db, "rhd", 16)
     try:
-        # training_lifting.py:44-46 reads with shuffle=True and four noise flags.  Shuffling and the noise flags are training-time
-        # augmentation, which the reader mirror refuses (TF's random streams cannot be matched anyway), so this driver reads in
-        # file order without noise.
-        dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=False, hand_crop=True, use_wrist_coord=False, path_to_db=path)
+        # training_lifting.py:44-46 reads with shuffle=True and four noise flags; --augment does the same (seeded draws, not TF's
+        # streams).  The default reads in file order without noise, as the losses recorded in DESIGN.md section 6 were measured.
+        if args.augment:
+            dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=True, hand_crop=True, use_wrist_coord=False, coord_uv_noise=True,
+                                     crop_center_noise=True, crop_offset_noise=True, crop_scale_noise=True, path_to_db=path, seed=args.seed)
+        else:
+            dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=False, hand_crop=True, use_wrist_coord=False, path_to_db=path)
 
         net = PosePriorNetwork(VARIANT)
         ctx = runtime.default_context()

@@ -5,6 +5,7 @@ up-sampling -> score-map loss -> Adam with TF 1.3 semantics, loss prints every s
 snapshot_freq iterations.
 
     python examples/train_posenet_demo.py [--db data/bin/rhd_training.bin] [--weights posenet.pickle] [--iters 30]
+                                          [--augment [--seed S]]
 
 Without --db it trains on a few synthetic records (examples/_synthetic_db.py) and without --weights from synthetic_weights(0): the
 TF checkpoint the reference starts from (load_weights_from_snapshot, :74-76) is not read here.  Snapshots are in the reference's
@@ -39,6 +40,9 @@ if __name__ == '__main__':
     ap.add_argument("--show-loss-freq", type=int, default=5)
     ap.add_argument("--snapshot-freq", type=int, default=0, help="0: only the final snapshot")
     ap.add_argument("--snapshot-dir", default=train_para['snapshot_dir'])
+    ap.add_argument("--augment", action="store_true",
+                    help="read as training_posenet.py does: shuffled, with coord_uv_noise and crop_center_noise")
+    ap.add_argument("--seed", type=int, default=None, help="seed of the reader's shuffle and augmentation (default: OS entropy)")
     ap.add_argument("--advance-global-step", action="store_true",
                     help="advance the global step so that the learning-rate schedule takes effect (the reference never does)")
     args = ap.parse_args()
@@ -47,10 +51,15 @@ if __name__ == '__main__':
 
     path, tmp = db_path(args.db, "rhd", 16)
     try:
-        # training_posenet.py:37-39 reads with shuffle=True, coord_uv_noise=True and crop_center_noise=True.  Shuffling and the noise
-        # flags are training-time augmentation, which the reader mirror refuses (TF's random streams cannot be matched anyway), so
-        # this driver reads in file order without noise.
-        dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=False, use_wrist_coord=False, hand_crop=True, path_to_db=path)
+        # training_posenet.py:37-39 reads with shuffle=True, coord_uv_noise=True and crop_center_noise=True; --augment does the same
+        # (seeded draws, not TF's streams).  The default reads in file order without noise, as the losses recorded in DESIGN.md
+        # section 6 were measured.
+        if args.augment:
+            dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=True, use_wrist_coord=False, hand_crop=True, coord_uv_noise=True,
+                                     crop_center_noise=True, path_to_db=path, seed=args.seed)
+            print('Reader seed:', dataset.seed)
+        else:
+            dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=False, use_wrist_coord=False, hand_crop=True, path_to_db=path)
 
         net = ColorHandPose3DNetwork()
         if args.weights:

@@ -66,6 +66,10 @@ SIGNATURES = {
     "h3d_rhd_reader_items": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "h3d_stb_reader_items": (_i, [_p, _p, _i, _i, _p, _p, _p, _p, _p, _p]),
     "h3d_gaussian_scoremap": (_i, [_p, _p, _p, _i, _i, _i, _i, _f, _p, _p]),
+    "h3d_reader_aug_params": (_i, [_p, _p, _i, C.c_uint64, _i, _p, _p]),
+    "h3d_augment_image": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
+    "h3d_rhd_reader_items_aug": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "h3d_gaussian_scoremap_dropout": (_i, [_p, _p, _p, _p, _i, _f, _i, _i, _i, _i, _f, _p, _p]),
     "h3d_canonical_trafo": (_i, [_p, _p, _p, _i, _p, _p, _p, _p]),
     "h3d_eval_keypoint_dist": (_i, [_p, _p, _p, _p, _i, _i, _p, _p]),
     "h3d_bone_rel_trafo_inv": (_i, [_p, _p, _p, _i, _p]),
@@ -86,6 +90,10 @@ SIGNATURES = {
     "h3d_mse_loss_backward": (_i, [_p, _p, _p, _p, _i64, _p, _p]),
 }
 ADAM_STATE_WORDS = 4   # H3D_ADAM_STATE_WORDS
+# training-mode reader augmentation (H3D_AUG_*): flags, and the per-sample parameter layout
+AUG_COORD_UV_NOISE, AUG_CROP_CENTER_NOISE, AUG_CROP_SCALE_NOISE, AUG_CROP_OFFSET_NOISE, AUG_HUE, AUG_RANDOM_CROP, AUG_SCOREMAP_DROPOUT = 1, 2, 4, 8, 16, 32, 64
+AUG_STREAM_ITEMS, AUG_STREAM_SHUFFLE, AUG_MAX_ATTEMPTS = 0, 1, 16
+AUG_UV_NOISE, AUG_CENTER_NOISE, AUG_SCALE, AUG_OFFSET_NOISE, AUG_HUE_DELTA, AUG_WINDOW, AUG_KEEP, AUG_USED, AUG_PARAMS = 0, 84, 86, 87, 89, 90, 92, 113, 128
 
 _lib = None
 

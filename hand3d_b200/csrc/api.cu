@@ -1025,7 +1025,7 @@ static int check_device() {
 extern "C" {
 
 const char* h3d_last_error(void) { return g_err; }
-int h3d_version(void) { return 100; }
+int h3d_version(void) { return 101; }
 
 int h3d_device_available(void) {
     int n = 0;
@@ -1719,6 +1719,44 @@ int h3d_gaussian_scoremap(h3d_ctx* ctx, const float* coords_hw, const uint8_t* v
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(coords_hw && scoremap && B > 0 && H > 0 && W > 0 && sigma > 0.f, "h3d_gaussian_scoremap: bad argument");
     int rc = launch_gaussian_map(coords_hw, valid, B, N, H, W, sigma, scoremap, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_reader_aug_params(h3d_ctx* ctx, const int64_t* serials, int B, uint64_t seed, int flags, float* params, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(serials && params && B > 0 && (flags & ~127) == 0, "h3d_reader_aug_params: bad argument");
+    int rc = launch_reader_aug_params(serials, B, seed, flags, params, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_augment_image(h3d_ctx* ctx, const float* image, const uint8_t* hand_parts, const float* params, int B, int H, int W, int flags,
+                      int window, float* out_image, int32_t* out_parts, int32_t* out_mask, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(image && out_image && B > 0 && H > 0 && W > 0 && (flags & ~(H3D_AUG_HUE | H3D_AUG_RANDOM_CROP)) == 0, "h3d_augment_image: bad argument");
+    H3D_REQUIRE(params || !flags, "h3d_augment_image: flags need params");
+    H3D_REQUIRE(hand_parts || (!out_parts && !out_mask), "h3d_augment_image: part / mask windows need hand_parts");
+    int rc = launch_augment_image(image, hand_parts, params, B, H, W, flags, window, out_image, out_parts, out_mask, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_rhd_reader_items_aug(h3d_ctx* ctx, const float* header, const uint8_t* hand_parts, const uint8_t* visibility, int B, int use_wrist_coord,
+                             int hand_crop, int crop_size, const float* params, int flags, float* keypoint_uv, float* keypoint_xyz21,
+                             float* keypoint_uv21, uint8_t* keypoint_vis21, float* hand_side, float* keypoint_scale, float* keypoint_xyz21_normed,
+                             float* crop_center, float* crop_scale, float* cam_mat, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(header && hand_parts && visibility && hand_side && B > 0 && crop_size > 1, "h3d_rhd_reader_items_aug: bad argument");
+    const int noise = H3D_AUG_COORD_UV_NOISE | H3D_AUG_CROP_CENTER_NOISE | H3D_AUG_CROP_SCALE_NOISE | H3D_AUG_CROP_OFFSET_NOISE;
+    H3D_REQUIRE((flags & ~noise) == 0, "h3d_rhd_reader_items_aug: flags other than the coordinate / crop noises");
+    int rc = launch_rhd_items(header, hand_parts, visibility, B, use_wrist_coord, hand_crop, crop_size, keypoint_xyz21, keypoint_uv21, keypoint_vis21,
+                              hand_side, keypoint_scale, keypoint_xyz21_normed, crop_center, crop_scale, cam_mat, s, params, flags, keypoint_uv);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_gaussian_scoremap_dropout(h3d_ctx* ctx, const float* coords_hw, const uint8_t* valid, const float* keep, int keep_stride, float keep_prob,
+                                  int B, int N, int H, int W, float sigma, float* scoremap, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(coords_hw && keep && scoremap && B > 0 && H > 0 && W > 0 && sigma > 0.f, "h3d_gaussian_scoremap_dropout: bad argument");
+    int rc = launch_gaussian_map(coords_hw, valid, B, N, H, W, sigma, scoremap, s, keep, keep_stride, keep_prob);
     if (!rc) ctx->launches += 1;
     return rc;
 }

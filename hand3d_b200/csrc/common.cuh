@@ -128,10 +128,15 @@ int launch_rotate_canonical(const float* coord_can, const float* uxyz, const flo
 // ---------------------------------------------------------------- kernels (reader.cu): the dataset readers' forward generators
 int launch_rhd_items(const float* header, const uint8_t* parts, const uint8_t* vis, int B, int use_wrist, int hand_crop, int crop_size,
                      float* xyz21, float* uv21, uint8_t* vis21, float* hand_side, float* kp_scale, float* xyz21_normed, float* crop_center,
-                     float* crop_scale, float* cam_mat, cudaStream_t s);
+                     float* crop_scale, float* cam_mat, cudaStream_t s, const float* params = nullptr, int flags = 0, float* uv42 = nullptr);
 int launch_stb_items(const float* header, int B, int use_wrist, float* xyz21, float* uv21, uint8_t* vis21, float* kp_scale, float* xyz21_normed,
                      cudaStream_t s);
-int launch_gaussian_map(const float* coords_hw, const uint8_t* valid, int B, int N, int H, int W, float sigma, float* out, cudaStream_t s);
+int launch_gaussian_map(const float* coords_hw, const uint8_t* valid, int B, int N, int H, int W, float sigma, float* out, cudaStream_t s,
+                        const float* keep = nullptr, int keep_stride = 0, float keep_prob = 1.f);
+// (reader_aug.cu) training-mode augmentation of the RHD reader: per-sample parameters, hue + window crop
+int launch_reader_aug_params(const int64_t* serials, int B, uint64_t seed, int flags, float* params, cudaStream_t s);
+int launch_augment_image(const float* image, const uint8_t* parts, const float* params, int B, int H, int W, int flags, int window,
+                         float* out_image, int32_t* out_parts, int32_t* out_mask, cudaStream_t s);
 int launch_canonical_trafo(const float* xyz, const uint8_t* cond_right, int B, float* can, float* rot, float* rot_inv, cudaStream_t s);
 
 // ---------------------------------------------------------------- kernels (conv_direct.cu)

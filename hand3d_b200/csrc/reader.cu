@@ -1,4 +1,5 @@
-// Forward generators of the reference's dataset readers, on device (SURVEY.md 8(f) row 4; evaluation mode = no augmentation):
+// Forward generators of the reference's dataset readers, on device (SURVEY.md 8(f) row 4; the training-mode noises of rhd_items and the
+// score-map dropout read the per-sample parameters of reader_aug.cu, and are skipped, not applied as identities, when their flag is off):
 //   data/BinaryDbReader.py:139-162 palm substitution, :210-250 dominant hand / 21-key-point subsets / root-relative normalisation,
 //   :269-346 ground-truth hand crop (centre, size, scale, key-points and intrinsics in crop space), :413-459 score-map targets,
 //   data/BinaryDbReaderSTB.py:123-196 (mm -> m, convert_kp, wrist extrapolation), utils/canonical_trafo.py:20-162.
@@ -13,7 +14,8 @@ namespace h3d {
 __global__ void rhd_items_kernel(const float* __restrict__ header, const uint8_t* __restrict__ parts, const uint8_t* __restrict__ vis, int use_wrist,
                                  int hand_crop, int crop_size, float* __restrict__ xyz21, float* __restrict__ uv21, uint8_t* __restrict__ vis21,
                                  float* __restrict__ hand_side, float* __restrict__ kp_scale, float* __restrict__ xyz21_normed,
-                                 float* __restrict__ crop_center, float* __restrict__ crop_scale, float* __restrict__ cam_mat) {
+                                 float* __restrict__ crop_center, float* __restrict__ crop_scale, float* __restrict__ cam_mat,
+                                 const float* __restrict__ params, int flags, float* __restrict__ uv42) {
     const int b = blockIdx.x;
     const float* h = header + (int64_t)b * 219;
     __shared__ int s_left, s_right;
@@ -50,6 +52,10 @@ __global__ void rhd_items_kernel(const float* __restrict__ header, const uint8_t
             s_vis[a] = s_vis[a] | s_vis[c];
         }
     }
+    const float* prm = params ? params + (int64_t)b * H3D_AUG_PARAMS : nullptr;
+    if (flags & H3D_AUG_COORD_UV_NOISE)              // keypoint_uv += truncated_normal([42, 2], 0, 2.5) before the 21-subset (:160-164)
+        for (int i = 0; i < 84; ++i) s_uv[i] = __fadd_rn(s_uv[i], prm[H3D_AUG_UV_NOISE + i]);
+    if (uv42) for (int i = 0; i < 84; ++i) uv42[(int64_t)b * 84 + i] = s_uv[i];
     const bool left = s_left > s_right;              // 'greater': a tie selects the right hand (:226-231)
     const int o = left ? 0 : 21;
     hand_side[2 * b] = left ? 1.f : 0.f; hand_side[2 * b + 1] = left ? 0.f : 1.f;
@@ -73,6 +79,9 @@ __global__ void rhd_items_kernel(const float* __restrict__ header, const uint8_t
     if (hand_crop) {
         float c0 = v[12], c1 = u[12];                // crop centre = key-point 12 as (row, col) (:271)
         if (!(isfinite(c0) && isfinite(c1))) { c0 = 0.f; c1 = 0.f; }
+        if (flags & H3D_AUG_CROP_CENTER_NOISE) {     // moves the centre before the crop size is measured (:277-279)
+            c0 = __fadd_rn(c0, prm[H3D_AUG_CENTER_NOISE]); c1 = __fadd_rn(c1, prm[H3D_AUG_CENTER_NOISE + 1]);
+        }
         const float inf = __int_as_float(0x7f800000);
         float mn0 = inf, mn1 = inf, mx0 = -inf, mx1 = -inf;
         for (int k = 0; k < 21; ++k)
@@ -84,6 +93,10 @@ __global__ void rhd_items_kernel(const float* __restrict__ header, const uint8_t
         if (!isfinite(best)) best = 200.f;
         float sc = __fdiv_rn((float)crop_size, best);
         sc = fminf(fmaxf(sc, 1.f), 10.f);
+        if (flags & H3D_AUG_CROP_SCALE_NOISE) sc = __fmul_rn(sc, prm[H3D_AUG_SCALE]);        // scale *= U[1, 1.2) (:307)
+        if (flags & H3D_AUG_CROP_OFFSET_NOISE) {     // after the size is fixed: key-points may leave the crop (:310-312)
+            c0 = __fadd_rn(c0, prm[H3D_AUG_OFFSET_NOISE]); c1 = __fadd_rn(c1, prm[H3D_AUG_OFFSET_NOISE + 1]);
+        }
         if (crop_center) { crop_center[2 * b] = c0; crop_center[2 * b + 1] = c1; }
         if (crop_scale) crop_scale[b] = sc;
         const float half = (float)(crop_size / 2);
@@ -111,10 +124,12 @@ __global__ void rhd_items_kernel(const float* __restrict__ header, const uint8_t
 
 int launch_rhd_items(const float* header, const uint8_t* parts, const uint8_t* vis, int B, int use_wrist, int hand_crop, int crop_size,
                      float* xyz21, float* uv21, uint8_t* vis21, float* hand_side, float* kp_scale, float* xyz21_normed, float* crop_center,
-                     float* crop_scale, float* cam_mat, cudaStream_t s) {
+                     float* crop_scale, float* cam_mat, cudaStream_t s, const float* params, int flags, float* uv42) {
     H3D_REQUIRE((((uintptr_t)parts) & 3) == 0, "rhd_items: hand_parts must be 4-byte aligned");
+    H3D_REQUIRE(params || !(flags & (H3D_AUG_COORD_UV_NOISE | H3D_AUG_CROP_CENTER_NOISE | H3D_AUG_CROP_SCALE_NOISE | H3D_AUG_CROP_OFFSET_NOISE)),
+                "rhd_items: noise flags need params");
     rhd_items_kernel<<<B, 256, 0, s>>>(header, parts, vis, use_wrist, hand_crop, crop_size, xyz21, uv21, vis21, hand_side, kp_scale, xyz21_normed,
-                                       crop_center, crop_scale, cam_mat);
+                                       crop_center, crop_scale, cam_mat, params, flags, uv42);
     H3D_CHECK_LAUNCH();
     return H3D_OK;
 }
@@ -163,16 +178,20 @@ int launch_stb_items(const float* header, int B, int use_wrist, float* xyz21, fl
 // out[b, y, x, n] = exp(-((y - r_n)^2 + (x - c_n)^2) / sigma^2) * cond_n with (r_n, c_n) = int32(coords_hw[b, n]) and cond_n = valid_n and
 // 0 < r_n < H - 1 and 0 < c_n < W - 1 (data/BinaryDbReader.py:413-459).  HBM-write bound: one thread produces 4 consecutive floats of the
 // flattened (x, n) row -> 16-byte stores.
+// kDrop: TF 1.3 dropout with one keep bit per (sample, channel) and the reader's rescale, ((g / keep_prob) * bit) * keep_prob, fused
+// into the store (data/BinaryDbReader.py:362-365): the per-channel multiply costs no extra traffic.
 constexpr int kMaxGaussKp = 64;
+template <bool kDrop>
 __global__ void gaussian_map_kernel(const float* __restrict__ coords_hw, const uint8_t* __restrict__ valid, int N, int H, int W, float sigma2,
-                                    float* __restrict__ out) {
-    __shared__ float s_r[kMaxGaussKp], s_c[kMaxGaussKp], s_on[kMaxGaussKp];
+                                    float* __restrict__ out, const float* __restrict__ keep, int keep_stride, float keep_prob) {
+    __shared__ float s_r[kMaxGaussKp], s_c[kMaxGaussKp], s_on[kMaxGaussKp], s_keep[kMaxGaussKp];
     const int b = blockIdx.y;
     if (threadIdx.x < N) {
         const int n = threadIdx.x;
         const int r = (int)coords_hw[((int64_t)b * N + n) * 2], c = (int)coords_hw[((int64_t)b * N + n) * 2 + 1];   // tf.cast(float -> int32): truncation
         const bool on = (valid ? valid[(int64_t)b * N + n] != 0 : true) && r < H - 1 && r > 0 && c < W - 1 && c > 0;
         s_r[n] = (float)r; s_c[n] = (float)c; s_on[n] = on ? 1.f : 0.f;
+        if (kDrop) s_keep[n] = keep[(int64_t)b * keep_stride + n];
     }
     __syncthreads();
     const int row_elems = W * N;                     // multiple of 4 is required by the launcher
@@ -189,16 +208,20 @@ __global__ void gaussian_map_kernel(const float* __restrict__ coords_hw, const u
             const float dy = __fsub_rn((float)y, s_r[n]), dx = __fsub_rn((float)x, s_c[n]);
             const float dist = __fadd_rn(__fmul_rn(dy, dy), __fmul_rn(dx, dx));
             o4[j] = __fmul_rn(expf(__fdiv_rn(-dist, sigma2)), s_on[n]);
+            if (kDrop) o4[j] = __fmul_rn(__fmul_rn(__fdiv_rn(o4[j], keep_prob), s_keep[n]), keep_prob);
         }
         reinterpret_cast<float4*>(ob)[i] = make_float4(o4[0], o4[1], o4[2], o4[3]);
     }
 }
 
-int launch_gaussian_map(const float* coords_hw, const uint8_t* valid, int B, int N, int H, int W, float sigma, float* out, cudaStream_t s) {
+int launch_gaussian_map(const float* coords_hw, const uint8_t* valid, int B, int N, int H, int W, float sigma, float* out, cudaStream_t s,
+                        const float* keep, int keep_stride, float keep_prob) {
     H3D_REQUIRE(N >= 1 && N <= kMaxGaussKp && ((W * N) & 3) == 0, "gaussian_scoremap: N must be in [1,64] and W * N a multiple of 4");
+    H3D_REQUIRE(!keep || (keep_stride >= N && keep_prob > 0.f && keep_prob <= 1.f), "gaussian_scoremap: keep_stride < N or keep_prob outside (0, 1]");
     const int64_t total = (int64_t)H * (W * N / 4);
     dim3 grid((unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div64(total, 256), 132 * 8 / std::max(1, std::min(B, 8)))), B);
-    gaussian_map_kernel<<<grid, 256, 0, s>>>(coords_hw, valid, N, H, W, sigma * sigma, out);
+    if (keep) gaussian_map_kernel<true><<<grid, 256, 0, s>>>(coords_hw, valid, N, H, W, sigma * sigma, out, keep, keep_stride, keep_prob);
+    else gaussian_map_kernel<false><<<grid, 256, 0, s>>>(coords_hw, valid, N, H, W, sigma * sigma, out, nullptr, 0, 1.f);
     H3D_CHECK_LAUNCH();
     return H3D_OK;
 }

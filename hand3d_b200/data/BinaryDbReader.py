@@ -1,9 +1,20 @@
-"""BinaryDbReader / BinaryDbReaderSTB -- H100-native mirrors of the reference's dataset readers for the EVALUATION drivers
-(data/BinaryDbReader.py:21-412, data/BinaryDbReaderSTB.py:21-330): same constructor arguments, `num_samples`, and `get()`
-returning the same dictionary keys, but eager: every get() call uploads the next `batch_size` fixed-length records as bytes and
-produces the raw and derived items on the GPU (h3d_decode_records, h3d_rhd_reader_items / h3d_stb_reader_items,
-h3d_crop_image_from_xy, h3d_gaussian_scoremap, h3d_canonical_trafo).  Training-time augmentation (hue, coordinate / crop noise,
-score-map dropout, random crops, shuffling) is out of scope and refused.
+"""BinaryDbReader / BinaryDbReaderSTB -- H100-native mirrors of the reference's dataset readers (data/BinaryDbReader.py:21-412,
+data/BinaryDbReaderSTB.py:21-330): same constructor arguments, `num_samples`, and `get()` returning the same dictionary keys, but
+eager: every get() call uploads the next `batch_size` fixed-length records as bytes and produces the raw and derived items on the GPU
+(h3d_decode_records, h3d_rhd_reader_items / h3d_stb_reader_items, h3d_crop_image_from_xy, h3d_gaussian_scoremap,
+h3d_canonical_trafo).
+
+The RHD reader also runs in training mode, as training_handsegnet.py, training_posenet.py and training_lifting.py build it:
+`shuffle=True` and the seven augmentation flags (hue_aug, coord_uv_noise, crop_center_noise, crop_scale_noise, crop_offset_noise,
+scoremap_dropout, random_crop_to_size) in the reference's order (data/BinaryDbReader.py:160-401).  TF's random streams cannot be
+reproduced, so the draws are the project's own: every random value is a pure function of (seed, serial, value), where `serial` is
+the sample's position in the enqueue stream (record = serial mod records in the file), computed on the device with Philox4x64-10
+(h3d_reader_aug_params; layouts in include/hand3d_b200.h).  The deterministic transforms given those draws follow the reference
+exactly.  `seed=None` draws a seed from OS entropy; `reader.seed` replays a run.  `shuffle=True` is the steady state of
+shuffle_batch_join(capacity=100, min_after_dequeue=50): a buffer of the next 100 stream positions, each dequeue taking a uniformly
+random slot that the stream then refills -- a windowed shuffle, not a permutation of the file.  A flag that is off is skipped, so
+with all flags off the items are bit-identical to the evaluation path.  STB keeps refusing augmentation and shuffling: no training
+script reads it.
 """
 from __future__ import annotations
 
@@ -12,10 +23,14 @@ import os
 import numpy as np
 import torch
 
-from .. import runtime
+from .. import _lib, runtime
 from .records import RHD_RECORD_BYTES, STB_RECORD_BYTES
 
 _AUG = ("random_crop_to_size", "hue_aug", "coord_uv_noise", "crop_center_noise", "crop_scale_noise", "crop_offset_noise", "scoremap_dropout")
+_AUG_BITS = {"coord_uv_noise": _lib.AUG_COORD_UV_NOISE, "crop_center_noise": _lib.AUG_CROP_CENTER_NOISE, "crop_scale_noise": _lib.AUG_CROP_SCALE_NOISE,
+             "crop_offset_noise": _lib.AUG_CROP_OFFSET_NOISE, "hue_aug": _lib.AUG_HUE, "random_crop_to_size": _lib.AUG_RANDOM_CROP,
+             "scoremap_dropout": _lib.AUG_SCOREMAP_DROPOUT}
+_ITEM_NOISE = _lib.AUG_COORD_UV_NOISE | _lib.AUG_CROP_CENTER_NOISE | _lib.AUG_CROP_SCALE_NOISE | _lib.AUG_CROP_OFFSET_NOISE
 
 
 class _RecordFile:
@@ -27,44 +42,105 @@ class _RecordFile:
         self.num_samples = min(num_samples, self.available) if self.available else num_samples
         self.pos = 0
 
-    def next_batch(self, n):
-        idx = [(self.pos + i) % max(1, self.available) for i in range(n)]       # the TF queue cycles through the file
-        self.pos += n
-        rec = np.stack([np.asarray(self.mm[i * self.record_bytes:(i + 1) * self.record_bytes]) for i in idx])
+    def gather(self, serials):
+        """The records at stream positions `serials`, uploaded: the TF queue cycles through the file, so record = serial mod count."""
+        n, rb = max(1, self.available), self.record_bytes
+        rec = np.stack([np.asarray(self.mm[(s % n) * rb:(s % n + 1) * rb]) for s in serials])
         dev = runtime.default_context().device
         return torch.from_numpy(rec).pin_memory().to(dev, non_blocking=True)
+
+    def next_batch(self, n):
+        serials = range(self.pos, self.pos + n)
+        self.pos += n
+        return self.gather(serials)
+
+
+class _ShuffleQueue:
+    """tf.train.shuffle_batch_join(capacity=100, min_after_dequeue=50) over the in-order record stream, in its steady state: the
+    buffer holds the next CAPACITY stream positions; each dequeue takes slot (w mod CAPACITY) and the stream refills it.  The words w
+    come from Philox4x64-10 keyed (seed, H3D_AUG_STREAM_SHUFFLE), one per dequeue in order (numpy.random.Philox, counter from 0),
+    so the sequence of serials depends on the seed only, not on how it is cut into batches."""
+    CAPACITY = 100
+
+    def __init__(self, seed):
+        self._bits = np.random.Philox(key=np.array([seed, _lib.AUG_STREAM_SHUFFLE], np.uint64))
+        self._slots = list(range(self.CAPACITY))
+        self._next = self.CAPACITY
+
+    def take(self, n):
+        out = []
+        for w in self._bits.random_raw(n):
+            k = int(w) % self.CAPACITY
+            out.append(self._slots[k])
+            self._slots[k] = self._next
+            self._next += 1
+        return out
 
 
 class BinaryDbReader(object):
     """ Reads data from a binary dataset created by create_binary_db.py (RHD). """
     def __init__(self, mode=None, batch_size=1, shuffle=True, use_wrist_coord=True, sigma=25.0, hand_crop=False, random_crop_to_size=False,
                  scale_to_size=False, hue_aug=False, coord_uv_noise=False, crop_center_noise=False, crop_scale_noise=False,
-                 crop_offset_noise=False, scoremap_dropout=False, path_to_db=None):
+                 crop_offset_noise=False, scoremap_dropout=False, path_to_db=None, seed=None):
         if mode == 'training':
             path, n = './data/bin/rhd_training.bin', 41258
         elif mode == 'evaluation':
             path, n = './data/bin/rhd_evaluation.bin', 2728
         else:
             assert 0, "Unknown dataset mode."
+        flags = 0
         for name in _AUG:
             if locals()[name]:
-                raise NotImplementedError("hand3d_b200 readers serve the evaluation drivers: %s is training-time augmentation" % name)
-        if shuffle:
-            raise NotImplementedError("shuffle=True (training) is out of scope; the evaluation drivers pass shuffle=False")
+                flags |= _AUG_BITS[name]
+        if scale_to_size:                  # random_crop_to_size is the elif branch after scale_to_size (:369-392)
+            flags &= ~_lib.AUG_RANDOM_CROP
+        if seed is None:                   # like TF's unseeded random ops; reader.seed replays the run
+            seed = int.from_bytes(os.urandom(8), "little")
+        if not 0 <= int(seed) < 2 ** 64:
+            raise ValueError("seed must be in [0, 2**64)")
         self._file = _RecordFile(path_to_db or path, RHD_RECORD_BYTES, n)
         self.path_to_db = path_to_db or path
         self.num_samples = self._file.num_samples
         self.batch_size, self.sigma, self.shuffle, self.use_wrist_coord = batch_size, sigma, shuffle, use_wrist_coord
         self.scale_to_size, self.scale_target_size, self.hand_crop = scale_to_size, (240, 320), hand_crop
         self.image_size, self.crop_size, self.num_kp = (320, 320), 256, 42
+        self.random_crop_size = 256
+        self.seed = int(seed)
+        self._flags = flags
+        self._queue = _ShuffleQueue(self.seed) if shuffle else None
+        self._next_serial = 0
 
     def get(self):
         """ Next batch as a dict of CUDA tensors with the reference's keys (data/BinaryDbReader.py:100-411). """
-        ctx = runtime.default_context()
         B = self.batch_size
-        raw = ctx.decode_records(self._file.next_batch(B), "rhd", 1)
+        if self._queue is not None:
+            serials = self._queue.take(B)
+        else:
+            serials = list(range(self._next_serial, self._next_serial + B))
+            self._next_serial += B
+        return self._get(serials)
+
+    def _get(self, serials, params=None):
+        """The samples at enqueue positions `serials`; `params` [B, H3D_AUG_PARAMS] replaces the drawn augmentation parameters."""
+        ctx = runtime.default_context()
+        B = len(serials)
+        flags = self._flags
+        raw = ctx.decode_records(self._file.gather(serials), "rhd", 1)
+        if flags and params is None:
+            params = ctx.reader_aug_params(torch.tensor(list(serials), dtype=torch.int64), self.seed, flags)
+        if flags & _lib.AUG_RANDOM_CROP:   # :382-392: only the three windows are kept, so nothing else is computed
+            img, parts, mask = ctx.augment_image(raw["image"], params, flags & (_lib.AUG_HUE | _lib.AUG_RANDOM_CROP), raw["mask"],
+                                                 self.random_crop_size)
+            return {"image": img, "hand_parts": parts, "hand_mask": mask}
         h = raw["header"]
-        it = ctx.rhd_reader_items(h, raw["mask"], raw["visibility"], self.use_wrist_coord, self.hand_crop, self.crop_size)
+        if flags:
+            it = ctx.rhd_reader_items_aug(h, raw["mask"], raw["visibility"], params, flags & _ITEM_NOISE, self.use_wrist_coord, self.hand_crop,
+                                          self.crop_size)
+        else:
+            it = ctx.rhd_reader_items(h, raw["mask"], raw["visibility"], self.use_wrist_coord, self.hand_crop, self.crop_size)
+        image = raw["image"]
+        if flags & _lib.AUG_HUE:           # :183-184, before image_crop is cut from it
+            image = ctx.augment_image(image, params, _lib.AUG_HUE)[0]
         xyz = h[:, :126].reshape(B, 42, 3)
         uv = h[:, 126:210].reshape(B, 42, 2).to(torch.int32).to(torch.float32)
         vis = raw["visibility"].to(torch.bool)
@@ -72,9 +148,11 @@ class BinaryDbReader(object):
             xyz = torch.cat([0.5 * (xyz[:, 0:1] + xyz[:, 12:13]), xyz[:, 1:21], 0.5 * (xyz[:, 21:22] + xyz[:, 33:34]), xyz[:, 22:]], 1)
             uv = torch.cat([0.5 * (uv[:, 0:1] + uv[:, 12:13]), uv[:, 1:21], 0.5 * (uv[:, 21:22] + uv[:, 33:34]), uv[:, 22:]], 1)
             vis = torch.cat([vis[:, 0:1] | vis[:, 12:13], vis[:, 1:21], vis[:, 21:22] | vis[:, 33:34], vis[:, 22:]], 1)
+        if flags:
+            uv = it["keypoint_uv"]         # palm-substituted on the device, + coord_uv_noise (:160-164)
         parts = raw["mask"].to(torch.int32)
         hand = parts > 1
-        d = {"keypoint_xyz": xyz, "keypoint_uv": uv, "cam_mat": it["cam_mat"], "image": raw["image"], "hand_parts": parts,
+        d = {"keypoint_xyz": xyz, "keypoint_uv": uv, "cam_mat": it["cam_mat"], "image": image, "hand_parts": parts,
              "hand_mask": torch.stack([~hand, hand], 3).to(torch.int32), "keypoint_vis": vis, "hand_side": it["hand_side"],
              "keypoint_xyz21": it["keypoint_xyz21"], "keypoint_scale": it["keypoint_scale"], "keypoint_xyz21_normed": it["keypoint_xyz21_normed"],
              "keypoint_vis21": it["keypoint_vis21"].to(torch.bool), "keypoint_uv21": it["keypoint_uv21"]}
@@ -85,13 +163,17 @@ class BinaryDbReader(object):
         size = self.image_size
         if self.hand_crop:
             d["crop_scale"] = it["crop_scale"]
-            d["image_crop"] = ctx.crop_image_from_xy(raw["image"], it["crop_center"], self.crop_size, it["crop_scale"])
+            d["image_crop"] = ctx.crop_image_from_xy(image, it["crop_center"], self.crop_size, it["crop_scale"])
             size = (self.crop_size, self.crop_size)
         hw21 = torch.stack([it["keypoint_uv21"][..., 1], it["keypoint_uv21"][..., 0]], -1).contiguous()
-        d["scoremap"] = ctx.gaussian_scoremap(hw21, size, self.sigma, it["keypoint_vis21"])
+        if flags & _lib.AUG_SCOREMAP_DROPOUT:      # :362-365
+            d["scoremap"] = ctx.gaussian_scoremap_dropout(hw21, size, self.sigma, it["keypoint_vis21"],
+                                                          params[:, _lib.AUG_KEEP:_lib.AUG_KEEP + 21], 0.8)
+        else:
+            d["scoremap"] = ctx.gaussian_scoremap(hw21, size, self.sigma, it["keypoint_vis21"])
         if self.scale_to_size:             # :368-381: everything else is dropped
             s = self.image_size
-            image = ctx.resize_bilinear(raw["image"], *self.scale_target_size)
+            image = ctx.resize_bilinear(image, *self.scale_target_size)
             sc = (self.scale_target_size[0] / float(s[0]), self.scale_target_size[1] / float(s[1]))
             uv21 = torch.stack([d["keypoint_uv21"][..., 0] * sc[1], d["keypoint_uv21"][..., 1] * sc[0]], -1)
             d = {"image": image, "keypoint_uv21": uv21, "keypoint_vis21": d["keypoint_vis21"]}
@@ -109,9 +191,9 @@ class BinaryDbReaderSTB(object):
             path, n = './data/stb/stb_eval.bin', 6000
         else:
             assert 0, "Unknown dataset mode."
-        for name in _AUG:
+        for name in _AUG:                  # no training script reads STB; its coord_uv_noise (:158-160) cannot build a graph either
             if locals().get(name):
-                raise NotImplementedError("hand3d_b200 readers serve the evaluation drivers: %s is training-time augmentation" % name)
+                raise NotImplementedError("BinaryDbReaderSTB serves the evaluation driver: %s is training-time augmentation" % name)
         if shuffle or hand_crop:
             raise NotImplementedError("shuffle / hand_crop on STB are training-time options; the evaluation driver (eval_full.py:45) uses neither")
         self._file = _RecordFile(path_to_db or path, STB_RECORD_BYTES, n)

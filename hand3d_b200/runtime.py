@@ -35,6 +35,15 @@ def _chk_f32(t, name, ndim=None):
     return t.contiguous()
 
 
+def _chk_params(params, B):
+    if params is None:
+        return None
+    params = _chk_f32(params, "params", 2)
+    if tuple(params.shape) != (B, _lib.AUG_PARAMS):
+        raise ValueError("params must be [%d, %d], got %s" % (B, _lib.AUG_PARAMS, tuple(params.shape)))
+    return params
+
+
 class Context:
     def __init__(self, device=None, precision="bf16x3"):
         self.lib = _lib.load()
@@ -593,6 +602,66 @@ class Context:
         out = torch.empty((B, H, W, N), dtype=torch.float32, device=coords_hw.device)
         _lib.check(self.lib.h3d_gaussian_scoremap(self.h, _ptr(coords_hw), _ptr(v), B, N, H, W, C.c_float(float(sigma)), _ptr(out), _stream()),
                    "h3d_gaussian_scoremap")
+        return out
+
+    def reader_aug_params(self, serials, seed, flags):
+        """Per-sample random parameters of the RHD reader's training augmentation: serials int64 [B] (enqueue positions) ->
+        params [B, _lib.AUG_PARAMS] fp32, a pure function of (seed, serial) for each flag in `flags` (the _lib.AUG_* bits)."""
+        serials = serials.to(device=self.device, dtype=torch.int64).contiguous()
+        B = serials.shape[0]
+        params = torch.empty((B, _lib.AUG_PARAMS), dtype=torch.float32, device=self.device)
+        _lib.check(self.lib.h3d_reader_aug_params(self.h, _ptr(serials), B, C.c_uint64(int(seed) & (2 ** 64 - 1)), int(flags), _ptr(params),
+                                                  _stream()), "h3d_reader_aug_params")
+        return params
+
+    def augment_image(self, image, params, flags, hand_parts=None, window=256):
+        """tf.image.random_hue and / or the random_crop window in one pass: image [B,H,W,3] -> image [B,h,w,3]; with
+        _lib.AUG_RANDOM_CROP in flags also the hand_parts [B,h,w] and hand_mask [B,h,w,2] int32 windows of hand_parts u8 [B,H,W]."""
+        image = _chk_f32(image, "image", 4)
+        B, H, W, _ = image.shape
+        crop = bool(flags & _lib.AUG_RANDOM_CROP)
+        oh, ow = (window, window) if crop else (H, W)
+        dev = image.device
+        out = torch.empty((B, oh, ow, 3), dtype=torch.float32, device=dev)
+        parts = mask = None
+        if crop and hand_parts is not None:
+            hand_parts = hand_parts.to(torch.uint8).contiguous()
+            parts = torch.empty((B, oh, ow), dtype=torch.int32, device=dev)
+            mask = torch.empty((B, oh, ow, 2), dtype=torch.int32, device=dev)
+        p = _chk_params(params, B)
+        _lib.check(self.lib.h3d_augment_image(self.h, _ptr(image), _ptr(hand_parts if parts is not None else None), _ptr(p), B, H, W,
+                                              int(flags), int(window), _ptr(out), _ptr(parts), _ptr(mask), _stream()), "h3d_augment_image")
+        return out, parts, mask
+
+    def rhd_reader_items_aug(self, header, hand_parts, visibility, params, flags, use_wrist_coord=True, hand_crop=False, crop_size=256):
+        """rhd_reader_items with the coordinate / crop noises of `flags` read from params; also returns keypoint_uv [B,42,2]."""
+        B = header.shape[0]
+        dev = header.device
+        f = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)      # noqa: E731
+        r = {"keypoint_uv": f(B, 42, 2), "keypoint_xyz21": f(B, 21, 3), "keypoint_uv21": f(B, 21, 2),
+             "keypoint_vis21": torch.empty((B, 21), dtype=torch.uint8, device=dev), "hand_side": f(B, 2), "keypoint_scale": f(B),
+             "keypoint_xyz21_normed": f(B, 21, 3), "cam_mat": f(B, 3, 3), "crop_center": f(B, 2) if hand_crop else None,
+             "crop_scale": f(B) if hand_crop else None}
+        p = _chk_params(params, B)
+        _lib.check(self.lib.h3d_rhd_reader_items_aug(
+            self.h, _ptr(header.contiguous()), _ptr(hand_parts.contiguous()), _ptr(visibility.contiguous()), B, int(bool(use_wrist_coord)),
+            int(bool(hand_crop)), int(crop_size), _ptr(p), int(flags), _ptr(r["keypoint_uv"]), _ptr(r["keypoint_xyz21"]), _ptr(r["keypoint_uv21"]),
+            _ptr(r["keypoint_vis21"]), _ptr(r["hand_side"]), _ptr(r["keypoint_scale"]), _ptr(r["keypoint_xyz21_normed"]), _ptr(r["crop_center"]),
+            _ptr(r["crop_scale"]), _ptr(r["cam_mat"]), _stream()), "h3d_rhd_reader_items_aug")
+        return r
+
+    def gaussian_scoremap_dropout(self, coords_hw, output_size, sigma, valid, keep, keep_prob=0.8):
+        """gaussian_scoremap followed by TF 1.3 dropout with per-(sample, key-point) keep bits and the reader's * keep_prob.
+        keep: fp32 [B, >= N] rows (a column slice of the augmentation parameters is fine: its row stride is used)."""
+        coords_hw = _chk_f32(coords_hw, "coords_hw", 3)
+        B, N, _ = coords_hw.shape
+        H, W = int(output_size[0]), int(output_size[1])
+        if keep.dtype != torch.float32 or keep.dim() != 2 or keep.shape[0] != B or keep.shape[1] < N or keep.stride(1) != 1:
+            raise ValueError("keep must be fp32 [B, >= N] with unit column stride")
+        v = valid.to(torch.uint8).contiguous() if valid is not None else None
+        out = torch.empty((B, H, W, N), dtype=torch.float32, device=coords_hw.device)
+        _lib.check(self.lib.h3d_gaussian_scoremap_dropout(self.h, _ptr(coords_hw), _ptr(v), _ptr(keep), int(keep.stride(0)), C.c_float(float(keep_prob)),
+                                                          B, N, H, W, C.c_float(float(sigma)), _ptr(out), _stream()), "h3d_gaussian_scoremap_dropout")
         return out
 
     def canonical_trafo(self, coords_xyz, cond_right=None):

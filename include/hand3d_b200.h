@@ -266,6 +266,62 @@ H3D_API int h3d_stb_reader_items(h3d_ctx* ctx, const float* header, int B, int u
  * (NULL = all valid) -> scoremap [B,H,W,N] = exp(-d^2 / sigma^2) for key-points strictly inside the map, 0 otherwise.  N <= 64. */
 H3D_API int h3d_gaussian_scoremap(h3d_ctx* ctx, const float* coords_hw, const uint8_t* valid, int B, int N, int H, int W, float sigma,
                                   float* scoremap, void* stream);
+/* ---- Training-mode augmentation of the RHD reader (data/BinaryDbReader.py:160-401 with its seven flags) ----
+ * Every random value is a pure function of (seed, serial, value id, attempt): serial is the sample's position in the ENQUEUE stream
+ * (record = serial mod records in the file), so a sample's augmentation depends neither on the batch size nor on the shuffle.
+ * Generator: Philox4x64-10 (Salmon et al., SC'11; numpy.random.Philox is the same function), key = (seed, H3D_AUG_STREAM_ITEMS),
+ * counter = (serial, value id, attempt, 0), four 64-bit words per call.  The value id is the parameter's index in the layout below.
+ *   uniform fp32 in [0, 1)   = (w0 >> 40) * 2^-24 (exact), then TF's random_uniform affine step u * (max - min) + min in fp32;
+ *   truncated normal         = Box-Muller in fp64 on (w0, w1) of attempt a = 0, 1, ...: z0 = r cos(2 pi u2), z1 = r sin(2 pi u2),
+ *                              u1 = ((w0 >> 11) + 1) 2^-53, u2 = (w1 >> 11) 2^-53; the first of z0, z1, z0', z1', ... with
+ *                              |z| <= 2 is kept (rounded to fp32), then TF's z * stddev + 0 in fp32; after H3D_AUG_MAX_ATTEMPTS
+ *                              attempts without one (probability ~1e-43) z = 0;
+ *   window offset in [0, 64] = w0 mod 65;  keep bit = floor(0.8f + u) in fp32 (TF 1.3 dropout, keep_prob 0.8).
+ * The shuffle queue's dequeue order is host logic on a separate key (seed, H3D_AUG_STREAM_SHUFFLE). */
+#define H3D_AUG_STREAM_ITEMS 0
+#define H3D_AUG_STREAM_SHUFFLE 1
+#define H3D_AUG_MAX_ATTEMPTS 16
+/* flags */
+#define H3D_AUG_COORD_UV_NOISE 1     /* truncated normal, sigma 2.5 px, on the 42 palm-substituted keypoint_uv (:160-164) */
+#define H3D_AUG_CROP_CENTER_NOISE 2  /* truncated normal, sigma 20 px, on the crop centre before the crop size (:277-279) */
+#define H3D_AUG_CROP_SCALE_NOISE 4   /* U[1, 1.2) factor on the clamped crop scale (:281-283, 307) */
+#define H3D_AUG_CROP_OFFSET_NOISE 8  /* truncated normal, sigma 10 px, on the crop centre after the crop size (:310-312) */
+#define H3D_AUG_HUE 16               /* tf.image.random_hue(image, 0.1) on image / 255 - 0.5 (:183-184) */
+#define H3D_AUG_RANDOM_CROP 32       /* one 256 x 256 window of image, hand_parts, hand_mask, offsets in [0, 64] (:382-392) */
+#define H3D_AUG_SCOREMAP_DROPOUT 64  /* per key-point keep bits, keep 0.8, then * 0.8 (:362-365) */
+/* per-sample parameter layout: params [B, H3D_AUG_PARAMS] fp32, FINAL values (px, factors, offsets, bits), not standard draws */
+#define H3D_AUG_UV_NOISE 0           /* [42][2] (u, v) px */
+#define H3D_AUG_CENTER_NOISE 84      /* [2] (row, col) px */
+#define H3D_AUG_SCALE 86             /* [1] factor in [1, 1.2) */
+#define H3D_AUG_OFFSET_NOISE 87      /* [2] (row, col) px */
+#define H3D_AUG_HUE_DELTA 89         /* [1] in [-0.1, 0.1) */
+#define H3D_AUG_WINDOW 90            /* [2] (row, col) offsets, integers in [0, 64] stored as floats */
+#define H3D_AUG_KEEP 92              /* [21] 0 or 1 */
+#define H3D_AUG_USED 113
+#define H3D_AUG_PARAMS 128
+/* serials [B] int64 (device) -> params [B, H3D_AUG_PARAMS]: the final value of every flag in `flags`; a flag that is off gets its
+ * neutral value (0 px, factor 1, delta 0, offset 0, keep 1) and unused slots are 0. */
+H3D_API int h3d_reader_aug_params(h3d_ctx* ctx, const int64_t* serials, int B, uint64_t seed, int flags, float* params, void* stream);
+/* tf.image.random_hue (TF 1.3 adjust_hue, non-fused: rgb_to_hsv, h = mod(h + (delta + 1), 1), hsv_to_rgb, in the functors' fp32 order)
+ * and / or the random_crop window, in one pass.  image [B,H,W,3] fp32, hand_parts [B,H,W] u8, params as above (delta at
+ * H3D_AUG_HUE_DELTA when flags has H3D_AUG_HUE, window at H3D_AUG_WINDOW when flags has H3D_AUG_RANDOM_CROP) -> out_image [B,h,w,3]
+ * and, with the window, out_parts [B,h,w] int32 and out_mask [B,h,w,2] int32 (background, hand) (each may be NULL); (h, w) = (window,
+ * window) with H3D_AUG_RANDOM_CROP, else (H, W). */
+H3D_API int h3d_augment_image(h3d_ctx* ctx, const float* image, const uint8_t* hand_parts, const float* params, int B, int H, int W,
+                              int flags, int window, float* out_image, int32_t* out_parts, int32_t* out_mask, void* stream);
+/* h3d_rhd_reader_items with the coordinate and crop noises of `flags` (H3D_AUG_COORD_UV_NOISE, _CROP_CENTER_NOISE, _CROP_SCALE_NOISE,
+ * _CROP_OFFSET_NOISE) read from params [B, H3D_AUG_PARAMS]; params may be NULL when flags is 0, which computes exactly what
+ * h3d_rhd_reader_items computes.  keypoint_uv [B,42,2] (may be NULL) is the reader's keypoint_uv item: palm-substituted when
+ * use_wrist_coord == 0, noisy with H3D_AUG_COORD_UV_NOISE.  crop_center is the final centre (both noises applied). */
+H3D_API int h3d_rhd_reader_items_aug(h3d_ctx* ctx, const float* header, const uint8_t* hand_parts, const uint8_t* visibility, int B,
+                                     int use_wrist_coord, int hand_crop, int crop_size, const float* params, int flags,
+                                     float* keypoint_uv, float* keypoint_xyz21, float* keypoint_uv21, uint8_t* keypoint_vis21,
+                                     float* hand_side, float* keypoint_scale, float* keypoint_xyz21_normed, float* crop_center,
+                                     float* crop_scale, float* cam_mat, void* stream);
+/* h3d_gaussian_scoremap followed by TF 1.3 dropout with one keep bit per (sample, key-point) and the reader's rescale:
+ * out = ((map / keep_prob) * keep[b * keep_stride + n]) * keep_prob, each step rounded in fp32. */
+H3D_API int h3d_gaussian_scoremap_dropout(h3d_ctx* ctx, const float* coords_hw, const uint8_t* valid, const float* keep, int keep_stride,
+                                          float keep_prob, int B, int N, int H, int W, float sigma, float* scoremap, void* stream);
 /* canonical_trafo (+ flip_right_hand, + the tf.matrix_inverse the readers apply) (utils/canonical_trafo.py:97-162,
  * data/BinaryDbReader.py:247-252): coords_xyz [B,21,3] -> coords_can [B,21,3] (z mirrored where cond_right[b] != 0; cond_right may be
  * NULL), rot_mat [B,3,3] (total rotation), rot_mat_inv [B,3,3]; each output may be NULL. */
