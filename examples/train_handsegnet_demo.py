@@ -4,11 +4,13 @@ on-device decode (BinaryDbReader mirror) -> inference_detection(train=True) -> s
 with TF 1.3 semantics, loss prints every show_loss_freq and pickled snapshots every snapshot_freq iterations.
 
     python examples/train_handsegnet_demo.py [--db data/bin/rhd_training.bin] [--weights handsegnet.pickle] [--iters 30]
-                                             [--augment [--seed S]]
+                                             [--augment [--seed S]] [--device-resident [--graph]]
 
 Without --db it trains on a few synthetic records (examples/_synthetic_db.py) and without --weights from synthetic_weights(0): the
 TF checkpoint the reference starts from (load_weights_from_snapshot, :73-75) is not read here.  Snapshots are in the reference's
-weight-pickle layout (ColorHandPose3DNetwork().init(weight_files=[...]) loads them), not TF checkpoints.
+weight-pickle layout (ColorHandPose3DNetwork().init(weight_files=[...]) loads them), not TF checkpoints.  --device-resident keeps the
+records on the GPU; --graph then captures reading, the step and Adam once after two eager iterations and replays that CUDA graph for
+every later iteration.  Both print the losses of the plain run.
 """
 import argparse
 import os
@@ -21,6 +23,7 @@ from nets.ColorHandPose3DNetwork import ColorHandPose3DNetwork       # training_
 from utils.general import LearningRateScheduler                      # training_handsegnet.py:26
 from hand3d_b200 import autograd as A, runtime, weights as Wt
 from hand3d_b200.optim import Adam
+from hand3d_b200.train_loop import GraphedIteration
 from examples._synthetic_db import cleanup, db_path
 
 # training parameters (training_handsegnet.py:29-34); max_iter is --iters, the frequencies shrink with it for a short demo run
@@ -44,7 +47,12 @@ if __name__ == '__main__':
     ap.add_argument("--seed", type=int, default=None, help="seed of the reader's shuffle and augmentation (default: OS entropy)")
     ap.add_argument("--advance-global-step", action="store_true",
                     help="advance the global step so that the learning-rate schedule takes effect (the reference never does)")
+    ap.add_argument("--device-resident", action="store_true", help="upload the records to the GPU once; get() then runs on the device")
+    ap.add_argument("--graph", action="store_true", help="replay each iteration (reading, step, Adam) from one CUDA graph; "
+                                                         "needs --device-resident")
     args = ap.parse_args()
+    if args.graph and not args.device_resident:
+        ap.error("--graph captures the reader too, which needs --device-resident")
     train_para.update(max_iter=args.iters, show_loss_freq=args.show_loss_freq, snapshot_freq=args.snapshot_freq or args.iters + 1,
                       snapshot_dir=args.snapshot_dir)
 
@@ -55,10 +63,10 @@ if __name__ == '__main__':
         # DESIGN.md section 6 were measured with.
         if args.augment:
             dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=True, hue_aug=True, random_crop_to_size=True, path_to_db=path,
-                                     seed=args.seed)
+                                     seed=args.seed, device_resident=args.device_resident)
             print('Reader seed:', dataset.seed)
         else:
-            dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=False, path_to_db=path)
+            dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=False, path_to_db=path, device_resident=args.device_resident)
 
         net = ColorHandPose3DNetwork()
         if args.weights:
@@ -79,7 +87,7 @@ if __name__ == '__main__':
             os.mkdir(train_para['snapshot_dir'])
             print('Created snapshot dir:', train_para['snapshot_dir'])
 
-        for i in range(train_para['max_iter']):
+        def iteration():
             data = dataset.get()
             hand_mask_pred = net.inference_detection(data['image'], train=True)                              # :47
             loss = 0.0
@@ -88,8 +96,13 @@ if __name__ == '__main__':
                 loss = loss + A.softmax_xent_loss(pred_item, data['hand_mask'].float())
             opt.zero_grad()
             loss.backward()
-            opt.set_lr(lr_scheduler.get_lr(global_step))
             opt.step()
+            return loss.detach()
+
+        run = GraphedIteration(iteration) if args.graph else iteration
+        for i in range(train_para['max_iter']):
+            opt.set_lr(lr_scheduler.get_lr(global_step))          # outside the iteration: a graph replays device work only
+            loss = run()
             if args.advance_global_step:
                 global_step += 1
 

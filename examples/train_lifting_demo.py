@@ -5,13 +5,15 @@ PosePriorNetwork(variant).inference(train=True) -> the variant's MSE loss -> Ada
 show_loss_freq and pickled snapshots every snapshot_freq iterations.
 
     python examples/train_lifting_demo.py --variant {direct,bottleneck,local,local_w_xyz_loss,proposed} [--db rhd_training.bin]
-                                          [--iters 30] [--augment] [--seed S]
+                                          [--iters 30] [--augment] [--seed S] [--device-resident [--graph]]
 
 Like the reference, it starts from the initialisers (weights.xavier_weights: Xavier-uniform weights, biases 1e-4; the same
 distributions as tf.global_variables_initializer(), not TF's random values), not from a pickle.  Without --db it trains on a few
 synthetic records (examples/_synthetic_db.py).  The reference never feeds its `evaluation` placeholder, whose default is True, so
 dropout is the identity in its training too.  Snapshots are in the reference's weight-pickle layout
-(PosePriorNetwork(variant).init(weight_files=[...]) loads them), not TF checkpoints.
+(PosePriorNetwork(variant).init(weight_files=[...]) loads them), not TF checkpoints.  --device-resident keeps the records on the GPU;
+--graph then captures reading, the step and Adam once after two eager iterations and replays that CUDA graph for every later
+iteration.  Both print the losses of the plain run.
 """
 import argparse
 import os
@@ -24,6 +26,7 @@ from nets.PosePriorNetwork import PosePriorNetwork                   # training_
 from utils.general import LearningRateScheduler                      # training_lifting.py:26
 from hand3d_b200 import autograd as A, runtime, weights as Wt
 from hand3d_b200.optim import Adam
+from hand3d_b200.train_loop import GraphedIteration
 from hand3d_b200.utils.relative_trafo import bone_rel_trafo_inv
 from examples._synthetic_db import cleanup, db_path
 
@@ -48,7 +51,12 @@ if __name__ == '__main__':
     ap.add_argument("--snapshot-dir", default=None)
     ap.add_argument("--advance-global-step", action="store_true",
                     help="advance the global step so that the learning-rate schedule takes effect (the reference never does)")
+    ap.add_argument("--device-resident", action="store_true", help="upload the records to the GPU once; get() then runs on the device")
+    ap.add_argument("--graph", action="store_true", help="replay each iteration (reading, step, Adam) from one CUDA graph; "
+                                                         "needs --device-resident")
     args = ap.parse_args()
+    if args.graph and not args.device_resident:
+        ap.error("--graph captures the reader too, which needs --device-resident")
     VARIANT = args.variant
     train_para.update(max_iter=args.iters, show_loss_freq=args.show_loss_freq, snapshot_freq=args.snapshot_freq or args.iters + 1,
                       snapshot_dir=args.snapshot_dir or train_para['snapshot_dir'] % VARIANT)
@@ -59,9 +67,11 @@ if __name__ == '__main__':
         # streams).  The default reads in file order without noise, as the losses recorded in DESIGN.md section 6 were measured.
         if args.augment:
             dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=True, hand_crop=True, use_wrist_coord=False, coord_uv_noise=True,
-                                     crop_center_noise=True, crop_offset_noise=True, crop_scale_noise=True, path_to_db=path, seed=args.seed)
+                                     crop_center_noise=True, crop_offset_noise=True, crop_scale_noise=True, path_to_db=path, seed=args.seed,
+                                     device_resident=args.device_resident)
         else:
-            dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=False, hand_crop=True, use_wrist_coord=False, path_to_db=path)
+            dataset = BinaryDbReader(mode='training', batch_size=8, shuffle=False, hand_crop=True, use_wrist_coord=False, path_to_db=path,
+                                     device_resident=args.device_resident)
 
         net = PosePriorNetwork(VARIANT)
         ctx = runtime.default_context()
@@ -83,8 +93,7 @@ if __name__ == '__main__':
             os.mkdir(train_para['snapshot_dir'])
             print('Created snapshot dir:', train_para['snapshot_dir'])
 
-        print('Starting to train ...')
-        for i in range(train_para['max_iter']):
+        def iteration():
             data = dataset.get()
             _, coord3d_pred, R = net.inference(data['scoremap'], data['hand_side'], True, train=True)       # :53-54
             if VARIANT in ('direct', 'bottleneck'):                                                          # :62-76
@@ -97,8 +106,14 @@ if __name__ == '__main__':
                 loss = A.mse_loss(coord3d_pred, data['keypoint_xyz21_can']) + A.mse_loss(R, data['rot_mat'])
             opt.zero_grad()
             loss.backward()
-            opt.set_lr(lr_scheduler.get_lr(global_step))
             opt.step()
+            return loss.detach()
+
+        run = GraphedIteration(iteration) if args.graph else iteration
+        print('Starting to train ...')
+        for i in range(train_para['max_iter']):
+            opt.set_lr(lr_scheduler.get_lr(global_step))          # outside the iteration: a graph replays device work only
+            loss = run()
             if args.advance_global_step:
                 global_step += 1
 

@@ -67,6 +67,8 @@ SIGNATURES = {
     "h3d_stb_reader_items": (_i, [_p, _p, _i, _i, _p, _p, _p, _p, _p, _p]),
     "h3d_gaussian_scoremap": (_i, [_p, _p, _p, _i, _i, _i, _i, _f, _p, _p]),
     "h3d_reader_aug_params": (_i, [_p, _p, _i, C.c_uint64, _i, _p, _p]),
+    "h3d_reader_next_serials": (_i, [_p, _p, _i, C.c_uint64, _i, _p, _p]),
+    "h3d_decode_records_gather": (_i, [_p, _i, _p, _i64, _p, _i, _i, _p, _p, _p, _p, _p]),
     "h3d_augment_image": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
     "h3d_rhd_reader_items_aug": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "h3d_gaussian_scoremap_dropout": (_i, [_p, _p, _p, _p, _i, _f, _i, _i, _i, _i, _f, _p, _p]),
@@ -94,6 +96,8 @@ ADAM_STATE_WORDS = 4   # H3D_ADAM_STATE_WORDS
 AUG_COORD_UV_NOISE, AUG_CROP_CENTER_NOISE, AUG_CROP_SCALE_NOISE, AUG_CROP_OFFSET_NOISE, AUG_HUE, AUG_RANDOM_CROP, AUG_SCOREMAP_DROPOUT = 1, 2, 4, 8, 16, 32, 64
 AUG_STREAM_ITEMS, AUG_STREAM_SHUFFLE, AUG_MAX_ATTEMPTS = 0, 1, 16
 AUG_UV_NOISE, AUG_CENTER_NOISE, AUG_SCALE, AUG_OFFSET_NOISE, AUG_HUE_DELTA, AUG_WINDOW, AUG_KEEP, AUG_USED, AUG_PARAMS = 0, 84, 86, 87, 89, 90, 92, 113, 128
+# device-resident reading (H3D_READER_*): the queue state layout and the largest gather
+READER_QUEUE_CAPACITY, READER_STATE_COUNT, READER_STATE_NEXT, READER_STATE_SLOTS, READER_STATE_WORDS, READER_MAX_GATHER = 100, 0, 1, 2, 102, 4096
 
 _lib = None
 

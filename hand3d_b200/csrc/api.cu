@@ -1025,7 +1025,7 @@ static int check_device() {
 extern "C" {
 
 const char* h3d_last_error(void) { return g_err; }
-int h3d_version(void) { return 101; }
+int h3d_version(void) { return 102; }
 
 int h3d_device_available(void) {
     int n = 0;
@@ -1678,21 +1678,42 @@ int h3d_gather_records_p2p(h3d_ctx* ctx, const float* coord3d, const int32_t* ke
     if (!rc) ctx->launches += 1;
     return rc;
 }
+// The record layouts of both datasets; index != NULL gathers record index[b] mod n_records of a resident file.
+static int decode_dataset_records(int dataset, const uint8_t* records, const int64_t* index, int64_t n_records, int B, int step,
+                                  float* header, float* image, uint8_t* mask, uint8_t* visibility, cudaStream_t s, const char* who) {
+    if (dataset == H3D_DATASET_RHD) {
+        const int hdr = 42 * 3 + 42 * 2 + 9;                           // 219 floats = 876 B, then 2 B padding
+        return launch_decode_records(records, 410520, hdr, 878, 320, 320, step, 878 + 320 * 320 * 3, 42, header, image, mask, visibility, B, s,
+                                     index, n_records);
+    } else if (dataset == H3D_DATASET_STB) {
+        const int hdr = 21 * 3 + 21 * 3;                               // 126 floats = 504 B
+        return launch_decode_records(records, 922104, hdr, 504, 480, 640, step, -1, 0, header, image, nullptr, nullptr, B, s, index,
+                                     n_records);
+    }
+    set_error("%s: unknown dataset %d", who, dataset);
+    return H3D_EINVAL;
+}
 int h3d_decode_records(h3d_ctx* ctx, int dataset, const uint8_t* records, int B, int step, float* header, float* image, uint8_t* mask,
                        uint8_t* visibility, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(records && image && B > 0 && (step == 1 || step == 2 || step == 4), "h3d_decode_records: bad argument");
-    int rc;
-    if (dataset == H3D_DATASET_RHD) {
-        const int hdr = 42 * 3 + 42 * 2 + 9;                           // 219 floats = 876 B, then 2 B padding
-        rc = launch_decode_records(records, 410520, hdr, 878, 320, 320, step, 878 + 320 * 320 * 3, 42, header, image, mask, visibility, B, s);
-    } else if (dataset == H3D_DATASET_STB) {
-        const int hdr = 21 * 3 + 21 * 3;                               // 126 floats = 504 B
-        rc = launch_decode_records(records, 922104, hdr, 504, 480, 640, step, -1, 0, header, image, nullptr, nullptr, B, s);
-    } else {
-        set_error("h3d_decode_records: unknown dataset %d", dataset);
-        return H3D_EINVAL;
-    }
+    int rc = decode_dataset_records(dataset, records, nullptr, 0, B, step, header, image, mask, visibility, s, "h3d_decode_records");
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_decode_records_gather(h3d_ctx* ctx, int dataset, const uint8_t* file, int64_t n_records, const int64_t* serials, int B, int step,
+                              float* header, float* image, uint8_t* mask, uint8_t* visibility, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(file && serials && image && n_records > 0 && B > 0 && B <= H3D_READER_MAX_GATHER && (step == 1 || step == 2 || step == 4),
+                "h3d_decode_records_gather: bad argument");
+    int rc = decode_dataset_records(dataset, file, serials, n_records, B, step, header, image, mask, visibility, s, "h3d_decode_records_gather");
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_reader_next_serials(h3d_ctx* ctx, int64_t* state, int B, uint64_t seed, int shuffle, int64_t* serials, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(state && serials && B > 0, "h3d_reader_next_serials: bad argument");
+    int rc = launch_reader_next_serials(state, B, seed, shuffle ? 1 : 0, serials, s);
     if (!rc) ctx->launches += 1;
     return rc;
 }

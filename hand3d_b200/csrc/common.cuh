@@ -110,9 +110,11 @@ int launch_resize_argmax21(const float* x, float* y, int B, int H, int W, int oh
                            int* n_launch);
 // dst[r, dst_off + c] = src[r, c] for c < C (fp32 channel copy into a wider NHWC tensor)
 int launch_copy_channels(const float* src, float* dst, int64_t rows, int C, int dst_total, int dst_off, cudaStream_t s);
+// index != NULL: sample b is record index[b] mod n_records of `rec` (a resident file), B <= kMaxGatherRecords
+constexpr int kMaxGatherRecords = H3D_READER_MAX_GATHER;
 int launch_decode_records(const uint8_t* rec, int64_t record_bytes, int header_floats, int64_t image_off, int H, int W, int step,
                           int64_t mask_off, int tail_bytes, float* header, float* image, uint8_t* mask, uint8_t* tail, int B,
-                          cudaStream_t s);
+                          cudaStream_t s, const int64_t* index = nullptr, int64_t n_records = 0);
 int launch_eval_dist(const float* gt, const uint8_t* vis, const float* pred, int n, int D, float* dist, cudaStream_t s);
 int launch_gather_records_p2p(const float* coord3d, const int32_t* uv, const float* center, const float* scale, int B,
                               const uint64_t* peer_buffers, const uint64_t* peer_signals, uint64_t multicast_ptr, int rank, int world,
@@ -135,6 +137,7 @@ int launch_gaussian_map(const float* coords_hw, const uint8_t* valid, int B, int
                         const float* keep = nullptr, int keep_stride = 0, float keep_prob = 1.f);
 // (reader_aug.cu) training-mode augmentation of the RHD reader: per-sample parameters, hue + window crop
 int launch_reader_aug_params(const int64_t* serials, int B, uint64_t seed, int flags, float* params, cudaStream_t s);
+int launch_reader_next_serials(int64_t* state, int B, uint64_t seed, int shuffle, int64_t* serials, cudaStream_t s);
 int launch_augment_image(const float* image, const uint8_t* parts, const float* params, int B, int H, int W, int flags, int window,
                          float* out_image, int32_t* out_parts, int32_t* out_mask, cudaStream_t s);
 int launch_canonical_trafo(const float* xyz, const uint8_t* cond_right, int B, float* can, float* rot, float* rot_inv, cudaStream_t s);

@@ -933,10 +933,21 @@ int launch_resize_argmax21(const float* x, float* y, int B, int H, int W, int oh
 //   STB (data/BinaryDbReaderSTB.py:99-185): 21x3 f32 xyz | 21x3 f32 (u, v, valid) | 480x640x3 u8 RGB = 922 104 B
 // The float header is copied as is; the image becomes fp32 `u8 / 255 - 0.5` (two fp32 ops, as the readers do), optionally
 // sub-sampled by `step` (eval_full.py:50 resizes 480x640 -> 240x320, which TF1's legacy bilinear turns into "every 2nd pixel").
+// kGather: sample b is record index[b] mod n_records of a resident file instead of the b-th of B consecutive records; the record
+// offsets are resolved once per CTA into shared memory, the decode itself is the same code.
 // =============================================================================================
+template <bool kGather>
 __global__ void decode_records_kernel(const uint8_t* __restrict__ rec, int64_t record_bytes, int header_floats, int64_t image_off,
                                       int H, int W, int step, int64_t mask_off, int tail_bytes, float* __restrict__ header,
-                                      float* __restrict__ image, uint8_t* __restrict__ mask, uint8_t* __restrict__ tail, int B) {
+                                      float* __restrict__ image, uint8_t* __restrict__ mask, uint8_t* __restrict__ tail, int B,
+                                      const int64_t* __restrict__ index, int64_t n_records) {
+    extern __shared__ int64_t s_record_off[];        // kGather: byte offset of sample b's record, [B]
+    if (kGather) {
+        for (int b = threadIdx.x; b < B; b += blockDim.x)
+            s_record_off[b] = (int64_t)((uint64_t)index[b] % (uint64_t)n_records) * record_bytes;
+        __syncthreads();
+    }
+    auto base = [&](int b) -> int64_t { return kGather ? s_record_off[b] : (int64_t)b * record_bytes; };
     const int Ho = H / step, Wo = W / step;
     const int64_t per_img = (int64_t)Ho * Wo * 3;
     const int64_t total = (int64_t)B * per_img;
@@ -944,14 +955,14 @@ __global__ void decode_records_kernel(const uint8_t* __restrict__ rec, int64_t r
         const int b = (int)(i / per_img);
         const int64_t r = i - (int64_t)b * per_img;
         const int c = (int)(r % 3), x = (int)((r / 3) % Wo), y = (int)(r / (3 * (int64_t)Wo));
-        const uint8_t v = rec[(int64_t)b * record_bytes + image_off + ((int64_t)(y * step) * W + x * step) * 3 + c];
+        const uint8_t v = rec[base(b) + image_off + ((int64_t)(y * step) * W + x * step) * 3 + c];
         image[i] = __fsub_rn(__fdiv_rn((float)v, 255.0f), 0.5f);
     }
     const int64_t gtid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, gstride = (int64_t)gridDim.x * blockDim.x;
     if (header) {
         for (int64_t i = gtid; i < (int64_t)B * header_floats; i += gstride) {
             const int b = (int)(i / header_floats), j = (int)(i - (int64_t)b * header_floats);
-            const uint8_t* p = rec + (int64_t)b * record_bytes + 4 * j;       // records start 4-byte aligned (both sizes are multiples of 4)
+            const uint8_t* p = rec + base(b) + 4 * j;       // records start 4-byte aligned (both sizes are multiples of 4)
             uint32_t u = (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
             header[i] = __uint_as_float(u);
         }
@@ -960,23 +971,30 @@ __global__ void decode_records_kernel(const uint8_t* __restrict__ rec, int64_t r
         const int64_t n = (int64_t)H * W;
         for (int64_t i = gtid; i < (int64_t)B * n; i += gstride) {
             const int b = (int)(i / n);
-            mask[i] = rec[(int64_t)b * record_bytes + mask_off + (i - (int64_t)b * n)];
+            mask[i] = rec[base(b) + mask_off + (i - (int64_t)b * n)];
         }
     }
     if (tail && tail_bytes > 0) {
         for (int64_t i = gtid; i < (int64_t)B * tail_bytes; i += gstride) {
             const int b = (int)(i / tail_bytes);
-            tail[i] = rec[(int64_t)b * record_bytes + record_bytes - tail_bytes + (i - (int64_t)b * tail_bytes)];
+            tail[i] = rec[base(b) + record_bytes - tail_bytes + (i - (int64_t)b * tail_bytes)];
         }
     }
 }
 
 int launch_decode_records(const uint8_t* rec, int64_t record_bytes, int header_floats, int64_t image_off, int H, int W, int step,
                           int64_t mask_off, int tail_bytes, float* header, float* image, uint8_t* mask, uint8_t* tail, int B,
-                          cudaStream_t s) {
+                          cudaStream_t s, const int64_t* index, int64_t n_records) {
+    H3D_REQUIRE(!index || (n_records > 0 && B <= kMaxGatherRecords), "decode_records: a gather needs n_records > 0 and B <= %d",
+                kMaxGatherRecords);
     const int64_t total = (int64_t)B * (H / step) * (W / step) * 3;
-    decode_records_kernel<<<(int)std::min<int64_t>(ceil_div64(total, 256), 132 * 16), 256, 0, s>>>(
-        rec, record_bytes, header_floats, image_off, H, W, step, mask_off, tail_bytes, header, image, mask, tail, B);
+    const int grid = (int)std::min<int64_t>(ceil_div64(total, 256), 132 * 16);
+    if (index)
+        decode_records_kernel<true><<<grid, 256, (size_t)B * sizeof(int64_t), s>>>(
+            rec, record_bytes, header_floats, image_off, H, W, step, mask_off, tail_bytes, header, image, mask, tail, B, index, n_records);
+    else
+        decode_records_kernel<false><<<grid, 256, 0, s>>>(
+            rec, record_bytes, header_floats, image_off, H, W, step, mask_off, tail_bytes, header, image, mask, tail, B, nullptr, 0);
     H3D_CHECK_LAUNCH();
     return H3D_OK;
 }

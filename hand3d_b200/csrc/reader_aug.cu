@@ -79,6 +79,56 @@ int launch_reader_aug_params(const int64_t* serials, int B, uint64_t seed, int f
     return H3D_OK;
 }
 
+// ------------------------------------------------------------------------------------------ shuffle queue
+// The windowed shuffle of shuffle_batch_join(capacity=100, min_after_dequeue=50) on the device (state layout with H3D_READER_STATE_*).
+// Dequeue n reads word n of Philox4x64-10 keyed (seed, H3D_AUG_STREAM_SHUFFLE) in numpy.random.Philox.random_raw order: numpy bumps
+// its 256-bit counter BEFORE it fills its 4-word buffer, so word n is word (n mod 4) of the block at counter (n / 4 + 1, 0, 0, 0).
+// The slot choices are independent of each other and are drawn in parallel; taking and refilling the slots is sequential (thread 0).
+constexpr int kQueueChunk = 128;
+__global__ void __launch_bounds__(kQueueChunk) next_serials_kernel(int64_t* __restrict__ state, int B, uint64_t seed, int shuffle,
+                                                                   int64_t* __restrict__ serials) {
+    __shared__ int64_t s_slot[H3D_READER_QUEUE_CAPACITY];
+    __shared__ int s_k[kQueueChunk];
+    const uint64_t n0 = (uint64_t)state[H3D_READER_STATE_COUNT];
+    int64_t next = state[H3D_READER_STATE_NEXT];
+    if (!shuffle) {                                  // the in-order stream: consecutive positions
+        for (int i = threadIdx.x; i < B; i += blockDim.x) serials[i] = next + i;
+        __syncthreads();                             // every thread has read the state before it moves
+        if (threadIdx.x == 0) { state[H3D_READER_STATE_COUNT] = (int64_t)(n0 + (uint64_t)B); state[H3D_READER_STATE_NEXT] = next + B; }
+        return;
+    }
+    for (int i = threadIdx.x; i < H3D_READER_QUEUE_CAPACITY; i += blockDim.x) s_slot[i] = state[H3D_READER_STATE_SLOTS + i];
+    for (int base = 0; base < B; base += kQueueChunk) {
+        const int i = base + threadIdx.x;
+        if (i < B) {
+            const uint64_t n = n0 + (uint64_t)i;
+            uint64_t c[4] = {(n >> 2) + 1, 0, 0, 0};
+            philox4x64_10(c, seed, H3D_AUG_STREAM_SHUFFLE);
+            const int j = (int)(n & 3);
+            const uint64_t w = j == 0 ? c[0] : j == 1 ? c[1] : j == 2 ? c[2] : c[3];
+            s_k[threadIdx.x] = (int)(w % (uint64_t)H3D_READER_QUEUE_CAPACITY);
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            const int m = min(kQueueChunk, B - base);
+            for (int t = 0; t < m; ++t) {
+                const int k = s_k[t];
+                serials[base + t] = s_slot[k];
+                s_slot[k] = next++;
+            }
+        }
+        __syncthreads();
+    }
+    for (int i = threadIdx.x; i < H3D_READER_QUEUE_CAPACITY; i += blockDim.x) state[H3D_READER_STATE_SLOTS + i] = s_slot[i];
+    if (threadIdx.x == 0) { state[H3D_READER_STATE_COUNT] = (int64_t)(n0 + (uint64_t)B); state[H3D_READER_STATE_NEXT] = next; }
+}
+
+int launch_reader_next_serials(int64_t* state, int B, uint64_t seed, int shuffle, int64_t* serials, cudaStream_t s) {
+    next_serials_kernel<<<1, kQueueChunk, 0, s>>>(state, B, seed, shuffle, serials);
+    H3D_CHECK_LAUNCH();
+    return H3D_OK;
+}
+
 // ------------------------------------------------------------------------------------------ adjust_hue (TF 1.3, non-fused)
 // rgb_to_hsv / hsv_to_rgb as TF's colorspace_op.h functors evaluate them, element by element in fp32, then h = mod(h + (delta + 1), 1)
 // between them (image_ops_impl.adjust_hue).  S = V > 0 ? range / V : 0, so a pixel whose largest channel is <= 0 -- every dark pixel

@@ -553,7 +553,13 @@ class Context:
         if records.dtype != torch.uint8 or not records.is_cuda or records.dim() != 2:
             raise TypeError("records must be a 2-D uint8 CUDA tensor")
         records = records.contiguous()
-        B = records.shape[0]
+        ds, image, header, mask, vis = self._decode_outputs(records, dataset, records.shape[0], step, want_aux)
+        _lib.check(self.lib.h3d_decode_records(self.h, ds, _ptr(records), records.shape[0], step, _ptr(header), _ptr(image), _ptr(mask),
+                                               _ptr(vis), _stream()), "h3d_decode_records")
+        return {"image": image, "header": header, "mask": mask, "visibility": vis}
+
+    @staticmethod
+    def _decode_outputs(records, dataset, B, step, want_aux):
         ds = {"rhd": 0, "stb": 1}[dataset]
         rb, H, W, hdr = (410520, 320, 320, 219) if ds == 0 else (922104, 480, 640, 126)
         if records.shape[1] != rb:
@@ -563,9 +569,31 @@ class Context:
         header = torch.empty((B, hdr), dtype=torch.float32, device=dev) if want_aux else None
         mask = torch.empty((B, H, W), dtype=torch.uint8, device=dev) if (want_aux and ds == 0) else None
         vis = torch.empty((B, 42), dtype=torch.uint8, device=dev) if (want_aux and ds == 0) else None
-        _lib.check(self.lib.h3d_decode_records(self.h, ds, _ptr(records), B, step, _ptr(header), _ptr(image), _ptr(mask), _ptr(vis),
-                                               _stream()), "h3d_decode_records")
+        return ds, image, header, mask, vis
+
+    def decode_records_gather(self, file, serials, dataset="rhd", step=1, want_aux=True):
+        """decode_records of records gathered on the device: file uint8 CUDA [n_records, record_bytes] (a resident dataset file),
+        serials int64 CUDA [B] (stream positions >= 0) -> the items of record serials[b] mod n_records, bit for bit as decode_records
+        computes them from those records.  Only enqueues work: capturable into a CUDA graph."""
+        if file.dtype != torch.uint8 or not file.is_cuda or file.dim() != 2 or not file.is_contiguous():
+            raise TypeError("file must be a contiguous 2-D uint8 CUDA tensor of whole records")
+        if serials.dtype != torch.int64 or serials.device != file.device or serials.dim() != 1 or not serials.is_contiguous():
+            raise TypeError("serials must be a contiguous 1-D int64 tensor on the file's device")
+        B = serials.shape[0]
+        ds, image, header, mask, vis = self._decode_outputs(file, dataset, B, step, want_aux)
+        _lib.check(self.lib.h3d_decode_records_gather(self.h, ds, _ptr(file), file.shape[0], _ptr(serials), B, step, _ptr(header), _ptr(image),
+                                                      _ptr(mask), _ptr(vis), _stream()), "h3d_decode_records_gather")
         return {"image": image, "header": header, "mask": mask, "visibility": vis}
+
+    def reader_next_serials(self, state, B, seed, shuffle):
+        """The next B stream positions of a reader queue whose state lives on the device (int64 [_lib.READER_STATE_WORDS], advanced in
+        place) -> int64 CUDA [B].  With shuffle, the same stream as BinaryDbReader's host queue for the same seed."""
+        if state.dtype != torch.int64 or not state.is_cuda or state.numel() != _lib.READER_STATE_WORDS or not state.is_contiguous():
+            raise TypeError("state must be a contiguous int64 CUDA tensor of %d words" % _lib.READER_STATE_WORDS)
+        out = torch.empty((int(B),), dtype=torch.int64, device=state.device)
+        _lib.check(self.lib.h3d_reader_next_serials(self.h, _ptr(state), int(B), C.c_uint64(int(seed) & (2 ** 64 - 1)), int(bool(shuffle)),
+                                                    _ptr(out), _stream()), "h3d_reader_next_serials")
+        return out
 
     def rhd_reader_items(self, header, hand_parts, visibility, use_wrist_coord=True, hand_crop=False, crop_size=256):
         """Derived items of BinaryDbReader.get() (evaluation mode) from the outputs of decode_records(..., "rhd")."""

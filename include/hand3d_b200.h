@@ -277,7 +277,8 @@ H3D_API int h3d_gaussian_scoremap(h3d_ctx* ctx, const float* coords_hw, const ui
  *                              |z| <= 2 is kept (rounded to fp32), then TF's z * stddev + 0 in fp32; after H3D_AUG_MAX_ATTEMPTS
  *                              attempts without one (probability ~1e-43) z = 0;
  *   window offset in [0, 64] = w0 mod 65;  keep bit = floor(0.8f + u) in fp32 (TF 1.3 dropout, keep_prob 0.8).
- * The shuffle queue's dequeue order is host logic on a separate key (seed, H3D_AUG_STREAM_SHUFFLE). */
+ * The shuffle queue's dequeue order comes from a separate key (seed, H3D_AUG_STREAM_SHUFFLE); h3d_reader_next_serials runs it on the
+ * device, and the Python reader's host queue draws the same words. */
 #define H3D_AUG_STREAM_ITEMS 0
 #define H3D_AUG_STREAM_SHUFFLE 1
 #define H3D_AUG_MAX_ATTEMPTS 16
@@ -302,6 +303,29 @@ H3D_API int h3d_gaussian_scoremap(h3d_ctx* ctx, const float* coords_hw, const ui
 /* serials [B] int64 (device) -> params [B, H3D_AUG_PARAMS]: the final value of every flag in `flags`; a flag that is off gets its
  * neutral value (0 px, factor 1, delta 0, offset 0, keep 1) and unused slots are 0. */
 H3D_API int h3d_reader_aug_params(h3d_ctx* ctx, const int64_t* serials, int B, uint64_t seed, int flags, float* params, void* stream);
+/* ---- Device-resident reading: the record stream and the record gather, with no host in the loop (capturable) ----
+ * Queue state: H3D_READER_STATE_WORDS int64 words of DEVICE memory owned by the caller:
+ *   [H3D_READER_STATE_COUNT] dequeues so far, [H3D_READER_STATE_NEXT] next stream position to enqueue,
+ *   [H3D_READER_STATE_SLOTS + k] stream position held by queue slot k (shuffle only).
+ * A fresh queue is count 0 and, with shuffle, next 100 and slot k = k (the first 100 stream positions); in order, next 0. */
+#define H3D_READER_QUEUE_CAPACITY 100
+#define H3D_READER_STATE_COUNT 0
+#define H3D_READER_STATE_NEXT 1
+#define H3D_READER_STATE_SLOTS 2
+#define H3D_READER_STATE_WORDS 102
+#define H3D_READER_MAX_GATHER 4096
+/* The next B serials (stream positions) of the reader's queue -> serials [B] int64 (device); advances state.  Without shuffle they are
+ * next, next + 1, ...  With shuffle (shuffle_batch_join(capacity=100, min_after_dequeue=50) in its steady state), dequeue n takes slot
+ * k = w_n mod 100 and refills it with next++, where w_n is word n of Philox4x64-10 keyed (seed, H3D_AUG_STREAM_SHUFFLE) in
+ * numpy.random.Philox.random_raw order: word (n mod 4) of the block at counter (n / 4 + 1, 0, 0, 0) (numpy increments the counter before
+ * it fills its 4-word buffer).  The stream depends on the seed and the dequeue count only, not on how it is cut into batches.
+ * count < 2^63.  One CTA; enqueue-only. */
+H3D_API int h3d_reader_next_serials(h3d_ctx* ctx, int64_t* state, int B, uint64_t seed, int shuffle, int64_t* serials, void* stream);
+/* h3d_decode_records of records gathered from a resident file: file = n_records whole records of `dataset` back to back (device),
+ * serials [B] int64 (device, >= 0); sample b is record serials[b] mod n_records, decoded exactly as h3d_decode_records decodes it.
+ * B <= H3D_READER_MAX_GATHER; outputs as h3d_decode_records. */
+H3D_API int h3d_decode_records_gather(h3d_ctx* ctx, int dataset, const uint8_t* file, int64_t n_records, const int64_t* serials, int B,
+                                      int step, float* header, float* image, uint8_t* mask, uint8_t* visibility, void* stream);
 /* tf.image.random_hue (TF 1.3 adjust_hue, non-fused: rgb_to_hsv, h = mod(h + (delta + 1), 1), hsv_to_rgb, in the functors' fp32 order)
  * and / or the random_crop window, in one pass.  image [B,H,W,3] fp32, hand_parts [B,H,W] u8, params as above (delta at
  * H3D_AUG_HUE_DELTA when flags has H3D_AUG_HUE, window at H3D_AUG_WINDOW when flags has H3D_AUG_RANDOM_CROP) -> out_image [B,h,w,3]
