@@ -122,18 +122,9 @@ struct StagePlan {
     int cur_lane = 0;                   // lane given to steps as they are appended (see seal())
     int B = 0, H = 0, W = 0, variant = -1;
     int64_t flops = 0;
-    // layer chains (per chained launch one ticket word + B per-image completion counters, zeroed by the plan's first step;
-    // chain_prev = the chained launch appended last, iff it is the plan's most recent step): only for plans that
-    // tc_conv_plan_chainable() accepts, none in the sm_90a build
-    int* sync = nullptr;
-    int sync_slots = 0;
-    TcConvPlan* chain_prev = nullptr;
-    size_t chain_prev_step = 0;
-    int* chain_prev_sig = nullptr;
     ~StagePlan() {
         for (auto* p : tc) tc_conv_plan_destroy(p);
         for (auto* p : fc) fc_chain_plan_destroy(p);
-        if (sync) cudaFree(sync);
     }
     // label every step appended since the last call with the current lane
     void seal(bool join = false) {
@@ -450,22 +441,9 @@ static int add_direct(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, con
     return H3D_OK;
 }
 
-constexpr int kMaxChainSlots = 96;
-
-// First step of a stage plan that chains layers: zero the ticket words and completion counters (one memset node per stage call)
-static int begin_chain_sync(StagePlan* pl, int B) {
-    if (!tc_tuning().chain) return H3D_OK;
-    const size_t bytes = (size_t)kMaxChainSlots * (B + 1) * sizeof(int);
-    H3D_CUDA(cudaMalloc(&pl->sync, bytes));   // plan build time, never on a launch path
-    int* sync = pl->sync;
-    pl->steps.push_back([sync, bytes](const Ext&, cudaStream_t s) { H3D_CUDA(cudaMemsetAsync(sync, 0, bytes, s)); return H3D_OK; });
-    pl->launches.push_back(0);
-    return H3D_OK;
-}
-
 static int add_tc(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, const LayerSpec& l, int B, int H, int W, Split x,
                   int Cin_total, int Cin_pad, const std::vector<int>& perm, Split y, int Cy_total, int cy_off, float* yf,
-                  int Cyf_total, int cyf_off, int pool = 0, int force_passes = 0, bool chain = false, const LayerSpec* first = nullptr) {
+                  int Cyf_total, int cyf_off, int pool = 0, int force_passes = 0) {
     const PackedW* pw;
     int rc = get_packed(ctx, scope, l, Cin_pad, perm, &pw, force_passes);
     if (rc) return rc;
@@ -478,34 +456,12 @@ static int add_tc(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, const L
     d.corr_scale = pw->corr_scale;
     d.pool = pool;
     d.err_flag = ctx->err_flag;
-    if (first) {   // conv1_1 (fp32 image -> 64 channels) is computed inside this layer's kernel; its input comes from Ext.in at launch
-        if ((rc = dev_weight(ctx, scope + "/" + first->name + "/weights", &d.c1_w))) return rc;
-        if ((rc = dev_weight(ctx, scope + "/" + first->name + "/biases", &d.c1_bias))) return rc;
-        d.c1_leaky = first->leaky;
-    }
     TcConvPlan* tp = tc_conv_plan_create(d);
     if (!tp) return H3D_ECUDA;
     pl->tc.push_back(tp);
-    if (chain && pl->sync && tc_conv_plan_chainable(tp) && pl->sync_slots < kMaxChainSlots) {
-        int* words = pl->sync + (size_t)pl->sync_slots++ * (B + 1);   // [ticket | completion counter per image]
-        const int* dep = nullptr; int target = 0;
-        if (tc_tuning().chain == 1 && pl->chain_prev && pl->chain_prev_step + 1 == pl->steps.size()) {
-            // the previous step is a chained launch: depend on it per image iff it produces ALL of this layer's input planes
-            const TcConvDesc& pd = tc_conv_plan_desc(pl->chain_prev);
-            const int ph = pd.pool ? pd.H / 2 : pd.H, pw = pd.pool ? pd.W / 2 : pd.W;
-            if (pd.y.hi == x.hi && pd.y.lo == x.lo && pd.y.l8 == x.l8 && pd.cy_off == 0 && pd.Cy_total == Cin_total && pd.Cout_pad == Cin_pad &&
-                pd.B == B && ph == H && pw == W) {
-                dep = pl->chain_prev_sig; target = tc_conv_plan_signal_target(pl->chain_prev);
-            }
-        }
-        tc_conv_plan_set_chain(tp, words, dep, target, words + 1);
-        pl->chain_prev = tp; pl->chain_prev_step = pl->steps.size(); pl->chain_prev_sig = words + 1;
-    }
-    if (first) pl->steps.push_back([tp](const Ext& e, cudaStream_t s) { return tc_conv_launch_image(tp, e.in, s); });
-    else pl->steps.push_back([tp](const Ext&, cudaStream_t s) { return tc_conv_launch(tp, s); });
+    pl->steps.push_back([tp](const Ext&, cudaStream_t s) { return tc_conv_launch(tp, s); });
     pl->launches.push_back(1);
-    const int64_t fl = 2ll * B * H * W * l.k * l.k * l.cin * l.cout / (pool == 2 ? 4 : 1) +
-                       (first ? 2ll * B * H * W * first->k * first->k * first->cin * first->cout : 0);
+    const int64_t fl = 2ll * B * H * W * l.k * l.k * l.cin * l.cout / (pool == 2 ? 4 : 1);
     pl->flops += fl;
     tag(pl, KIND_TC, fl);
     return H3D_OK;
@@ -521,7 +477,6 @@ static int build_trunk(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, co
     const Half16 half = half_of(ctx->precision);
     char* slots[2] = {slot0, slot1};
     int cur = 0;
-    const LayerSpec* fused_first = nullptr;
     Act in;   // empty -> external fp32 input
     int h = H, w = W, rc;
     for (int i = 0; i < n; ++i) {
@@ -532,19 +487,8 @@ static int build_trunk(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, co
         const int c_off = last_layer ? final_c_off : 0;
         const bool pool_after = !strcmp(l.name, "conv1_2") || !strcmp(l.name, "conv2_2") || !strcmp(l.name, "conv3_4");
         const bool fuse_pool = use_tc && pool_after && (h % 2 == 0) && (w % 2 == 0) && !tc_tuning().no_pool_fusion;
-        // conv1_1 + conv1_2 as one launch where tc_conv_can_fuse_first() allows it (never in the sm_90a build): layer 0 is skipped
-        // here and handed to layer 1
-        if (tc && i == 0 && n > 1 && l.cin == 3 && l.cout == 64 && l.k == 3 && l.stride == 1 &&
-            !strcmp(layers[1].name, "conv1_2") && (h % 2 == 0) && (w % 2 == 0) && !tc_tuning().no_pool_fusion &&
-            tc_conv_can_fuse_first(h, w, layers[1].cin, layers[1].cout, layers[1].k, lo, 1)) {
-            fused_first = &layers[0];
-            continue;
-        }
-        if (use_tc && fused_first) {
-            rc = add_tc(ctx, pl, scope, l, B, h, w, Split(), 64, l.cin, {}, out.s, out.C, c_off, nullptr, 0, 0, fuse_pool ? 1 : 0, 0, true, fused_first);
-            fused_first = nullptr;
-        } else if (use_tc) {
-            rc = add_tc(ctx, pl, scope, l, B, h, w, in.s, in.C, l.cin, {}, out.s, out.C, c_off, nullptr, 0, 0, fuse_pool ? 1 : 0, 0, true);
+        if (use_tc) {
+            rc = add_tc(ctx, pl, scope, l, B, h, w, in.s, in.C, l.cin, {}, out.s, out.C, c_off, nullptr, 0, 0, fuse_pool ? 1 : 0);
         } else if (tc) {   // first layer (Cin = 3): CUDA-core conv writing the split planes directly
             rc = add_direct(ctx, pl, scope, l, B, h, w, in.f, i == 0 ? l.cin : in.C, 0, nullptr, 0, 0, out.s, out.C, c_off);
         } else {
@@ -573,7 +517,6 @@ static int build_handsegnet(h3d_ctx* ctx, int B, int H, int W) {
     auto pl = std::make_unique<StagePlan>();
     pl->B = B; pl->H = H; pl->W = W;
     const bool tc = is_tc(ctx->precision);
-    if (tc) { if (int rc0 = begin_chain_sync(pl.get(), B)) return rc0; }
     char* r = ctx->ws + ctx->lay.seg_off;
     const int64_t se = slot_elems_seg(B, H, W);
     char* slot0 = r; char* slot1 = r + align_up(se * 4, 1024);
@@ -584,8 +527,8 @@ static int build_handsegnet(h3d_ctx* ctx, int B, int H, int W) {
     float* low = ctx->lay.seg_low;
     if (tc) {
         Act mid = slot_view(other, (int64_t)B * h * w * 512, 512, true, passes_of(ctx->precision));
-        if ((rc = add_tc(ctx, pl.get(), "HandSegNet", kHandSeg[14], B, h, w, last.s, last.C, 128, {}, mid.s, 512, 0, nullptr, 0, 0, 0, 0, true))) return rc;
-        if ((rc = add_tc(ctx, pl.get(), "HandSegNet", kHandSeg[15], B, h, w, mid.s, 512, 512, {}, Split(), 0, 0, low, 2, 0, 0, 0, true))) return rc;
+        if ((rc = add_tc(ctx, pl.get(), "HandSegNet", kHandSeg[14], B, h, w, last.s, last.C, 128, {}, mid.s, 512, 0, nullptr, 0, 0))) return rc;
+        if ((rc = add_tc(ctx, pl.get(), "HandSegNet", kHandSeg[15], B, h, w, mid.s, 512, 512, {}, Split(), 0, 0, low, 2, 0))) return rc;
     } else {
         float* f512 = (float*)other;
         if ((rc = add_direct(ctx, pl.get(), "HandSegNet", kHandSeg[14], B, h, w, last.f, last.C, 0, f512, 512, 0, Split(), 0, 0))) return rc;
@@ -604,7 +547,6 @@ static int build_posenet(h3d_ctx* ctx, int B, int Hc, int Wc) {
     auto pl = std::make_unique<StagePlan>();
     pl->B = B; pl->H = Hc; pl->W = Wc;
     const bool tc = is_tc(ctx->precision);
-    if (tc) { if (int rc0 = begin_chain_sync(pl.get(), B)) return rc0; }
     const int lo = passes_of(ctx->precision);
     const int h8 = Hc / 8, w8 = Wc / 8;
     const int LH = std::max(ctx->lay.H, 256), LW = std::max(ctx->lay.W, 256);
@@ -634,15 +576,14 @@ static int build_posenet(h3d_ctx* ctx, int B, int Hc, int Wc) {
     }
     if ((rc = build_trunk(ctx, pl.get(), "PoseNet2D", kPoseTrunk, 15, B, Hc, Wc, slot0, slot1, se, &last, &h, &w, &cb, tc ? 0 : 21))) return rc;
     float** S = ctx->lay.s;
-    const Half16 half = half_of(ctx->precision);
     auto head = [&](const char* n6, const char* n7, int cin6, float* sm_out, bool feed_back, const Act& in6) -> int {
         // 1x1 conv (cin6 -> 512 or 128, leaky) then 1x1 conv (-> 21, linear); score-map also fed back into the concat buffer
         LayerSpec l6{n6, 1, 1, 128, cin6, 1}, l7{n7, 1, 1, cin6, 21, 0};
         int rc2;
         if (tc) {
             Act mid = slot_view((char*)f512, pix * cin6, cin6, true, lo);
-            if ((rc2 = add_tc(ctx, pl.get(), "PoseNet2D", l6, B, h, w, in6.s, in6.C, 128, {}, mid.s, cin6, 0, nullptr, 0, 0, 0, 0, true))) return rc2;
-            rc2 = add_tc(ctx, pl.get(), "PoseNet2D", l7, B, h, w, mid.s, cin6, cin6, {}, feed_back ? cb.s : Split(), 192, 128, sm_out, 21, 0, 0, 0, true);
+            if ((rc2 = add_tc(ctx, pl.get(), "PoseNet2D", l6, B, h, w, in6.s, in6.C, 128, {}, mid.s, cin6, 0, nullptr, 0, 0))) return rc2;
+            rc2 = add_tc(ctx, pl.get(), "PoseNet2D", l7, B, h, w, mid.s, cin6, cin6, {}, feed_back ? cb.s : Split(), 192, 128, sm_out, 21, 0);
         } else {
             if ((rc2 = add_direct(ctx, pl.get(), "PoseNet2D", l6, B, h, w, in6.f, in6.C, in6.f == cb.f ? 21 : 0, f512, cin6, 0, Split(), 0, 0))) return rc2;
             rc2 = add_direct(ctx, pl.get(), "PoseNet2D", l7, B, h, w, f512, cin6, 0, sm_out, 21, 0, Split(), 0, 0);
@@ -667,14 +608,13 @@ static int build_posenet(h3d_ctx* ctx, int B, int Hc, int Wc) {
         for (int i = 0; i < 5; ++i) {
             LayerSpec l{nm[i], 7, 1, i == 0 ? 149 : 128, 128, 1};
             Act out = slot_view(slots[i & 1], pix * 128, 128, tc, lo);
-            if (tc) rc = add_tc(ctx, pl.get(), "PoseNet2D", l, B, h, w, in.s, in.C, i == 0 ? 192 : 128, i == 0 ? perm : std::vector<int>(), out.s, 128, 0, nullptr, 0, 0, 0, 0, true);
+            if (tc) rc = add_tc(ctx, pl.get(), "PoseNet2D", l, B, h, w, in.s, in.C, i == 0 ? 192 : 128, i == 0 ? perm : std::vector<int>(), out.s, 128, 0, nullptr, 0, 0);
             else rc = add_direct(ctx, pl.get(), "PoseNet2D", l, B, h, w, in.f, in.C, 0, out.f, 128, 0, Split(), 0, 0);
             if (rc) return rc;
             in = out;
         }
         if ((rc = head(nm[5], nm[6], 128, S[u - 5], u == 6, in))) return rc;
     }
-    (void)half;
     ctx->pose = std::move(pl);
     return H3D_OK;
 }
@@ -1025,7 +965,7 @@ static int check_device() {
 extern "C" {
 
 const char* h3d_last_error(void) { return g_err; }
-int h3d_version(void) { return 102; }
+int h3d_version(void) { return 103; }
 
 int h3d_device_available(void) {
     int n = 0;

@@ -196,28 +196,16 @@ struct TcConvDesc {
     Half16 half;
     int pool = 0;  // 1: fuse the following 2x2/2 max-pool; 2: stride-2 'SAME' convolution (even H, W); outputs are [B, H/2, W/2, C]
     int* err_flag = nullptr;   // device int: a barrier wait that times out stores its code here before trapping (h3d_ctx owns it)
-    // conv1_1 fused into this layer: tc_conv_plan_create rejects it in the sm_90a build (tc_conv_can_fuse_first is false)
-    const float* c1_w = nullptr; const float* c1_bias = nullptr; int c1_leaky = 0;
 };
 // Tuning switches: initialised from the environment once (H3D_TC_BN, H3D_FC_CHAIN, ...), changed only through tc_set_tuning().
 struct TcTuning {
-    // two_cta, c64, c64x2, pair128, stack, exp, c3_tma, c64_tma_out, chain, small_batch_split and fuse_c1 chose between kernel
-    // variants of an earlier build; the sm_90a build has one convolution kernel family and accepts them without effect.
-    int two_cta = -1;
     int bn = 0;            // 0 policy, else forced N tile (64 or 128)
-    int c64 = 1, c64x2 = 1, pair128 = 1, stack = 1;
     int chunk_kb = 0;      // 0 policy, else K blocks per tensor-core partial sum
-    int exp = 0;
     int no_side_stream = 0, no_pool_fusion = 0, lift_direct = 0;
     int c3_ffma = 0;       // 1: first layer on the register-tiled FFMA kernel instead of the tensor cores
     int no_seg_fusion = 0; // 1: HandSegNet's x8 up-sampling as its own launch (instead of fused into the mask post-processing)
-    int c64_tma_out = 1;
     int fc_chain = 1;      // FC stacks + rotation epilogue of the lifting stage as one kernel (0 = one launch per layer)
-    int fuse_c1 = 1;
-    int small_batch_split = 1;
-    int chain = 1;
     int pdl = 1;           // programmatic dependent launch between the tensor-core kernels (prologue overlaps the previous kernel's tail)
-    int c3_tma = 1;
 };
 TcTuning& tc_tuning();
 int tc_set_tuning(const char* key, int value);
@@ -241,13 +229,7 @@ void fc_chain_plan_destroy(FcChainPlan* p);
 int fc_chain_launch(const FcChainPlan* p, const float* hand_side, float* rot, float* out, cudaStream_t s);
 TcConvPlan* tc_conv_plan_create(const TcConvDesc& d);   // nullptr on failure (h3d_last_error set)
 void tc_conv_plan_destroy(TcConvPlan* p);
-bool tc_conv_plan_chainable(const TcConvPlan* p);
-int tc_conv_plan_signal_target(const TcConvPlan* p);
-const TcConvDesc& tc_conv_plan_desc(const TcConvPlan* p);
-void tc_conv_plan_set_chain(TcConvPlan* p, int* sched, const int* dep_cnt, int dep_target, int* sig_cnt);
 int tc_conv_launch(const TcConvPlan* p, cudaStream_t s);
-int tc_conv_launch_image(const TcConvPlan* p, const float* image, cudaStream_t s);   // plans with TcConvDesc::c1_w (none on sm_90a)
-bool tc_conv_can_fuse_first(int H, int W, int Cin, int Cout, int k, int passes, int pool);
 int64_t tc_conv_flops(const TcConvPlan* p);
 int tc_num_sms();
 

@@ -772,25 +772,14 @@ TcTuning& tc_tuning() {
     static TcTuning t = [] {
         TcTuning v;
         auto geti = [](const char* n, int d) { const char* e = getenv(n); return e ? atoi(e) : d; };
-        v.two_cta = geti("H3D_TC_2CTA", -1);
         v.bn = geti("H3D_TC_BN", 0);
-        v.c64 = geti("H3D_TC_C64", 1);
-        v.c64x2 = geti("H3D_TC_C64X2", 1);
-        v.pair128 = geti("H3D_TC_PAIR128", 1);
-        v.stack = geti("H3D_TC_STACK", 1);
         v.chunk_kb = geti("H3D_TC_CHUNK_KB", 0);
-        v.exp = geti("H3D_TC_EXP", 0);
         v.no_side_stream = geti("H3D_NO_SIDE_STREAM", 0);
         v.no_pool_fusion = geti("H3D_NO_POOL_FUSION", 0);
         v.lift_direct = geti("H3D_LIFT_DIRECT", 0);
         v.c3_ffma = geti("H3D_C3_FFMA", 0);
-        v.c3_tma = geti("H3D_C3_TMA", 1);
         v.pdl = geti("H3D_PDL", 1);
         v.fc_chain = geti("H3D_FC_CHAIN", 1);
-        v.c64_tma_out = geti("H3D_C64_TMA_OUT", 1);
-        v.chain = geti("H3D_TC_CHAIN", 1);
-        v.small_batch_split = geti("H3D_TC_SMALL_SPLIT", 1);
-        v.fuse_c1 = geti("H3D_FUSE_C1", 1);
         v.no_seg_fusion = geti("H3D_NO_SEG_FUSION", 0);
         return v;
     }();
@@ -799,25 +788,14 @@ TcTuning& tc_tuning() {
 int tc_set_tuning(const char* key, int value) {
     TcTuning& t = tc_tuning();
     const std::string k(key ? key : "");
-    if (k == "tc_2cta") t.two_cta = value;
-    else if (k == "tc_bn") t.bn = value;
-    else if (k == "tc_c64") t.c64 = value;
-    else if (k == "tc_c64x2") t.c64x2 = value;
-    else if (k == "tc_pair128") t.pair128 = value;
-    else if (k == "tc_stack") t.stack = value;
+    if (k == "tc_bn") t.bn = value;
     else if (k == "tc_chunk_kb") t.chunk_kb = value;
-    else if (k == "tc_exp") t.exp = value;
     else if (k == "no_side_stream") t.no_side_stream = value;
     else if (k == "no_pool_fusion") t.no_pool_fusion = value;
     else if (k == "lift_direct") t.lift_direct = value;
     else if (k == "c3_ffma") t.c3_ffma = value;
-    else if (k == "c3_tma") t.c3_tma = value;
     else if (k == "pdl") t.pdl = value;
     else if (k == "fc_chain") t.fc_chain = value;
-    else if (k == "c64_tma_out") t.c64_tma_out = value;
-    else if (k == "tc_chain") t.chain = value;
-    else if (k == "tc_small_split") t.small_batch_split = value;
-    else if (k == "fuse_c1") t.fuse_c1 = value;
     else if (k == "no_seg_fusion") t.no_seg_fusion = value;
     else { set_error("h3d_set_tuning: unknown key '%s'", k.c_str()); return H3D_EINVAL; }
     return H3D_OK;
@@ -846,7 +824,6 @@ TcConvPlan* tc_conv_plan_create(const TcConvDesc& d) {
     if (padded_out && d.pool == 1) { set_error("tc_conv: fused pooling needs Cout %% 32 == 0"); return nullptr; }
     if (d.pool < 0 || d.pool > 2) { set_error("tc_conv: pool mode must be 0 (none), 1 (max-pool) or 2 (stride 2)"); return nullptr; }
     if (d.pool == 2 && d.k < 3) { set_error("tc_conv: stride 2 needs k >= 3 (for k = 1 TF's 'SAME' samples the even pixels, not the odd ones)"); return nullptr; }
-    if (d.c1_w) { set_error("tc_conv: conv1_1 is not fused into conv1_2 on sm_90a (tc_conv_can_fuse_first is false)"); return nullptr; }
     if (d.passes == 3 && (!d.x.lo || !d.w.lo)) { set_error("tc_conv: 3-pass mode needs lo planes"); return nullptr; }
     if (d.passes == 4 && (!d.x.l8 || !d.x.h8 || !d.w.l8 || !d.w.h8 || d.half != Half16::FP16 || d.corr_scale <= 0.f)) {
         set_error("tc_conv: fp8-correction mode needs fp16 + e4m3 l8/h8 planes for activations and weights and a correction scale");
@@ -909,23 +886,8 @@ TcConvPlan* tc_conv_plan_create(const TcConvDesc& d) {
 
 void tc_conv_plan_destroy(TcConvPlan* p) { delete p; }
 
-// Layer chains (per-image dependencies between consecutive launches) are not used by the sm_90a kernels: consecutive layers are
-// ordered by the stream and overlap only through programmatic dependent launch.
-bool tc_conv_plan_chainable(const TcConvPlan*) { return false; }
-int tc_conv_plan_signal_target(const TcConvPlan* p) { return p->p.tiles_w * p->p.tiles_h * p->p.n_tiles; }
-const TcConvDesc& tc_conv_plan_desc(const TcConvPlan* p) { return p->d; }
-void tc_conv_plan_set_chain(TcConvPlan*, int*, const int*, int, int*) {}
-
 int64_t tc_conv_flops(const TcConvPlan* p) {
     return 2ll * p->d.B * p->d.H * p->d.W * p->d.k * p->d.k * (int64_t)p->d.Cin_pad * p->d.Cout_pad;
-}
-
-// conv1_1 always runs as its own launch (conv_c3_tc_kernel) on sm_90a
-bool tc_conv_can_fuse_first(int, int, int, int, int, int, int) { return false; }
-
-int tc_conv_launch_image(const TcConvPlan*, const float*, cudaStream_t) {
-    set_error("tc_conv_launch_image: conv1_1 is not fused into conv1_2 on sm_90a");
-    return H3D_EINVAL;
 }
 
 int tc_conv_launch(const TcConvPlan* pl, cudaStream_t s) {

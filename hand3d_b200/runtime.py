@@ -68,8 +68,8 @@ class Context:
 
     # ---- configuration -------------------------------------------------------------------
     def _no_live_graphs(self, what):
-        # captured graphs bake in plan-owned device pointers (tile-ticket / completion counters, packed operands): rebuilding the
-        # plans under a live graph would make its replay touch freed memory
+        # captured graphs bake in plan-owned device pointers (packed operands, workspace views): rebuilding the plans under a
+        # live graph would make its replay touch freed memory
         if getattr(self, "_graphs_captured", 0):
             raise RuntimeError("%s rebuilds the stage plans, which captured CUDA graphs still point into; drop the graphs and call "
                                "release_graphs() first" % what)

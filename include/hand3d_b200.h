@@ -39,7 +39,7 @@ extern "C" {
 
 #define H3D_OK 0
 #define H3D_EINVAL (-1)     /* bad argument / shape                                   */
-#define H3D_ENODEVICE (-2)  /* no CUDA device, or not compute capability 10.x          */
+#define H3D_ENODEVICE (-2)  /* no CUDA device, or not compute capability 9.0           */
 #define H3D_ECUDA (-3)      /* CUDA runtime / driver error (message in h3d_last_error) */
 #define H3D_EWEIGHTS (-4)   /* weights missing, unknown name, wrong shape, NaN/Inf     */
 #define H3D_EWORKSPACE (-5) /* workspace arena missing or too small                    */
@@ -66,7 +66,7 @@ typedef struct h3d_ctx h3d_ctx;
 
 H3D_API const char* h3d_last_error(void);
 H3D_API int h3d_version(void);
-/* 1 when a CUDA device with compute capability 10.x is visible, else 0 (never fails). */
+/* 1 when a CUDA device with compute capability 9.0 is visible, else 0 (never fails). */
 H3D_API int h3d_device_available(void);
 
 /* ---- context ----------------------------------------------------------------------------- */
@@ -75,11 +75,9 @@ H3D_API int h3d_destroy(h3d_ctx* ctx);
 H3D_API int h3d_set_precision(h3d_ctx* ctx, int precision);
 H3D_API int h3d_get_precision(const h3d_ctx* ctx);
 /* Kernel-selection switches for A/B measurements and forced-variant tests (process-wide; initialised ONCE from the H3D_*
- * environment variables when the library is first used, never read on a launch path).  Keys: "tc_2cta" (-1 policy / 0 / 1),
- * "tc_bn" (0 policy / 64 / 128), "tc_c64", "tc_c64x2", "tc_pair128", "tc_stack", "tc_chunk_kb", "no_side_stream",
- * "no_pool_fusion", "lift_direct", "c3_ffma", "c3_tma", "pdl", "fc_chain", "c64_tma_out", "tc_chain", "tc_small_split", "fuse_c1",
- * "no_seg_fusion".  "tc_2cta", "tc_c64", "tc_c64x2", "tc_pair128", "tc_stack", "c3_tma", "c64_tma_out", "tc_chain", "tc_small_split"
- * and "fuse_c1" select nothing in the sm_90a build (one convolution kernel family) and are accepted for compatibility.
+ * environment variables when the library is first used, never read on a launch path).  Keys: "tc_bn" (0 policy / 64 / 128),
+ * "tc_chunk_kb" (0 policy, else K blocks per partial sum), "no_side_stream", "no_pool_fusion", "lift_direct", "c3_ffma", "pdl",
+ * "fc_chain", "no_seg_fusion".  Any other key returns H3D_EINVAL.
  * ctx may be NULL; when given, its cached layer plans are dropped (never while a CUDA graph captured from this context is alive:
  * graphs hold plan-owned pointers). */
 H3D_API int h3d_set_tuning(h3d_ctx* ctx, const char* key, int value);

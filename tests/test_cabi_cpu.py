@@ -36,6 +36,21 @@ def test_version_and_error_string(lib):
     assert isinstance(lib.h3d_last_error(), bytes)
 
 
+def test_set_tuning_keys(lib):
+    """The nine switches that select a real path are accepted (set to their defaults, so no process-wide state changes); the
+    switches of an earlier build that selected nothing on sm_90a are unknown keys."""
+    from hand3d_b200 import _lib
+    live = {"tc_bn": 0, "tc_chunk_kb": 0, "no_side_stream": 0, "no_pool_fusion": 0, "lift_direct": 0, "c3_ffma": 0, "pdl": 1,
+            "fc_chain": 1, "no_seg_fusion": 0}
+    for key, default in live.items():
+        assert lib.h3d_set_tuning(None, key.encode(), default) == _lib.OK, key
+    removed = ["tc_2cta", "tc_c64", "tc_c64x2", "tc_pair128", "tc_stack", "tc_exp", "c3_tma", "c64_tma_out", "tc_chain",
+               "tc_small_split", "fuse_c1"]
+    for key in removed:
+        assert lib.h3d_set_tuning(None, key.encode(), 0) == _lib.EINVAL, key
+        assert b"unknown key" in lib.h3d_last_error(), key
+
+
 def test_no_cpu_fallback(lib):
     import torch
     if torch.cuda.is_available():

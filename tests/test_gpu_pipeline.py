@@ -55,57 +55,31 @@ def test_handsegnet_stage(net, ctx, seg_ref, prec):
     assert err < TOL[prec], "HandSegNet %s: max abs err %.3e" % (prec, err)
 
 
-@pytest.mark.parametrize("knobs", [{"fuse_c1": 0}, {"fuse_c1": 0, "c3_tma": 0}, {"fuse_c1": 0, "c3_ffma": 1}], ids=["c3_tma", "c3_tc", "c3_ffma"])
-def test_first_layer_kernel_variants(net, ctx, seg_ref, knobs):
-    """conv1_1 runs on the tensor cores (conv_c3_tc_kernel, default) or as the register-tiled FFMA kernel (c3_ffma = 1); fuse_c1 and
-    c3_tma are accepted without effect on sm_90a.  Every setting must give the HandSegNet parity."""
+def test_first_layer_ffma_kernel(net, ctx, seg_ref):
+    """conv1_1 as the register-tiled FFMA kernel (c3_ffma = 1) instead of the tensor cores (conv_c3_tc_kernel, the default that
+    test_handsegnet_stage runs) must give the HandSegNet parity too."""
     img, ref = seg_ref
     ctx.set_precision("bf16x3")
-    default = {"fuse_c1": 1, "c3_tma": 1, "c3_ffma": 0}
-    for k, v in knobs.items():
-        ctx.set_tuning(k, v)
+    ctx.set_tuning("c3_ffma", 1)
     try:
         out = net.inference_detection(_dev(img))[0].cpu().numpy()
     finally:
-        for k in knobs:
-            ctx.set_tuning(k, default[k])
+        ctx.set_tuning("c3_ffma", 0)
     assert np.abs(out - ref).max() < 1e-3
 
 
-@pytest.mark.parametrize("fused", [0, 1], ids=["c3+c64x2", "fused_c1f"])
 @pytest.mark.parametrize("prec", ["bf16x3", "fp16x3"])
 @pytest.mark.parametrize("shape", [(3, 40, 40), (1, 24, 56), (2, 72, 48)])
-def test_handsegnet_small_odd_maps(net, ctx, wd, shape, prec, fused):
+def test_handsegnet_small_odd_maps(net, ctx, wd, shape, prec):
     """Maps that are no multiple of the pixel tile, odd numbers of tiles and tiles that lie entirely in conv1_2's zero padding:
-    exercises the masking of the first-layer and the implicit-GEMM kernels (with fuse_c1 set to 0 and 1)."""
+    exercises the masking of the first-layer and the implicit-GEMM kernels."""
     B, H, W = shape
     img = Wt.synthetic_images(B, H, W, seed=17)
     ctx.set_precision(prec)
-    ctx.set_tuning("fuse_c1", fused)
-    try:
-        out = net.inference_detection(_dev(img))[0].cpu().numpy()
-    finally:
-        ctx.set_tuning("fuse_c1", 1)
+    out = net.inference_detection(_dev(img))[0].cpu().numpy()
     ref = O.inference_detection(img, wd)[-1]
     assert out.shape == (B, H, W, 2)
     assert np.abs(out - ref).max() < 1e-3
-
-
-def test_fused_first_layers_full_pipeline(net, ctx, wd):
-    """The default first layers against fuse_c1 = 0 through the whole pipeline: 1e-3 maps, identical crops."""
-    B = 4
-    img = np.concatenate([Wt.synthetic_images(2, 320, 320, seed=51), Wt.synthetic_blob_images(2, 320, 320, seed=52)], 0)
-    hs = Wt.synthetic_hand_side(B, seed=53)
-    ctx.set_precision("bf16x3")
-    base = ctx.pipeline(_dev(img), _dev(hs), True)
-    ctx.set_tuning("fuse_c1", 0)
-    try:
-        r = ctx.pipeline(_dev(img), _dev(hs), True, force_center=base["center"], force_scale=base["scale_crop"])
-    finally:
-        ctx.set_tuning("fuse_c1", 1)
-    for k in ("hand_scoremap", "keypoints_scoremap", "keypoint_coord3d"):
-        assert (r[k] - base[k]).abs().max().item() < 1e-3, k
-    assert torch.equal(r["image_crop"], base["image_crop"])
 
 
 def test_handsegnet_240x320(net, ctx, wd):

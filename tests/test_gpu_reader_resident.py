@@ -61,7 +61,7 @@ def _same(a, b):
 
 # ------------------------------------------------------------------------------------------ 1. the serial stream
 @pytest.mark.parametrize("B", [1, 7, 8, 32])
-@pytest.mark.parametrize("seed", [0, 1, 2 ** 64 - 1, RANDOM_SEED])
+@pytest.mark.parametrize("seed", [0, 1, 2 ** 64 - 1, pytest.param(RANDOM_SEED, id="random")])   # the seed is in err_msg
 def test_device_serials_equal_host_queue(seed, B):
     from hand3d_b200.data.BinaryDbReader import _DeviceStream, _ShuffleQueue
     steps = -(-2000 // B)

@@ -28,16 +28,6 @@ CASES = [  # B,H,W,Cin,Cout,k
 ]
 
 
-@pytest.fixture
-def tuning(ctx):
-    """Sets tuning switches for one test and restores the defaults afterwards.  tc_2cta, tc_c64, tc_c64x2, tc_pair128 and tc_stack
-    selected kernel variants of an earlier build; the sm_90a build accepts them without effect, which these tests pin."""
-    defaults = {"tc_2cta": -1, "tc_bn": 0, "tc_c64": 1, "tc_c64x2": 1, "tc_pair128": 1, "tc_stack": 1}
-    yield ctx.set_tuning
-    for k, v in defaults.items():
-        ctx.set_tuning(k, v)
-
-
 @pytest.fixture(scope="module")
 def ctx():
     from hand3d_b200 import runtime
@@ -56,54 +46,6 @@ def test_conv2d_tc_vs_oracle(ctx, case, prec):
     ref = T.leaky_relu(T.conv2d_same(x, w, b, 1, np.float64))
     err = np.abs(y - ref).max()
     assert err < TOL[prec], "max abs err %.3e (tolerance %.1e)" % (err, TOL[prec])
-
-
-@pytest.mark.parametrize("prec", ["bf16x3", "fp16", "fp16_f8c"])
-@pytest.mark.parametrize("case", [CASES[3], CASES[4], CASES[6]])
-def test_conv2d_tc_forced_cta_pair(ctx, case, prec, tuning):
-    """tc_2cta = 1 (a CTA-pair request) leaves the results of ragged tile counts and N = 128 / 256 layers within tolerance."""
-    tuning("tc_2cta", 1)
-    B, H, W, Cin, Cout, k = case
-    rng = np.random.default_rng(15)
-    x = rng.normal(size=(B, H, W, Cin)).astype(f32)
-    w = (rng.normal(size=(k, k, Cin, Cout)) / np.sqrt(k * k * Cin)).astype(f32)
-    b = rng.normal(size=Cout).astype(f32)
-    y = ctx.conv2d_tc(torch.from_numpy(x).cuda(), w, b, leaky=True, precision=prec).cpu().numpy()
-    ref = T.leaky_relu(T.conv2d_same(x, w, b, 1, np.float64))
-    err = np.abs(y - ref).max()
-    assert err < TOL[prec], "max abs err %.3e (tolerance %.1e)" % (err, TOL[prec])
-
-
-@pytest.mark.parametrize("switch", ["tc_pair128", "tc_c64x2", "tc_c64", "tc_stack"])
-@pytest.mark.parametrize("case", [CASES[2], CASES[4], CASES[7], CASES[9], CASES[11]])
-def test_conv2d_tc_single_cta_variants(ctx, case, switch, tuning):
-    """Each of the former kernel-variant switches set to 0 leaves these shapes (64 -> 64, 64 -> 128, 7x7, N = 128) within tolerance."""
-    tuning(switch, 0)
-    B, H, W, Cin, Cout, k = case
-    rng = np.random.default_rng(16)
-    x = rng.normal(size=(B, H, W, Cin)).astype(f32)
-    w = (rng.normal(size=(k, k, Cin, Cout)) / np.sqrt(k * k * Cin)).astype(f32)
-    b = rng.normal(size=Cout).astype(f32)
-    y = ctx.conv2d_tc(torch.from_numpy(x).cuda(), w, b, leaky=True, precision="bf16x3").cpu().numpy()
-    ref = T.leaky_relu(T.conv2d_same(x, w, b, 1, np.float64))
-    err = np.abs(y - ref).max()
-    assert err < TOL["bf16x3"], "max abs err %.3e (tolerance %.1e)" % (err, TOL["bf16x3"])
-
-
-@pytest.mark.parametrize("pair", [1, 0])
-def test_conv2d_tc_c64_two_channel_groups(ctx, pair, tuning):
-    """64 -> 128 channels (conv2_1) in a 3-pass and the single-pass mode with the former 64-channel-kernel switches set."""
-    tuning("tc_c64", 2)
-    tuning("tc_c64x2", pair)
-    B, H, W, Cin, Cout, k = CASES[9]
-    rng = np.random.default_rng(17)
-    x = rng.normal(size=(B, H, W, Cin)).astype(f32)
-    w = (rng.normal(size=(k, k, Cin, Cout)) / np.sqrt(k * k * Cin)).astype(f32)
-    b = rng.normal(size=Cout).astype(f32)
-    for prec in ("bf16x3", "fp16"):
-        y = ctx.conv2d_tc(torch.from_numpy(x).cuda(), w, b, leaky=True, precision=prec).cpu().numpy()
-        ref = T.leaky_relu(T.conv2d_same(x, w, b, 1, np.float64))
-        assert np.abs(y - ref).max() < TOL[prec]
 
 
 STRIDED = [  # B,H,W,Cin,Cout: the stride-2 layers of the lifting pyramids (nets/ColorHandPose3DNetwork.py:255-258,291-294)
