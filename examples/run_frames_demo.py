@@ -1,0 +1,86 @@
+"""run.py over a stream of camera frames: every frame is resized to 240x320 on the device exactly as scipy.misc.imresize did
+(run.py:57-59), then goes through ColorHandPose3DNetwork.inference; key-points come back in frame pixels.
+
+    python examples/run_frames_demo.py                      # seeded synthetic 1080p frames, synthetic weights
+    python examples/run_frames_demo.py --video clip.mp4     # decoded with OpenCV (BGR -> RGB)
+    python examples/run_frames_demo.py --weights weights/   # the reference's pickled weights
+"""
+import argparse
+import os
+import sys
+import time
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def synthetic_batches(n_batches, B, H, W, seed):
+    rng = np.random.default_rng(seed)
+    for _ in range(n_batches):
+        yield rng.integers(0, 256, (B, H, W, 3), dtype=np.uint8)
+
+
+def video_batches(path, B, max_batches):
+    import cv2
+    cap = cv2.VideoCapture(path)
+    batch = []
+    n = 0
+    while n < max_batches:
+        ok, bgr = cap.read()
+        if not ok:
+            break
+        batch.append(cv2.cvtColor(bgr, cv2.COLOR_BGR2RGB))
+        if len(batch) == B:
+            yield np.stack(batch)
+            batch, n = [], n + 1
+    cap.release()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--video", default=None, help="video file (cv2 decodes it); default: synthetic frames")
+    ap.add_argument("--batch", type=int, default=8)
+    ap.add_argument("--batches", type=int, default=10)
+    ap.add_argument("--height", type=int, default=1080)
+    ap.add_argument("--width", type=int, default=1920)
+    ap.add_argument("--weights", default=None, help="directory of the reference's pickles (default: synthetic weights)")
+    ap.add_argument("--seed", type=int, default=0)
+    args = ap.parse_args()
+
+    from hand3d_b200 import runtime, weights as Wt
+    from hand3d_b200.frames import FrameRunner
+    from hand3d_b200.nets.ColorHandPose3DNetwork import ColorHandPose3DNetwork
+
+    net = ColorHandPose3DNetwork()
+    if args.weights:
+        net.init(None, weight_files=[os.path.join(args.weights, f) for f in ("handsegnet-rhd.pickle",
+                                                                          "posenet3d-rhd-stb-slr-finetuned.pickle")])
+    else:
+        net.init(None, weights=Wt.synthetic_weights(0))
+    ctx = runtime.default_context()
+
+    if args.video:
+        import cv2
+        cap = cv2.VideoCapture(args.video)
+        hw = (int(cap.get(cv2.CAP_PROP_FRAME_HEIGHT)), int(cap.get(cv2.CAP_PROP_FRAME_WIDTH)))
+        cap.release()
+        batches = video_batches(args.video, args.batch, args.batches)
+    else:
+        hw = (args.height, args.width)
+        batches = synthetic_batches(args.batches, args.batch, hw[0], hw[1], args.seed)
+
+    runner = FrameRunner(ctx, args.batch, hw)
+    t0 = time.perf_counter()
+    n = 0
+    for i, r in enumerate(runner.stream(batches)):
+        n += args.batch
+        kp = r["keypoints_frame"][0]
+        print("batch %d: frame 0 key-points (row, col) in %dx%d pixels: wrist %s, index tip %s" % (i, hw[0], hw[1], np.round(kp[0], 1),
+                                                                                               np.round(kp[8], 1)))
+    dt = time.perf_counter() - t0
+    print("%d frames in %.3f s: %.1f frames/s" % (n, dt, n / dt if dt > 0 else 0.0))
+
+
+if __name__ == "__main__":
+    main()

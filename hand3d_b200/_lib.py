@@ -69,7 +69,8 @@ SIGNATURES = {
     "h3d_reader_aug_params": (_i, [_p, _p, _i, C.c_uint64, _i, _p, _p]),
     "h3d_reader_next_serials": (_i, [_p, _p, _i, C.c_uint64, _i, _p, _p]),
     "h3d_decode_records_gather": (_i, [_p, _i, _p, _i64, _p, _i, _i, _p, _p, _p, _p, _p]),
-    "h3d_augment_image": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
+    "h3d_resize_frames": (_i, [_p, _p, _i, _i, _i, _i, _i, _i, _p, _p]),
+    "h3d_augment_image":(_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
     "h3d_rhd_reader_items_aug": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "h3d_gaussian_scoremap_dropout": (_i, [_p, _p, _p, _p, _i, _f, _i, _i, _i, _i, _f, _p, _p]),
     "h3d_canonical_trafo": (_i, [_p, _p, _p, _i, _p, _p, _p, _p]),
@@ -98,6 +99,8 @@ AUG_STREAM_ITEMS, AUG_STREAM_SHUFFLE, AUG_MAX_ATTEMPTS = 0, 1, 16
 AUG_UV_NOISE, AUG_CENTER_NOISE, AUG_SCALE, AUG_OFFSET_NOISE, AUG_HUE_DELTA, AUG_WINDOW, AUG_KEEP, AUG_USED, AUG_PARAMS = 0, 84, 86, 87, 89, 90, 92, 113, 128
 # device-resident reading (H3D_READER_*): the queue state layout and the largest gather
 READER_QUEUE_CAPACITY, READER_STATE_COUNT, READER_STATE_NEXT, READER_STATE_SLOTS, READER_STATE_WORDS, READER_MAX_GATHER = 100, 0, 1, 2, 102, 4096
+# camera frames (H3D_FRAME_*): the largest frame side and output side of h3d_resize_frames
+FRAME_MAX_SIDE, FRAME_MAX_OUT = 4096, 512
 
 _lib = None
 

@@ -16,12 +16,15 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libhand3d_b200.so")
 STAMP = os.path.join(HERE, ".libhand3d_b200.stamp")
-SOURCES = ["api.cu", "elementwise.cu", "reader.cu", "reader_aug.cu", "conv_direct.cu", "conv_wgmma.cu", "conv_wgrad.cu", "train.cu", "train_lift.cu"]
+SOURCES = ["api.cu", "elementwise.cu", "reader.cu", "reader_aug.cu", "conv_direct.cu", "conv_wgmma.cu", "conv_wgrad.cu", "train.cu", "train_lift.cu",
+           "frames.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--cudart=static", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",
     "-Xptxas", "-v",
 ]
+# per-source additions: frames.cu builds Pillow's resampling coefficients on the host in double, which must not be fused into FMAs
+SOURCE_FLAGS = {"frames.cu": ["-Xcompiler", "-ffp-contract=off"]}
 
 
 def _nvcc():
@@ -40,6 +43,7 @@ def _digest():
             h.update(n.encode())
             h.update(open(p, "rb").read())
     h.update(" ".join(NVCC_FLAGS).encode())
+    h.update(repr(sorted(SOURCE_FLAGS.items())).encode())
     return h.hexdigest()
 
 
@@ -52,7 +56,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(os.path.join(HERE, "build"), exist_ok=True)
     for src in SOURCES:
         obj = os.path.join(HERE, "build", src.replace(".cu", ".o"))
-        cmd = [_nvcc(), *NVCC_FLAGS, "-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [_nvcc(), *NVCC_FLAGS, *SOURCE_FLAGS.get(src, []), "-c", os.path.join(CSRC, src), "-o", obj]
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
         objs.append(obj)
     log = []

@@ -1,5 +1,6 @@
 // C ABI (include/hand3d_b200.h): context, weight loading / packing, workspace layout, the fixed layer
 // schedules of HandSegNet / PoseNet2D / PosePrior / ViewpointNet and the full pipeline.
+#include <array>
 #include <cstdarg>
 #include <cstring>
 #include <functional>
@@ -175,6 +176,9 @@ struct h3d_ctx {
     bool profiling = false;
     struct ProfRec { cudaEvent_t a, b; int kind; int64_t flops; };
     std::vector<ProfRec> prof;
+    // h3d_resize_frames plans by (Hf, Wf, h, w): created outside graph capture, freed only by h3d_destroy (captured graphs point into
+    // their coefficients, so adding a plan never frees or moves another)
+    std::map<std::array<int, 4>, FramePlan*> frame_plans;
 };
 
 namespace h3d {
@@ -965,7 +969,7 @@ static int check_device() {
 extern "C" {
 
 const char* h3d_last_error(void) { return g_err; }
-int h3d_version(void) { return 103; }
+int h3d_version(void) { return 104; }
 
 int h3d_device_available(void) {
     int n = 0;
@@ -1043,6 +1047,7 @@ int h3d_destroy(h3d_ctx* ctx) {
     for (void* p : ctx->retired) cudaFree(p);
     if (ctx->err_flag) cudaFreeHost(ctx->err_flag);
     if (ctx->fc_counter) cudaFree(ctx->fc_counter);
+    for (auto& kv : ctx->frame_plans) frame_plan_destroy(kv.second);
     delete ctx;
     return H3D_OK;
 }
@@ -1654,6 +1659,30 @@ int h3d_reader_next_serials(h3d_ctx* ctx, int64_t* state, int B, uint64_t seed, 
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(state && serials && B > 0, "h3d_reader_next_serials: bad argument");
     int rc = launch_reader_next_serials(state, B, seed, shuffle ? 1 : 0, serials, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_resize_frames(h3d_ctx* ctx, const uint8_t* frames, int B, int H, int W, int out_h, int out_w, int normalize, void* out, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(frames && out && B > 0 && (normalize == 0 || normalize == 1), "h3d_resize_frames: bad argument");
+    H3D_REQUIRE(H >= 1 && H <= H3D_FRAME_MAX_SIDE && W >= 1 && W <= H3D_FRAME_MAX_SIDE && out_h >= 1 && out_h <= H3D_FRAME_MAX_OUT &&
+                    out_w >= 1 && out_w <= H3D_FRAME_MAX_OUT,
+                "h3d_resize_frames: frames must be 1..%d pixels a side and the output 1..%d, got %dx%d -> %dx%d", H3D_FRAME_MAX_SIDE,
+                H3D_FRAME_MAX_OUT, H, W, out_h, out_w);
+    const std::array<int, 4> key{H, W, out_h, out_w};
+    auto it = ctx->frame_plans.find(key);
+    if (it == ctx->frame_plans.end()) {
+        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+        H3D_CUDA(cudaStreamIsCapturing(s, &cs));
+        H3D_REQUIRE(cs == cudaStreamCaptureStatusNone,
+                    "h3d_resize_frames: %dx%d -> %dx%d was not resized before this stream capture began, and its plan cannot be built "
+                    "under capture (the coefficients are uploaded with a host-to-device copy): resize one batch of this size first",
+                    H, W, out_h, out_w);
+        FramePlan* p = frame_plan_create(H, W, out_h, out_w, s);
+        if (!p) return H3D_ECUDA;
+        it = ctx->frame_plans.emplace(key, p).first;
+    }
+    int rc = launch_resize_frames(it->second, frames, B, normalize, out, s);
     if (!rc) ctx->launches += 1;
     return rc;
 }

@@ -1,0 +1,257 @@
+// Camera frames in: run.py:57-59's scipy.misc.imresize(image_raw, (240, 320)) (Pillow's 8-bit BILINEAR resample) of uint8 RGB frames,
+// bit for bit, optionally fused with run.py's normalisation float32(float64(u) / 255.0 - 0.5).
+//
+// Pillow's resample (libImaging/Resample.c): per axis a triangle filter of support max(in / out, 1), coefficients computed in double
+// and normalised per output pixel, then converted to fixed point with 22 fractional bits (rounded half away from zero); every output
+// value is (2^21 + sum of taps) >> 22 clipped to 0..255.  The horizontal pass runs first into a uint8 intermediate, then the vertical
+// pass; an axis whose size does not change gets no pass.  The coefficients are built on the host once per (Hf, Wf, h, w) plan; this
+// file is compiled with -ffp-contract=off so that the host never fuses a multiply-add into an FMA there.
+//
+// One kernel does both passes: a CTA owns one band of output rows of one image.  It streams the band's input rows (its rows plus the
+// vertical filter's halo) from HBM through a double-buffered shared-memory stage (cp.async for the 16-byte words inside the row, byte
+// loads at its unaligned ends), filters them horizontally into a uint8 chunk and adds each chunk's vertical contributions to int32
+// accumulators of the band's output rows.  No intermediate leaves the SM.
+#include <cstring>
+#include <vector>
+
+#include "common.cuh"
+
+namespace h3d {
+
+namespace {
+
+constexpr int kFrameThreads = 512;
+constexpr int kPrecisionBits = 22;                 // Pillow: 32 - 8 - 2
+constexpr int kStageBudget = 28 * 1024;            // bytes per staging buffer (two of them)
+constexpr int kAccBudget = 36 * 1024;              // bytes of int32 accumulators (the band's output rows)
+constexpr int kMaxChunk = 8, kMaxBand = 16;
+
+struct FrameArgs {
+    const uint8_t* in;
+    void* out;
+    int Hf, Wf, h, w, normalize;
+    int kxs, kys, band, chunk, row_stride, nbands;
+    int acc_bytes, inter_bytes;
+    const int32_t *xb, *kx, *yb, *ky;   // bounds (first tap, taps) and fixed-point coefficients per output column / row
+    const float* lut;                   // [256] run.py's normalisation of each code
+};
+
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
+    const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all_but_one() { asm volatile("cp.async.wait_group 1;\n" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;\n" ::: "memory"); }
+
+// Byte j of input row r lands at buf[i * row_stride + (address of the row & 15) + j] (i = r - c0): the 16-byte words of the row keep
+// their alignment in shared memory.  Words that lie wholly inside the row go through cp.async, the partial words at its ends byte by
+// byte, so nothing outside the frames is read.
+__device__ __forceinline__ void stage_rows(const FrameArgs& a, const uint8_t* img, int c0, int n, uint8_t* buf) {
+    const int64_t rb = (int64_t)a.Wf * 3;
+    const int words = a.row_stride >> 4;
+    for (int k = threadIdx.x; k < n * words; k += kFrameThreads) {
+        const int i = k / words, wd = k - i * words;
+        const uintptr_t lo = (uintptr_t)(img + (int64_t)(c0 + i) * rb), hi = lo + (uintptr_t)rb;
+        const uintptr_t g = (lo & ~(uintptr_t)15) + 16 * (uintptr_t)wd;
+        uint8_t* d = buf + (int64_t)i * a.row_stride + 16 * wd;
+        if (g >= lo && g + 16 <= hi) {
+            cp_async16(d, (const void*)g);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+                if (g + j >= lo && g + j < hi) d[j] = __ldg((const uint8_t*)(g + j));
+        }
+    }
+}
+
+__device__ __forceinline__ int clip8(int v) { return min(255, max(0, v >> kPrecisionBits)); }
+
+__global__ void __launch_bounds__(kFrameThreads, 2) resize_frames_kernel(FrameArgs a) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    const int band = blockIdx.x % a.nbands;
+    const int64_t b = blockIdx.x / a.nbands;
+    const int y0 = band * a.band, y1 = min(a.h, y0 + a.band), ny = y1 - y0;
+    const int w3 = a.w * 3;
+    int32_t* acc = reinterpret_cast<int32_t*>(smem);                     // [band][w3]
+    uint8_t* inter = smem + a.acc_bytes;                                 // [chunk][w3]: the horizontal pass of the current chunk
+    uint8_t* stage = inter + a.inter_bytes;                              // 2 x [chunk][row_stride]
+    const int64_t stage_bytes = (int64_t)a.chunk * a.row_stride;
+    const int64_t rb = (int64_t)a.Wf * 3;
+    const uint8_t* img = a.in + b * a.Hf * rb;
+    const int r0 = a.yb[2 * y0], r1 = a.yb[2 * (y1 - 1)] + a.yb[2 * (y1 - 1) + 1];   // the band's input rows (bounds are monotone)
+    const int nchunks = (r1 - r0 + a.chunk - 1) / a.chunk;
+
+    for (int i = threadIdx.x; i < ny * w3; i += kFrameThreads) acc[i] = 1 << (kPrecisionBits - 1);
+    stage_rows(a, img, r0, min(a.chunk, r1 - r0), stage);
+    cp_async_commit();
+    for (int c = 0; c < nchunks; ++c) {
+        const int c0 = r0 + c * a.chunk, n = min(a.chunk, r1 - c0);
+        const uint8_t* cur = stage + (c & 1) * stage_bytes;
+        if (c + 1 < nchunks) {        // the other buffer was last read before the barrier that ended the previous iteration
+            stage_rows(a, img, c0 + a.chunk, min(a.chunk, r1 - c0 - a.chunk), stage + ((c + 1) & 1) * stage_bytes);
+            cp_async_commit();
+            cp_async_wait_all_but_one();
+        } else {
+            cp_async_wait_all();
+        }
+        __syncthreads();
+        // horizontal pass: n input rows x w output columns, three channels per thread (one coefficient load per tap)
+        for (int i = threadIdx.x; i < n * a.w; i += kFrameThreads) {
+            const int r = i / a.w, x = i - r * a.w;
+            const int off = (int)((uintptr_t)(img + (int64_t)(c0 + r) * rb) & 15);
+            const int xmin = __ldg(a.xb + 2 * x), nx = __ldg(a.xb + 2 * x + 1);
+            const int32_t* k = a.kx + (int64_t)x * a.kxs;
+            const uint8_t* p = cur + (int64_t)r * a.row_stride + off + xmin * 3;
+            int s0 = 1 << (kPrecisionBits - 1), s1 = s0, s2 = s0;
+            for (int t = 0; t < nx; ++t) {
+                const int kt = __ldg(k + t);
+                s0 += p[3 * t] * kt;
+                s1 += p[3 * t + 1] * kt;
+                s2 += p[3 * t + 2] * kt;
+            }
+            uint8_t* q = inter + r * w3 + 3 * x;
+            q[0] = (uint8_t)clip8(s0); q[1] = (uint8_t)clip8(s1); q[2] = (uint8_t)clip8(s2);
+        }
+        __syncthreads();
+        // vertical pass: the chunk's contributions to every output row of the band whose taps reach into it
+        for (int y = y0; y < y1; ++y) {
+            const int ymin = __ldg(a.yb + 2 * y), yend = ymin + __ldg(a.yb + 2 * y + 1);
+            const int lo = max(c0, ymin), hi = min(c0 + n, yend);
+            if (lo >= hi) continue;
+            const int32_t* k = a.ky + (int64_t)y * a.kys + (lo - ymin);
+            for (int xc = threadIdx.x; xc < w3; xc += kFrameThreads) {
+                int s = 0;
+                for (int r = lo; r < hi; ++r) s += inter[(r - c0) * w3 + xc] * __ldg(k + (r - lo));
+                acc[(y - y0) * w3 + xc] += s;
+            }
+        }
+        __syncthreads();
+    }
+    const int64_t o = (b * a.h + y0) * (int64_t)w3;   // the band's output rows are contiguous
+    if (a.normalize) {
+        float* out = static_cast<float*>(a.out) + o;
+        for (int i = threadIdx.x; i < ny * w3; i += kFrameThreads) out[i] = __ldg(a.lut + clip8(acc[i]));
+    } else {
+        uint8_t* out = static_cast<uint8_t*>(a.out) + o;
+        for (int i = threadIdx.x; i < ny * w3; i += kFrameThreads) out[i] = (uint8_t)clip8(acc[i]);
+    }
+}
+
+// Pillow's precompute_coeffs + normalize_coeffs_8bpc for the bilinear filter (support 1) over a whole axis.  An axis that keeps its
+// size gets one tap of weight 1 per pixel (Pillow does not resample it: a copy).  bounds[2i] = first input pixel, bounds[2i+1] = taps.
+int pil_bilinear_coeffs(int in, int out, std::vector<int32_t>& bounds, std::vector<int32_t>& kk) {
+    bounds.assign(2 * (size_t)out, 0);
+    if (in == out) {
+        kk.assign((size_t)out, 1 << kPrecisionBits);
+        for (int i = 0; i < out; ++i) { bounds[2 * i] = i; bounds[2 * i + 1] = 1; }
+        return 1;
+    }
+    const double scale = (double)in / (double)out;
+    const double filterscale = scale < 1.0 ? 1.0 : scale;
+    const double support = 1.0 * filterscale;
+    const int ksize = (int)std::ceil(support) * 2 + 1;
+    const double ss = 1.0 / filterscale;
+    kk.assign((size_t)out * ksize, 0);
+    std::vector<double> k((size_t)ksize);
+    for (int xx = 0; xx < out; ++xx) {
+        const double center = (xx + 0.5) * scale;
+        int xmin = (int)(center - support + 0.5);
+        if (xmin < 0) xmin = 0;
+        int xmax = (int)(center + support + 0.5);
+        if (xmax > in) xmax = in;
+        xmax -= xmin;
+        double ww = 0.0;
+        for (int x = 0; x < xmax; ++x) {
+            double t = (x + xmin - center + 0.5) * ss;
+            if (t < 0.0) t = -t;
+            const double w = t < 1.0 ? 1.0 - t : 0.0;
+            k[x] = w;
+            ww += w;
+        }
+        for (int x = 0; x < xmax; ++x)
+            if (ww != 0.0) k[x] /= ww;
+        for (int x = 0; x < xmax; ++x)
+            kk[(size_t)xx * ksize + x] = k[x] < 0 ? (int32_t)(-0.5 + k[x] * (1 << kPrecisionBits)) : (int32_t)(0.5 + k[x] * (1 << kPrecisionBits));
+        bounds[2 * xx] = xmin;
+        bounds[2 * xx + 1] = xmax;
+    }
+    return ksize;
+}
+
+}  // namespace
+
+struct FramePlan {
+    int Hf = 0, Wf = 0, h = 0, w = 0;
+    int kxs = 0, kys = 0, band = 0, chunk = 0, row_stride = 0, nbands = 0, acc_bytes = 0, inter_bytes = 0, smem = 0;
+    std::vector<int32_t> host;      // the source of the asynchronous upload, kept for the plan's lifetime
+    int32_t* dev = nullptr;         // [xb | kx | yb | ky | lut]
+    const int32_t *xb = nullptr, *kx = nullptr, *yb = nullptr, *ky = nullptr;
+    const float* lut = nullptr;
+};
+
+FramePlan* frame_plan_create(int Hf, int Wf, int h, int w, cudaStream_t s) {
+    auto* p = new FramePlan();
+    p->Hf = Hf; p->Wf = Wf; p->h = h; p->w = w;
+    std::vector<int32_t> xb, kx, yb, ky;
+    p->kxs = pil_bilinear_coeffs(Wf, w, xb, kx);
+    p->kys = pil_bilinear_coeffs(Hf, h, yb, ky);
+    const int w3 = 3 * w;
+    p->row_stride = (int)align_up((int64_t)Wf * 3 + 15, 16);
+    p->chunk = std::max(1, std::min(kMaxChunk, kStageBudget / p->row_stride));
+    p->band = std::max(1, std::min({kMaxBand, h, kAccBudget / (w3 * 4)}));
+    p->nbands = ceil_div(h, p->band);
+    p->acc_bytes = (int)align_up((int64_t)p->band * w3 * 4, 16);
+    p->inter_bytes = (int)align_up((int64_t)p->chunk * w3, 16);
+    p->smem = p->acc_bytes + p->inter_bytes + 2 * p->chunk * p->row_stride;
+    auto& v = p->host;
+    const size_t oxb = 0, okx = oxb + xb.size(), oyb = okx + kx.size(), oky = oyb + yb.size(), olut = oky + ky.size();
+    v.resize(olut + 256);
+    std::copy(xb.begin(), xb.end(), v.begin() + oxb);
+    std::copy(kx.begin(), kx.end(), v.begin() + okx);
+    std::copy(yb.begin(), yb.end(), v.begin() + oyb);
+    std::copy(ky.begin(), ky.end(), v.begin() + oky);
+    for (int u = 0; u < 256; ++u) {    // run.py:59: image_raw.astype('float') / 255.0 - 0.5 in double, then the float32 input
+        const float f = (float)((double)u / 255.0 - 0.5);
+        memcpy(&v[olut + u], &f, 4);
+    }
+    // the attribute is per kernel, not per plan: only ever raise it, or a plan with less shared memory would break the earlier ones
+    cudaFuncAttributes fa;
+    cudaError_t e = cudaFuncGetAttributes(&fa, resize_frames_kernel);
+    if (e == cudaSuccess && fa.maxDynamicSharedSizeBytes < p->smem)
+        e = cudaFuncSetAttribute(resize_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, p->smem);
+    if (e == cudaSuccess) e = cudaMalloc(&p->dev, v.size() * 4);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(p->dev, v.data(), v.size() * 4, cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) {
+        cuda_fail(e, "frame_plan_create", __FILE__, __LINE__);
+        frame_plan_destroy(p);
+        return nullptr;
+    }
+    p->xb = p->dev + oxb; p->kx = p->dev + okx; p->yb = p->dev + oyb; p->ky = p->dev + oky;
+    p->lut = reinterpret_cast<const float*>(p->dev + olut);
+    return p;
+}
+
+void frame_plan_destroy(FramePlan* p) {
+    if (!p) return;
+    if (p->dev) cudaFree(p->dev);
+    delete p;
+}
+
+int launch_resize_frames(const FramePlan* p, const uint8_t* frames, int B, int normalize, void* out, cudaStream_t s) {
+    const int64_t grid = (int64_t)B * p->nbands;
+    if (grid >= (1ll << 31)) {
+        set_error("h3d_resize_frames: B = %d frames of %dx%d is too many for one launch", B, p->Hf, p->Wf);
+        return H3D_EINVAL;
+    }
+    FrameArgs a;
+    a.in = frames; a.out = out; a.Hf = p->Hf; a.Wf = p->Wf; a.h = p->h; a.w = p->w; a.normalize = normalize;
+    a.kxs = p->kxs; a.kys = p->kys; a.band = p->band; a.chunk = p->chunk; a.row_stride = p->row_stride; a.nbands = p->nbands;
+    a.acc_bytes = p->acc_bytes; a.inter_bytes = p->inter_bytes;
+    a.xb = p->xb; a.kx = p->kx; a.yb = p->yb; a.ky = p->ky; a.lut = p->lut;
+    resize_frames_kernel<<<(unsigned)grid, kFrameThreads, p->smem, s>>>(a);
+    H3D_CHECK_LAUNCH();
+    return H3D_OK;
+}
+
+}  // namespace h3d

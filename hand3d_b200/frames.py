@@ -1,0 +1,225 @@
+"""Camera frames in: run.py's front door (run.py:57-59) on the device.
+
+    image_raw = scipy.misc.imresize(image_raw, (240, 320))          # Pillow's 8-bit BILINEAR resample
+    image_v = np.expand_dims((image_raw.astype('float') / 255.0) - 0.5, 0)
+
+imresize() is that first line, bit for bit, for uint8 RGB frames of 1..4096 pixels a side (scipy.misc.imresize is gone from current
+scipy); to_network_input() fuses both lines into one kernel; frame_coords() maps coordinates of the 240x320 image back to frame
+pixels; FrameRunner serves a stream of equal-size frames through the resize and the whole pipeline as one CUDA graph per buffer.
+"""
+from __future__ import annotations
+
+import numpy as np
+import torch
+
+from . import _lib, runtime
+from .utils.general import trafo_coords
+
+NETWORK_SIZE = (240, 320)   # run.py:58
+
+
+def _ctx_for(t):
+    return runtime.default_context(t.device if isinstance(t, torch.Tensor) and t.is_cuda else None)
+
+
+def _batched(frames):
+    """CUDA uint8 [H,W,3] or [B,H,W,3] -> ([B,H,W,3], squeezed)."""
+    if not isinstance(frames, torch.Tensor):
+        raise TypeError("frames must be a torch.Tensor or a numpy array")
+    if not frames.is_cuda:
+        raise RuntimeError("frames must be a CUDA tensor here (numpy arrays are accepted by imresize)")
+    if frames.dim() == 3:
+        return frames.unsqueeze(0), True
+    return frames, False
+
+
+def _out_size(size, H, W):
+    """scipy.misc.imresize's size argument: an int is a percentage, a float a fraction, a tuple (h, w[, ...])."""
+    if isinstance(size, (bool, np.bool_)):
+        raise TypeError("size must be an int, a float or a tuple (h, w)")
+    if isinstance(size, (int, np.signedinteger)):
+        w, h = (np.array((W, H)) * (size / 100.0)).astype(int)
+        return int(h), int(w)
+    if isinstance(size, (float, np.floating)):
+        w, h = (np.array((W, H)) * size).astype(int)
+        return int(h), int(w)
+    return int(size[0]), int(size[1])
+
+
+def imresize(arr, size, interp="bilinear", mode=None):
+    """scipy.misc.imresize(arr, size) for uint8 RGB frames (its default interp='bilinear', mode=None), computed on the device.
+
+    arr: numpy uint8 [H,W,3] -> numpy uint8 [h,w,3]; or a CUDA uint8 tensor [H,W,3] / [B,H,W,3] -> a CUDA tensor of the same rank.
+    Equal, byte for byte, to Pillow's Image.resize((w, h), BILINEAR), which scipy called (see DESIGN.md section 4.12)."""
+    if interp != "bilinear":
+        raise ValueError("imresize: only interp='bilinear' (run.py's) is implemented, got %r" % (interp,))
+    if mode is not None:
+        raise ValueError("imresize: only mode=None (uint8 RGB in, RGB out) is implemented, got %r" % (mode,))
+    if isinstance(arr, np.ndarray):
+        if arr.dtype != np.uint8:
+            raise TypeError("imresize: frames must be uint8 (scipy would have rescaled %s data with bytescale), got %s" % (arr.dtype, arr.dtype))
+        if arr.ndim != 3 or arr.shape[2] != 3:
+            raise ValueError("imresize: a numpy frame must be [H,W,3] RGB, got %s" % (arr.shape,))
+        ctx = runtime.default_context()
+        h, w = _out_size(size, arr.shape[0], arr.shape[1])
+        t = torch.from_numpy(np.ascontiguousarray(arr)).to(ctx.device).unsqueeze(0)
+        return ctx.resize_frames(t, h, w, normalize=False)[0].cpu().numpy()
+    frames, squeeze = _batched(arr)
+    h, w = _out_size(size, frames.shape[1], frames.shape[2])
+    out = _ctx_for(frames).resize_frames(frames, h, w, normalize=False)
+    return out[0] if squeeze else out
+
+
+def to_network_input(frames, size=NETWORK_SIZE, out=None):
+    """run.py:58-59 in one kernel: CUDA uint8 frames [B,H,W,3] (or [H,W,3]) -> float32 [B,h,w,3] = float64(imresize(frame, size))
+    / 255.0 - 0.5 rounded to float32, the pipeline's input.  With `out` (float32 [B,h,w,3]) it writes there and allocates nothing, so a
+    call of an already seen size can be captured into a CUDA graph."""
+    frames, squeeze = _batched(frames)
+    r = _ctx_for(frames).resize_frames(frames, size[0], size[1], normalize=True, out=None if out is None else (out.unsqueeze(0) if squeeze else out))
+    return r[0] if squeeze else r
+
+
+def frame_coords(keypoints_hw, frame_hw, size=NETWORK_SIZE):
+    """Coordinates (row, col) in the size image (trafo_coords' output) -> frame pixels, with Pillow's pixel-centre convention:
+    (c + 0.5) * Hf / h - 0.5 for rows, the same with Wf / w for columns, in float64 on the device.  A CUDA tensor gives a CUDA float64
+    tensor (no host synchronisation, capturable); numpy gives numpy."""
+    if isinstance(keypoints_hw, np.ndarray):
+        dev = runtime.default_context().device
+        return frame_coords(torch.from_numpy(np.asarray(keypoints_hw, np.float64)).to(dev), frame_hw, size).cpu().numpy()
+    c = keypoints_hw.to(torch.float64)
+    # divide by a tensor: torch turns a division by a Python scalar into a multiplication by its reciprocal, which is not IEEE division
+    h = torch.full_like(c[..., 0], float(size[0]))
+    w = torch.full_like(c[..., 1], float(size[1]))
+    rows = (c[..., 0] + 0.5) * float(frame_hw[0]) / h - 0.5
+    cols = (c[..., 1] + 0.5) * float(frame_hw[1]) / w - 0.5
+    return torch.stack([rows, cols], -1)
+
+
+class FrameRunner:
+    """Serves a stream of equal-size uint8 RGB frames through run.py's resize and ColorHandPose3DNetwork.inference.
+
+    Each step is h3d_resize_frames (fused normalisation) followed by Context.pipeline on fixed buffers, captured as one CUDA graph
+    per input buffer (two buffers, used alternately).  ctx must have its weights loaded.
+
+    submit(frames, hand_side=None) enqueues one batch and returns its result tensors on the device:
+      keypoints_frame [B,21,2] float64 (row, col) key-points in frame pixels, keypoints_uv [B,21,2] int32 (256x256 crop),
+      keypoint_coord3d [B,21,3], center [B,2] and scale_crop [B,1] (float32).
+    Those tensors belong to buffer (call index mod 2): the replay of the call after next overwrites them, in stream order on the
+    current stream; read them (or copy them) before that call.
+      - Host frames (numpy or CPU torch, [B,H,W,3] uint8) are copied into a pinned staging buffer and uploaded on a copy stream, so
+        the upload of one batch overlaps the replay of the previous one.  A staging buffer is refilled only after its previous upload
+        has finished (an event wait for the upload two calls back).
+      - CUDA frames are copied into the graph's input buffer on the current stream; nothing synchronises the host.
+    hand_side [B,2] (run.py's constant [[1, 0]] when None) goes with each batch.
+
+    stream(batches) is the overlapped loop: it submits batch i + 1 before it reads back batch i, and yields the host results of
+    every batch in order (numpy dicts owned by the caller)."""
+
+    RESULT_KEYS = ("keypoints_frame", "keypoints_uv", "keypoint_coord3d", "center", "scale_crop")
+
+    def __init__(self, ctx, batch, frame_hw, size=NETWORK_SIZE, outputs="keypoints"):
+        self.ctx, self.B = ctx, int(batch)
+        self.frame_hw, self.size = (int(frame_hw[0]), int(frame_hw[1])), (int(size[0]), int(size[1]))
+        dev = ctx.device
+        Hf, Wf = self.frame_hw
+        h, w = self.size
+        self._frames = [torch.empty((self.B, Hf, Wf, 3), dtype=torch.uint8, device=dev) for _ in range(2)]
+        self._frames[0].zero_(); self._frames[1].zero_()
+        self._default_hs = torch.tensor([[1.0, 0.0]], dtype=torch.float32).expand(self.B, 2).contiguous().to(dev)
+        self._hs = [self._default_hs.clone() for _ in range(2)]
+        self._image = [torch.empty((self.B, h, w, 3), dtype=torch.float32, device=dev) for _ in range(2)]
+        self._stage = [None, None]          # pinned host copies of frames, created on the first host submission
+        self._stage_hs = [torch.empty((self.B, 2), dtype=torch.float32).pin_memory() for _ in range(2)]
+        self._copy = torch.cuda.Stream(device=dev)
+        self._d2h = torch.cuda.Stream(device=dev)
+        self._uploaded = [torch.cuda.Event() for _ in range(2)]
+        self._consumed = [torch.cuda.Event() for _ in range(2)]
+        self._d2h_done = [torch.cuda.Event() for _ in range(2)]
+        self._host = [None, None]
+        self._i = 0
+        ctx.ensure_workspace(self.B, h, w)
+
+        def body(k):
+            ctx.resize_frames(self._frames[k], h, w, normalize=True, out=self._image[k])
+            r = ctx.pipeline(self._image[k], self._hs[k], True, outputs=outputs)
+            r["keypoints_frame"] = frame_coords(trafo_coords(r["keypoints_uv"], r["center"], r["scale_crop"], 256), self.frame_hw, self.size)
+            return r
+
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):       # warm-up outside capture: builds the resize and stage plans, packs weights
+            for k in range(2):
+                body(k)
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize(dev)
+        self._graphs, self._results = [], []
+        for k in range(2):
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                r = body(k)
+            ctx._graphs_captured = getattr(ctx, "_graphs_captured", 0) + 1   # the graphs bake in workspace pointers
+            self._graphs.append(g)
+            self._results.append(r)
+
+    def _check_frames(self, frames):
+        shape = (self.B,) + self.frame_hw + (3,)
+        if tuple(frames.shape) != shape:
+            raise ValueError("FrameRunner: frames must be %s, got %s" % (shape, tuple(frames.shape)))
+
+    def submit(self, frames, hand_side=None):
+        k = self._i & 1
+        self._i += 1
+        cur = torch.cuda.current_stream(self.ctx.device)
+        cur.wait_event(self._d2h_done[k])           # stream() may still be reading this buffer's previous results
+        if isinstance(frames, torch.Tensor) and frames.is_cuda:
+            if frames.dtype != torch.uint8 or not frames.is_contiguous():
+                raise TypeError("FrameRunner: frames must be contiguous uint8")
+            self._check_frames(frames)
+            self._frames[k].copy_(frames)
+            if hand_side is None:
+                self._hs[k].copy_(self._default_hs)
+            else:
+                self._hs[k].copy_(torch.as_tensor(hand_side, dtype=torch.float32).to(self.ctx.device).reshape(self.B, 2))
+        else:
+            src = torch.from_numpy(np.ascontiguousarray(frames)) if isinstance(frames, np.ndarray) else frames
+            if not isinstance(src, torch.Tensor) or src.dtype != torch.uint8:
+                raise TypeError("FrameRunner: frames must be uint8 (numpy, CPU torch or CUDA torch)")
+            self._check_frames(src)
+            if self._stage[k] is None:
+                self._stage[k] = torch.empty(src.shape, dtype=torch.uint8).pin_memory()
+            self._uploaded[k].synchronize()         # the upload that last read this staging buffer (two calls back) has finished
+            self._stage[k].copy_(src)
+            self._stage_hs[k].copy_(torch.as_tensor(np.asarray([[1.0, 0.0]] * self.B if hand_side is None else hand_side, np.float32)).reshape(self.B, 2))
+            with torch.cuda.stream(self._copy):
+                self._copy.wait_event(self._consumed[k])      # the replay that last read this input buffer has finished
+                self._frames[k].copy_(self._stage[k], non_blocking=True)
+                self._hs[k].copy_(self._stage_hs[k], non_blocking=True)
+                self._uploaded[k].record(self._copy)
+            cur.wait_event(self._uploaded[k])
+        self._graphs[k].replay()
+        self._consumed[k].record(cur)
+        return {n: self._results[k][n] for n in self.RESULT_KEYS}
+
+    def stream(self, batches):
+        """batches: iterable of frames, or of (frames, hand_side) -> yields one numpy dict per batch, in order."""
+        pending = None
+        for item in batches:
+            frames, hs = item if isinstance(item, tuple) else (item, None)
+            res = self.submit(frames, hs)
+            k = (self._i - 1) & 1
+            if self._host[k] is None:
+                self._host[k] = {n: torch.empty(t.shape, dtype=t.dtype).pin_memory() for n, t in res.items()}
+            with torch.cuda.stream(self._d2h):
+                self._d2h.wait_event(self._consumed[k])
+                for n, t in res.items():
+                    self._host[k][n].copy_(t, non_blocking=True)
+                self._d2h_done[k].record(self._d2h)
+            if pending is not None:
+                yield self._collect(pending)
+            pending = k
+        if pending is not None:
+            yield self._collect(pending)
+
+    def _collect(self, k):
+        self._d2h_done[k].synchronize()             # the read-back the caller asked for
+        return {n: t.numpy().copy() for n, t in self._host[k].items()}

@@ -396,6 +396,30 @@ class Context:
                    "h3d_resize_bilinear_tf1")
         return y
 
+    def resize_frames(self, frames, out_h, out_w, normalize, out=None):
+        """run.py:57-59 on the device: frames uint8 CUDA [B,H,W,3] (contiguous RGB) -> [B,out_h,out_w,3], uint8 scipy.misc.imresize
+        bytes (Pillow BILINEAR) or, with normalize, float32 u / 255.0 - 0.5 computed in double.  The first call with a new size builds
+        its plan (not under graph capture); later calls only enqueue one kernel."""
+        if not isinstance(frames, torch.Tensor):
+            raise TypeError("frames must be a torch.Tensor")
+        if not frames.is_cuda:
+            raise RuntimeError("frames must live on a CUDA device (hand3d_b200 has no CPU path)")
+        if frames.dtype != torch.uint8:
+            raise TypeError("frames must be uint8, got %s" % frames.dtype)
+        if frames.dim() != 4 or frames.shape[3] != 3:
+            raise ValueError("frames must be [B,H,W,3] RGB, got %s" % (tuple(frames.shape),))
+        if not frames.is_contiguous():
+            raise ValueError("frames must be contiguous")
+        B, H, W, _ = frames.shape
+        dt = torch.float32 if normalize else torch.uint8
+        if out is None:
+            out = torch.empty((B, int(out_h), int(out_w), 3), dtype=dt, device=frames.device)
+        elif out.dtype != dt or tuple(out.shape) != (B, int(out_h), int(out_w), 3) or not out.is_contiguous() or out.device != frames.device:
+            raise ValueError("out must be a contiguous %s tensor [%d,%d,%d,3] on the frames' device" % (dt, B, out_h, out_w))
+        _lib.check(self.lib.h3d_resize_frames(self.h, _ptr(frames), B, H, W, int(out_h), int(out_w), int(bool(normalize)), _ptr(out),
+                                              _stream()), "h3d_resize_frames")
+        return out
+
     # ---- training (h3d_resize_bilinear_tf1_backward, the two losses, Adam) ----------------------
     def variables(self, scope):
         """Ordered {reference variable name: torch.nn.Parameter} of "HandSegNet", "PoseNet2D", "PosePrior" (with fc_bottleneck when

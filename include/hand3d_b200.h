@@ -324,6 +324,19 @@ H3D_API int h3d_reader_next_serials(h3d_ctx* ctx, int64_t* state, int B, uint64_
  * B <= H3D_READER_MAX_GATHER; outputs as h3d_decode_records. */
 H3D_API int h3d_decode_records_gather(h3d_ctx* ctx, int dataset, const uint8_t* file, int64_t n_records, const int64_t* serials, int B,
                                       int step, float* header, float* image, uint8_t* mask, uint8_t* visibility, void* stream);
+
+/* ---- camera frames (run.py:57-59: image_raw = scipy.misc.imresize(image_raw, (240, 320)); image_raw.astype('float') / 255.0 - 0.5)
+ * frames [B,H,W,3] uint8 RGB, contiguous (device) -> out [B,out_h,out_w,3]: with normalize = 0 uint8, exactly scipy.misc.imresize(frame,
+ * (out_h, out_w)) with interp='bilinear', i.e. Pillow's Image.resize((out_w, out_h), BILINEAR) (8-bit fixed point, 22 fractional bits,
+ * horizontal pass into uint8 first, no pass on an axis that keeps its size); with normalize = 1 float32, run.py's network input
+ * float32(float64(u) / 255.0 - 0.5) of that uint8 result.  1 <= H, W <= H3D_FRAME_MAX_SIDE and 1 <= out_h, out_w <= H3D_FRAME_MAX_OUT,
+ * anything else is H3D_EINVAL.  The first call with a new (H, W, out_h, out_w) builds its coefficients on the host and uploads them on
+ * `stream`; such a call is refused while `stream` is being captured.  Later calls only enqueue one kernel (capturable); a context keeps
+ * every plan until h3d_destroy. */
+#define H3D_FRAME_MAX_SIDE 4096
+#define H3D_FRAME_MAX_OUT 512
+H3D_API int h3d_resize_frames(h3d_ctx* ctx, const uint8_t* frames, int B, int H, int W, int out_h, int out_w, int normalize, void* out,
+                              void* stream);
 /* tf.image.random_hue (TF 1.3 adjust_hue, non-fused: rgb_to_hsv, h = mod(h + (delta + 1), 1), hsv_to_rgb, in the functors' fp32 order)
  * and / or the random_crop window, in one pass.  image [B,H,W,3] fp32, hand_parts [B,H,W] u8, params as above (delta at
  * H3D_AUG_HUE_DELTA when flags has H3D_AUG_HUE, window at H3D_AUG_WINDOW when flags has H3D_AUG_RANDOM_CROP) -> out_image [B,h,w,3]
