@@ -91,6 +91,9 @@ SIGNATURES = {
     "h3d_bone_rel_trafo": (_i, [_p, _p, _p, _i, _p]),
     "h3d_mse_loss_forward": (_i, [_p, _p, _p, _i64, _p, _p]),
     "h3d_mse_loss_backward": (_i, [_p, _p, _p, _p, _i64, _p, _p]),
+    "h3d_eval_store_bytes": (_i64, [_i, _i, _i]),
+    "h3d_eval_feed": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _i, _i, _p]),
+    "h3d_eval_stats": (_i, [_p, _p, _i, _i, _i, _p, _i, _p, _p]),
 }
 ADAM_STATE_WORDS = 4   # H3D_ADAM_STATE_WORDS
 # training-mode reader augmentation (H3D_AUG_*): flags, and the per-sample parameter layout
@@ -101,6 +104,11 @@ AUG_UV_NOISE, AUG_CENTER_NOISE, AUG_SCALE, AUG_OFFSET_NOISE, AUG_HUE_DELTA, AUG_
 READER_QUEUE_CAPACITY, READER_STATE_COUNT, READER_STATE_NEXT, READER_STATE_SLOTS, READER_STATE_WORDS, READER_MAX_GATHER = 100, 0, 1, 2, 102, 4096
 # camera frames (H3D_FRAME_*): the largest frame side and output side of h3d_resize_frames
 FRAME_MAX_SIDE, FRAME_MAX_OUT = 4096, 512
+# device evaluation store (H3D_EVAL_*): dtypes, the header layout, the limits and the layout of a stats row
+EVAL_FLOAT32, EVAL_FLOAT64 = 0, 1
+EVAL_KEPT, EVAL_DROPPED, EVAL_TICKET, EVAL_COUNT, EVAL_HEADER_WORDS = 0, 1, 2, 8, 72
+EVAL_MAX_KP, EVAL_MAX_DIM, EVAL_MAX_SAMPLES, EVAL_MAX_THRESHOLDS = 64, 4, 1 << 24, 4096
+EVAL_STAT_N, EVAL_STAT_MEAN, EVAL_STAT_MEDIAN, EVAL_STAT_COUNTS = 0, 1, 2, 3
 
 _lib = None
 

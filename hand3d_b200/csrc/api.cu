@@ -969,7 +969,7 @@ static int check_device() {
 extern "C" {
 
 const char* h3d_last_error(void) { return g_err; }
-int h3d_version(void) { return 104; }
+int h3d_version(void) { return 105; }
 
 int h3d_device_available(void) {
     int n = 0;
@@ -1762,6 +1762,39 @@ int h3d_eval_keypoint_dist(h3d_ctx* ctx, const float* gt, const uint8_t* vis, co
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(gt && vis && pred && dist && n > 0 && D >= 1 && D <= 4, "h3d_eval_keypoint_dist: bad argument");
     int rc = launch_eval_dist(gt, vis, pred, n, D, dist, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+static int eval_store_check(const char* what, int K, int num_samples, int dtype) {
+    H3D_REQUIRE(K >= 1 && K <= H3D_EVAL_MAX_KP, "%s: K = %d key-points, the store holds 1..%d", what, K, H3D_EVAL_MAX_KP);
+    H3D_REQUIRE(num_samples >= 1 && num_samples <= H3D_EVAL_MAX_SAMPLES, "%s: num_samples = %d, the store holds 1..%d", what, num_samples,
+                H3D_EVAL_MAX_SAMPLES);
+    H3D_REQUIRE(dtype == H3D_EVAL_FLOAT32 || dtype == H3D_EVAL_FLOAT64, "%s: dtype %d is neither H3D_EVAL_FLOAT32 nor H3D_EVAL_FLOAT64",
+                what, dtype);
+    return H3D_OK;
+}
+int64_t h3d_eval_store_bytes(int K, int num_samples, int dtype) {
+    if (int rc = eval_store_check("h3d_eval_store_bytes", K, num_samples, dtype)) return rc;
+    return (int64_t)H3D_EVAL_HEADER_WORDS * 8 + (int64_t)K * num_samples * (dtype == H3D_EVAL_FLOAT64 ? 8 : 4);
+}
+int h3d_eval_feed(h3d_ctx* ctx, void* store, int K, int num_samples, int dtype, const void* gt, const uint8_t* vis, const void* pred, int n,
+                  int D, void* stream) {
+    if (int rc = eval_store_check("h3d_eval_feed", K, num_samples, dtype)) return rc;
+    H3D_REQUIRE(D >= 1 && D <= H3D_EVAL_MAX_DIM, "h3d_eval_feed: D = %d coordinates, 1..%d are supported", D, H3D_EVAL_MAX_DIM);
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(store && gt && vis && pred && n > 0, "h3d_eval_feed: bad argument");
+    int rc = launch_eval_feed(store, K, num_samples, dtype, gt, vis, pred, n, D, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_eval_stats(h3d_ctx* ctx, const void* store, int K, int num_samples, int dtype, const double* thresholds, int T, int64_t* out,
+                   void* stream) {
+    if (int rc = eval_store_check("h3d_eval_stats", K, num_samples, dtype)) return rc;
+    H3D_REQUIRE(T >= 1 && T <= H3D_EVAL_MAX_THRESHOLDS, "h3d_eval_stats: T = %d thresholds, 1..%d are supported", T,
+                H3D_EVAL_MAX_THRESHOLDS);
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(store && thresholds && out, "h3d_eval_stats: bad argument");
+    int rc = launch_eval_stats(store, K, num_samples, dtype, thresholds, T, out, s);
     if (!rc) ctx->launches += 1;
     return rc;
 }

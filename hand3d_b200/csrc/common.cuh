@@ -81,6 +81,28 @@ __device__ __forceinline__ float rotate_canonical_point(const float* can_b, cons
     return cx * R[j] + cy * R[3 + j] + cz * R[6 + j];
 }
 
+// ---------------------------------------------------------------- EvalUtil.feed's distance (utils/general.py:541)
+// np.sqrt(np.sum(np.square(gt - pred), axis=1)) of one key-point in T (float or double): separately rounded subtract, multiply and add
+// from 0 (no FMA contraction), then a correctly rounded square root.
+__device__ __forceinline__ float rn_sub(float a, float b) { return __fsub_rn(a, b); }
+__device__ __forceinline__ float rn_mul(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ float rn_add(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ float rn_sqrt(float a) { return __fsqrt_rn(a); }
+__device__ __forceinline__ double rn_sub(double a, double b) { return __dsub_rn(a, b); }
+__device__ __forceinline__ double rn_mul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double rn_add(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double rn_sqrt(double a) { return __dsqrt_rn(a); }
+
+template <typename T>
+__device__ __forceinline__ T keypoint_dist(const T* __restrict__ gt, const T* __restrict__ pred, int D) {
+    T acc = T(0);
+    for (int d = 0; d < D; ++d) {
+        const T df = rn_sub(gt[d], pred[d]);
+        acc = rn_add(acc, rn_mul(df, df));
+    }
+    return rn_sqrt(acc);
+}
+
 // ---------------------------------------------------------------- launch counter
 struct LaunchCounter {
     int64_t n = 0;
@@ -148,6 +170,11 @@ struct FramePlan;   // opaque: the coefficients of one (Hf, Wf, h, w) on the dev
 FramePlan* frame_plan_create(int Hf, int Wf, int h, int w, cudaStream_t s);
 void frame_plan_destroy(FramePlan* p);
 int launch_resize_frames(const FramePlan* p, const uint8_t* frames, int B, int normalize, void* out, cudaStream_t s);
+
+// ---------------------------------------------------------------- kernels (eval.cu): EvalUtil's store and measures (arguments checked)
+int launch_eval_feed(void* store, int K, int N, int dtype, const void* gt, const uint8_t* vis, const void* pred, int n, int D,
+                     cudaStream_t s);
+int launch_eval_stats(const void* store, int K, int N, int dtype, const double* thr, int nthr, int64_t* out, cudaStream_t s);
 
 // ---------------------------------------------------------------- kernels (conv_direct.cu)
 struct DirectConvArgs {

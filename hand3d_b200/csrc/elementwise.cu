@@ -1006,12 +1006,8 @@ __global__ void eval_dist_kernel(const float* __restrict__ gt, const uint8_t* __
                                  int n, int D, float* __restrict__ dist) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    float acc = 0.f;
-    for (int d = 0; d < D; ++d) {
-        const float df = __fsub_rn(gt[(int64_t)i * D + d], pred[(int64_t)i * D + d]);
-        acc = __fadd_rn(acc, __fmul_rn(df, df));
-    }
-    dist[i] = vis[i] ? sqrtf(acc) : -1.0f;
+    const float d = keypoint_dist(gt + (int64_t)i * D, pred + (int64_t)i * D, D);
+    dist[i] = vis[i] ? d : -1.0f;
 }
 
 int launch_eval_dist(const float* gt, const uint8_t* vis, const float* pred, int n, int D, float* dist, cudaStream_t s) {

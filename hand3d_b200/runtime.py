@@ -738,6 +738,36 @@ class Context:
                    "h3d_eval_keypoint_dist")
         return dist
 
+    def eval_feed(self, store, num_kp, num_samples, gt, vis, pred):
+        """h3d_eval_feed: appends the distances of gt / pred [n, K, D] (float32 or float64, the store's dtype) where vis [n, K] (uint8,
+        nonzero = visible) to the store (a uint8 CUDA tensor of h3d_eval_store_bytes bytes).  Enqueue-only and capturable."""
+        dtype = {torch.float32: _lib.EVAL_FLOAT32, torch.float64: _lib.EVAL_FLOAT64}.get(gt.dtype)
+        if dtype is None or pred.dtype != gt.dtype:
+            raise TypeError("gt and pred must both be float32 or both float64, got %s and %s" % (gt.dtype, pred.dtype))
+        if vis.dtype != torch.uint8:
+            raise TypeError("vis must be uint8, got %s" % vis.dtype)
+        for t, name in ((store, "store"), (gt, "gt"), (vis, "vis"), (pred, "pred")):
+            if not t.is_cuda or not t.is_contiguous():
+                raise ValueError("%s must be a contiguous CUDA tensor" % name)
+        if gt.dim() != 3 or tuple(pred.shape) != tuple(gt.shape) or tuple(vis.shape) != tuple(gt.shape[:2]) or gt.shape[1] != num_kp:
+            raise ValueError("gt / pred must be [n, %d, D] and vis [n, %d], got %s, %s and %s"
+                             % (num_kp, num_kp, tuple(gt.shape), tuple(pred.shape), tuple(vis.shape)))
+        n, _, D = gt.shape
+        _lib.check(self.lib.h3d_eval_feed(self.h, _ptr(store), int(num_kp), int(num_samples), dtype, _ptr(gt), _ptr(vis), _ptr(pred), int(n),
+                                          int(D), _stream()), "h3d_eval_feed")
+
+    def eval_stats(self, store, num_kp, num_samples, dtype, thresholds):
+        """h3d_eval_stats: -> int64 [K, EVAL_STAT_COUNTS + T] on the device, per key-point n_k, the mean and median (float64 bit patterns)
+        and the threshold counts; thresholds is a float64 CUDA tensor [T]."""
+        code = {torch.float32: _lib.EVAL_FLOAT32, torch.float64: _lib.EVAL_FLOAT64}[dtype]
+        if thresholds.dtype != torch.float64 or not thresholds.is_cuda or thresholds.dim() != 1 or not thresholds.is_contiguous():
+            raise TypeError("thresholds must be a contiguous float64 CUDA tensor [T]")
+        T = thresholds.shape[0]
+        out = torch.empty((int(num_kp), _lib.EVAL_STAT_COUNTS + T), dtype=torch.int64, device=store.device)
+        _lib.check(self.lib.h3d_eval_stats(self.h, _ptr(store), int(num_kp), int(num_samples), code, _ptr(thresholds), int(T), _ptr(out),
+                                           _stream()), "h3d_eval_stats")
+        return out
+
     def bone_rel_trafo_inv(self, coords_rel):
         coords_rel = _chk_f32(coords_rel, "coords_rel")
         if coords_rel.dim() == 2:

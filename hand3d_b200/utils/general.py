@@ -16,7 +16,7 @@ import contextlib
 import numpy as np
 import torch
 
-from .. import runtime
+from .. import _lib, runtime
 
 _scope_stack = []
 
@@ -253,3 +253,130 @@ class EvalUtil:
             aucs.append(trapz(curve, thresholds) / norm_factor)
         return (np.mean(np.array(means)), np.mean(np.array(medians)), np.mean(np.array(aucs)), np.mean(np.array(curves), 0),
                 thresholds)
+
+
+def calc_auc(x, y):
+    """ utils/general.py:654-659: the trapezoid integral of y over x, normalised by the length of x. """
+    trapz = getattr(np, "trapezoid", None) or np.trapz
+    integral = trapz(y, x)
+    norm = trapz(np.ones_like(y), x)
+    return integral / norm
+
+
+def measures_from_stats(stats, val_min, val_max, steps, dtype):
+    """ EvalUtil.get_measures (utils/general.py:570-611) finished from per-key-point statistics.
+
+        stats is int64 [K, EVAL_STAT_COUNTS + steps] as h3d_eval_stats writes it: n_k, the mean and the median (float64 bit patterns
+        of values of `dtype`) and the counts of distances <= each threshold of np.linspace(val_min, val_max, steps).  A key-point's PCK
+        is count / n_k in float64, which is what np.mean of the reference's 0 / 1 array gives; the rest is the reference's own numpy.
+    """
+    trapz = getattr(np, "trapezoid", None) or np.trapz
+    dtype = np.dtype(dtype).type
+    stats = np.asarray(stats, dtype=np.int64)
+    thresholds = np.linspace(val_min, val_max, steps)
+    norm_factor = trapz(np.ones_like(thresholds), thresholds)
+    means, medians, aucs, curves = [], [], [], []
+    for row in stats:
+        n = row[_lib.EVAL_STAT_N]
+        if n == 0:
+            continue                          # no valid measurement for this key-point
+        means.append(dtype(row[_lib.EVAL_STAT_MEAN:_lib.EVAL_STAT_MEAN + 1].view(np.float64)[0]))
+        medians.append(dtype(row[_lib.EVAL_STAT_MEDIAN:_lib.EVAL_STAT_MEDIAN + 1].view(np.float64)[0]))
+        curve = np.array([np.float64(c) / np.float64(n) for c in row[_lib.EVAL_STAT_COUNTS:]])
+        curves.append(curve)
+        aucs.append(trapz(curve, thresholds) / norm_factor)
+    return (np.mean(np.array(means)), np.mean(np.array(medians)), np.mean(np.array(aucs)), np.mean(np.array(curves), 0),
+            thresholds)
+
+
+class DeviceEvalUtil:
+    """ EvalUtil with its distance lists kept on the device (h3d_eval_feed / h3d_eval_stats).
+
+        feed() only enqueues one kernel, so an evaluation loop can be captured into a CUDA graph; get_measures() makes one stats launch
+        and one small copy to the host.  The measures are bit-identical to the reference's EvalUtil fed the same arrays one sample at a
+        time: the distances are computed in numpy's promoted dtype of gt and pred (float32, or float64 if either is), np.mean and
+        np.median are restated exactly, and the PCK curve and AUC are the reference's own numpy over those values.
+
+        The store holds num_samples samples: rows fed past that are dropped (counted in `dropped`), so a loop whose last batch wraps
+        around the dataset counts every sample once.
+    """
+    def __init__(self, num_kp=21, num_samples=None):
+        if num_samples is None:
+            raise TypeError("DeviceEvalUtil needs num_samples: its store holds num_kp x num_samples distances")
+        num_kp, num_samples = int(num_kp), int(num_samples)
+        if not 1 <= num_kp <= _lib.EVAL_MAX_KP:
+            raise ValueError("num_kp = %d, the device store holds 1..%d key-points" % (num_kp, _lib.EVAL_MAX_KP))
+        if not 1 <= num_samples <= _lib.EVAL_MAX_SAMPLES:
+            raise ValueError("num_samples = %d, the device store holds 1..%d samples" % (num_samples, _lib.EVAL_MAX_SAMPLES))
+        self.num_kp, self.num_samples = num_kp, num_samples
+        self.dtype = None          # torch dtype of the distances, fixed by the first feed
+        self._store = None
+        self._ctx = None
+
+    def _header(self):
+        return self._store[:_lib.EVAL_HEADER_WORDS * 8].view(torch.int64)
+
+    def feed(self, keypoint_gt, keypoint_vis, keypoint_pred):
+        """ keypoint_gt / keypoint_pred CUDA [B,K,D] or [K,D], keypoint_vis [B,K] or [K] (nonzero = visible). """
+        for t, name in ((keypoint_gt, "keypoint_gt"), (keypoint_vis, "keypoint_vis"), (keypoint_pred, "keypoint_pred")):
+            if not torch.is_tensor(t) or not t.is_cuda:
+                raise TypeError("DeviceEvalUtil.feed: %s must be a CUDA tensor" % name)
+        dtype = torch.promote_types(keypoint_gt.dtype, keypoint_pred.dtype)
+        if dtype not in (torch.float32, torch.float64):
+            raise TypeError("DeviceEvalUtil.feed: gt %s and pred %s promote to %s; the distances are float32 or float64"
+                            % (keypoint_gt.dtype, keypoint_pred.dtype, dtype))
+        K = self.num_kp
+        gt = keypoint_gt.reshape(-1, K, keypoint_gt.shape[-1])
+        pred = keypoint_pred.reshape(gt.shape)
+        vis = keypoint_vis.reshape(gt.shape[0], K)
+        if self._store is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("DeviceEvalUtil: the first feed allocates the store and must run eagerly (GraphedIteration's "
+                                   "warm-up calls do), not under graph capture")
+            self._ctx = runtime.default_context()
+            code = _lib.EVAL_FLOAT64 if dtype == torch.float64 else _lib.EVAL_FLOAT32
+            nbytes = self._ctx.lib.h3d_eval_store_bytes(K, self.num_samples, code)
+            if nbytes < 0:
+                raise ValueError(_lib.last_error())
+            self._store = torch.empty(nbytes, dtype=torch.uint8, device=gt.device)
+            self._header().zero_()
+            self.dtype = dtype
+        elif dtype != self.dtype:
+            raise TypeError("DeviceEvalUtil: the store holds %s distances, this feed gives %s" % (self.dtype, dtype))
+        self._ctx.eval_feed(self._store, K, self.num_samples, gt.to(dtype).contiguous(), (vis != 0).to(torch.uint8).contiguous(),
+                            pred.to(dtype).contiguous())
+
+    def reset(self):
+        """ Empties the store (a memset of its header; capturable). """
+        if self._store is not None:
+            self._header().zero_()
+
+    @property
+    def kept(self):
+        """ Samples stored so far (synchronises). """
+        return 0 if self._store is None else int(self._header()[_lib.EVAL_KEPT])
+
+    @property
+    def dropped(self):
+        """ Samples fed past num_samples and not stored (synchronises). """
+        return 0 if self._store is None else int(self._header()[_lib.EVAL_DROPPED])
+
+    def lists(self):
+        """ The per-key-point distance lists as numpy arrays (synchronises): what EvalUtil.data holds. """
+        if self._store is None:
+            return [np.zeros(0, np.float32) for _ in range(self.num_kp)]
+        hdr = self._header().cpu().numpy()
+        data = self._store[_lib.EVAL_HEADER_WORDS * 8:].view(self.dtype).reshape(self.num_kp, self.num_samples)
+        return [data[k, :hdr[_lib.EVAL_COUNT + k]].cpu().numpy() for k in range(self.num_kp)]
+
+    def get_measures(self, val_min, val_max, steps):
+        """ (mean EPE, median EPE, AUC, PCK curve, thresholds), as EvalUtil.get_measures returns them.  Not under graph capture. """
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("DeviceEvalUtil.get_measures copies its result to the host and cannot run under graph capture")
+        thresholds = np.linspace(val_min, val_max, steps)
+        if self._store is None:
+            return measures_from_stats(np.zeros((self.num_kp, _lib.EVAL_STAT_COUNTS + len(thresholds)), np.int64), val_min, val_max,
+                                       steps, np.float32)
+        thr = torch.from_numpy(thresholds).to(self._store.device)
+        stats = self._ctx.eval_stats(self._store, self.num_kp, self.num_samples, self.dtype, thr).cpu().numpy()
+        return measures_from_stats(stats, val_min, val_max, steps, np.float64 if self.dtype == torch.float64 else np.float32)

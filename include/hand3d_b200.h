@@ -366,6 +366,44 @@ H3D_API int h3d_canonical_trafo(h3d_ctx* ctx, const float* coords_xyz, const uin
  * dist [n] = ||gt - pred||_2, or -1 where the key-point is not visible. */
 H3D_API int h3d_eval_keypoint_dist(h3d_ctx* ctx, const float* gt, const uint8_t* vis, const float* pred, int n, int D, float* dist,
                                    void* stream);
+/* ---- EvalUtil on the device (utils/general.py:522-611): a store of per-key-point distance lists and its measures ----
+ * A store is caller-owned DEVICE memory of h3d_eval_store_bytes(K, num_samples, dtype) bytes:
+ *   int64 header [H3D_EVAL_HEADER_WORDS]: [H3D_EVAL_KEPT] samples kept, [H3D_EVAL_DROPPED] rows dropped, [H3D_EVAL_TICKET] scratch
+ *   of h3d_eval_feed (0 between calls), [H3D_EVAL_COUNT + k] distances held for key-point k;
+ *   then K x num_samples distance slots of the store's dtype: key-point k's list at slot k * num_samples.
+ * Zeroing the header (a memset of H3D_EVAL_HEADER_WORDS * 8 bytes) resets the store.  dtype is H3D_EVAL_FLOAT32 or H3D_EVAL_FLOAT64;
+ * 1 <= K <= H3D_EVAL_MAX_KP, 1 <= num_samples <= H3D_EVAL_MAX_SAMPLES, 1 <= D <= H3D_EVAL_MAX_DIM, 1 <= T <= H3D_EVAL_MAX_THRESHOLDS;
+ * anything else is H3D_EINVAL. */
+#define H3D_EVAL_FLOAT32 0
+#define H3D_EVAL_FLOAT64 1
+#define H3D_EVAL_KEPT 0
+#define H3D_EVAL_DROPPED 1
+#define H3D_EVAL_TICKET 2
+#define H3D_EVAL_COUNT 8
+#define H3D_EVAL_HEADER_WORDS 72
+#define H3D_EVAL_MAX_KP 64
+#define H3D_EVAL_MAX_DIM 4
+#define H3D_EVAL_MAX_SAMPLES 16777216
+#define H3D_EVAL_MAX_THRESHOLDS 4096
+/* h3d_eval_stats output: int64 [K][H3D_EVAL_STAT_COUNTS + T]; the mean and median are float64 bit patterns (exact for float32). */
+#define H3D_EVAL_STAT_N 0
+#define H3D_EVAL_STAT_MEAN 1
+#define H3D_EVAL_STAT_MEDIAN 2
+#define H3D_EVAL_STAT_COUNTS 3
+/* Bytes of a store, or H3D_EINVAL (< 0) outside the limits. */
+H3D_API int64_t h3d_eval_store_bytes(int K, int num_samples, int dtype);
+/* EvalUtil.feed of n samples: gt / pred [n, K, D] and vis [n, K] u8 (nonzero = visible), contiguous, in the store's dtype (device).
+ * Key-point k of sample r gets np.sqrt(np.sum(np.square(gt - pred), axis=1)) in that dtype (as h3d_eval_keypoint_dist, in float64 too),
+ * appended to its list when visible: lists grow in feed order, then sample order, as the reference's per-sample loop appends.  Samples
+ * past the store's num_samples are not stored but counted as dropped.  No atomics decide positions: the store is deterministic.
+ * One kernel, enqueue-only and capturable. */
+H3D_API int h3d_eval_feed(h3d_ctx* ctx, void* store, int K, int num_samples, int dtype, const void* gt, const uint8_t* vis,
+                          const void* pred, int n, int D, void* stream);
+/* The measures of every key-point k with n_k > 0 (one kernel): n_k, np.mean of its list (numpy 2.x pairwise summation, then / n_k, in
+ * the store's dtype), np.median (the middle order statistic, or (a + b) / 2 in the store's dtype; NaN if the list holds NaN) and
+ * counts[t] = #{d : float64(d) <= thresholds[t]} for thresholds [T] float64 (device).  A key-point with no data gets a row of zeros. */
+H3D_API int h3d_eval_stats(h3d_ctx* ctx, const void* store, int K, int num_samples, int dtype, const double* thresholds, int T,
+                           int64_t* out, void* stream);
 /* bone_rel_trafo_inv (utils/relative_trafo.py:243-295): coords_rel [B,21,3] (length, angle_x, angle_y) -> xyz [B,21,3]. */
 H3D_API int h3d_bone_rel_trafo_inv(h3d_ctx* ctx, const float* coords_rel, float* coords_xyz, int B, void* stream);
 /* _get_rot_mat + _flip_right_hand + matmul (nets/ColorHandPose3DNetwork.py:239-247,311-384). */
