@@ -460,8 +460,8 @@ static int add_tc(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, const L
     d.corr_scale = pw->corr_scale;
     d.pool = pool;
     d.err_flag = ctx->err_flag;
-    TcConvPlan* tp = tc_conv_plan_create(d);
-    if (!tp) return H3D_ECUDA;
+    TcConvPlan* tp = tc_conv_plan_create(d, &rc);
+    if (!tp) return rc;
     pl->tc.push_back(tp);
     pl->steps.push_back([tp](const Ext&, cudaStream_t s) { return tc_conv_launch(tp, s); });
     pl->launches.push_back(1);
@@ -969,7 +969,7 @@ static int check_device() {
 extern "C" {
 
 const char* h3d_last_error(void) { return g_err; }
-int h3d_version(void) { return 105; }
+int h3d_version(void) { return 106; }
 
 int h3d_device_available(void) {
     int n = 0;
@@ -1379,8 +1379,8 @@ static int conv_tc_run(h3d_ctx* ctx, const float* x, float* y, int B, int H, int
     d.B = B; d.H = H; d.W = W; d.k = ksize; d.leaky = leaky; d.passes = passes; d.half = half; d.corr_scale = pw.corr_scale;
     d.pool = stride == 2 ? 2 : 0;
     d.err_flag = ctx->err_flag;
-    TcConvPlan* tp = tc_conv_plan_create(d);     // host-side only: tensor maps + launch geometry (passed to the kernel by value)
-    if (!tp) return H3D_ECUDA;
+    TcConvPlan* tp = tc_conv_plan_create(d, &rc);     // host-side only: tensor maps + launch geometry (passed to the kernel by value)
+    if (!tp) return rc;
     rc = tc_conv_launch(tp, s);
     tc_conv_plan_destroy(tp);
     if (rc) return rc;
@@ -1475,8 +1475,8 @@ int h3d_conv2d_tc_backward(h3d_ctx* ctx, const float* x, const float* y, const f
         d.y = Split(); d.Cy_total = 0; d.cy_off = 0; d.yf = dx; d.Cyf_total = Cin; d.cyf_off = 0;
         d.B = B; d.H = H; d.W = W; d.k = ksize; d.leaky = 0; d.passes = passes; d.half = Half16::BF16; d.pool = 0;
         d.err_flag = ctx->err_flag;
-        TcConvPlan* tp = tc_conv_plan_create(d);
-        if (!tp) return H3D_ECUDA;
+        TcConvPlan* tp = tc_conv_plan_create(d, &rc);
+        if (!tp) return rc;
         rc = tc_conv_launch(tp, s);
         tc_conv_plan_destroy(tp);
         if (rc) return rc;
@@ -1510,6 +1510,85 @@ int h3d_conv2d_tc_strided(h3d_ctx* ctx, const float* x, const float* host_w_hwio
     if (rc) return rc;
     rc = h3d_conv2d_tc_packed(ctx, x, pk, y, B, H, W, stride, leaky, stream);
     h3d_free_packed_conv(ctx, pk);               // host-weight convenience entry: the free waits for the kernel (documented exception)
+    return rc;
+}
+
+// One network layer as build_trunk / build_handsegnet / build_posenet issue it through add_tc (route 0) or add_direct (route 1), with
+// the layer's planes, channel offsets, fused pool and input permutation given explicitly instead of taken from a stage plan.
+int h3d_conv2d_layer_planes(h3d_ctx* ctx, const float* x, int B, int H, int W, int Cx, const float* host_w_hwio, const float* host_bias,
+                            int ksize, int Cin, int Cout, const int32_t* host_perm, int pool, int leaky, int precision, int route,
+                            void* y_hi, void* y_lo, void* y_l8, void* y_h8, int Cy_total, int cy_off, float* yf, int Cyf_total,
+                            int cyf_off, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(x && host_w_hwio && host_bias && B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && Cx >= Cin,
+                "h3d_conv2d_layer_planes: bad argument");
+    H3D_REQUIRE(precision >= H3D_PREC_BF16X3 && precision <= H3D_PREC_FP16_F8C, "h3d_conv2d_layer_planes: precision must be a tensor-core mode");
+    H3D_REQUIRE(ksize == 1 || ksize == 3 || ksize == 5 || ksize == 7, "h3d_conv2d_layer_planes: ksize must be 1, 3, 5 or 7");
+    H3D_REQUIRE(route == 0 || route == 1, "h3d_conv2d_layer_planes: route must be 0 (tensor-core layer) or 1 (CUDA-core / first layer)");
+    H3D_REQUIRE(y_hi || yf, "h3d_conv2d_layer_planes: no output requested");
+    const int passes = passes_of(precision);
+    const Half16 half = half_of(precision);
+    // the planes of the precision's format, as slot_view lays them out: other plane pointers are ignored (never written)
+    Split ys;
+    if (y_hi) {
+        H3D_REQUIRE(passes != 3 || y_lo, "h3d_conv2d_layer_planes: this precision writes a lo plane");
+        H3D_REQUIRE(passes != 4 || (y_l8 && y_h8), "h3d_conv2d_layer_planes: fp16_f8c writes l8 and h8 planes");
+        ys.hi = (uint16_t*)y_hi;
+        if (passes == 3) ys.lo = (uint16_t*)y_lo;
+        if (passes == 4) { ys.l8 = (uint8_t*)y_l8; ys.h8 = (uint8_t*)y_h8; }
+    }
+    const int64_t rows = (int64_t)B * H * W;
+    char* base = nullptr;
+    int rc;
+    if (route == 1) {
+        H3D_REQUIRE(pool == 0 && !host_perm, "h3d_conv2d_layer_planes: route 1 has no fused pool and no input permutation");
+        const int64_t wn = (int64_t)ksize * ksize * Cin * Cout, wb = align_up(wn * 4, 1024);
+        if ((rc = op_scratch(ctx, wb + Cout * 4, &base))) return rc;
+        float* w = (float*)base; float* b = (float*)(base + wb);
+        H3D_CUDA(cudaMemcpyAsync(w, host_w_hwio, wn * 4, cudaMemcpyHostToDevice, s));   // pageable: returns once the source is staged
+        H3D_CUDA(cudaMemcpyAsync(b, host_bias, Cout * 4, cudaMemcpyHostToDevice, s));
+        DirectConvArgs a;
+        a.x = x; a.Cin_total = Cx; a.cin_off = 0; a.w = w; a.bias = b; a.y = yf; a.Cout_total = Cyf_total; a.cout_off = cyf_off;
+        a.ys = ys; a.Cs_total = Cy_total; a.cs_off = cy_off; a.half = half;
+        a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.k = ksize; a.stride = 1; a.leaky = leaky;
+        a.err_flag = ctx->err_flag;
+        if ((rc = launch_conv_direct(a, s))) return rc;
+        ctx->launches += conv_direct_num_launches(a);
+        return H3D_OK;
+    }
+    const int Cin_pad = (int)align_up(Cin, 64), Cout_pad = (int)align_up(Cout, 64);
+    H3D_REQUIRE(Cin_pad <= Cx && Cx % 16 == 0, "h3d_conv2d_layer_planes: x needs Cx >= align_up(Cin, 64) channels, Cx a multiple of 16");
+    std::vector<int> perm;
+    if (host_perm) {
+        perm.assign(host_perm, host_perm + Cin_pad);
+        for (int v : perm) H3D_REQUIRE(v >= -1 && v < Cin, "h3d_conv2d_layer_planes: perm entries must lie in [-1, Cin)");
+    }
+    // operator scratch: the input planes [hi | lo] or [fp16 | l8 | h8] with Cin_total = Cx
+    const int64_t xb = align_up(rows * Cx * 2, 1024), x8 = align_up(rows * Cx, 1024);
+    if ((rc = op_scratch(ctx, 2 * xb + (passes == 4 ? x8 : 0), &base))) return rc;
+    Split xs;
+    xs.hi = (uint16_t*)base;
+    if (passes == 3) xs.lo = (uint16_t*)(base + xb);
+    if (passes == 4) { xs.l8 = (uint8_t*)(base + xb); xs.h8 = xs.l8 + x8; }
+    if ((rc = launch_f32_to_split(x, xs, rows, Cx, Cx, half, s))) return rc;
+    ctx->launches += 1;
+    PackedW pw;
+    if ((rc = pack_conv_weights(host_w_hwio, host_bias, ksize, Cin, Cout, Cin_pad, Cout_pad, perm, half, passes, &pw))) {
+        free_packed(pw);
+        return rc;
+    }
+    TcConvDesc d;
+    d.x = xs; d.Cin_total = Cx; d.Cin_pad = Cin_pad; d.w = pw.w; d.bias = pw.bias; d.w_scale = pw.w_scale; d.Cout = Cout; d.Cout_pad = Cout_pad;
+    d.y = ys; d.Cy_total = Cy_total; d.cy_off = cy_off; d.yf = yf; d.Cyf_total = Cyf_total; d.cyf_off = cyf_off;
+    d.B = B; d.H = H; d.W = W; d.k = ksize; d.leaky = leaky; d.passes = passes; d.half = half; d.corr_scale = pw.corr_scale; d.pool = pool;
+    d.err_flag = ctx->err_flag;
+    TcConvPlan* tp = tc_conv_plan_create(d, &rc);
+    if (tp) {
+        rc = tc_conv_launch(tp, s);
+        tc_conv_plan_destroy(tp);
+        if (!rc) ctx->launches += 1;
+    }
+    free_packed(pw);   // host weights: the free waits for the kernel, as in h3d_conv2d_tc
     return rc;
 }
 

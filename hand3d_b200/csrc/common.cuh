@@ -261,7 +261,9 @@ FcChainPlan* fc_chain_plan_create(const FcChainDesc* chains, int num_chains, int
                                   unsigned int* counter, int* err_flag);
 void fc_chain_plan_destroy(FcChainPlan* p);
 int fc_chain_launch(const FcChainPlan* p, const float* hand_side, float* rot, float* out, cudaStream_t s);
-TcConvPlan* tc_conv_plan_create(const TcConvDesc& d);   // nullptr on failure (h3d_last_error set)
+// nullptr on failure (h3d_last_error set); *rc (optional): H3D_EINVAL for an illegal descriptor, H3D_ECUDA when a tensor map
+// cannot be encoded, H3D_OK on success
+TcConvPlan* tc_conv_plan_create(const TcConvDesc& d, int* rc = nullptr);
 void tc_conv_plan_destroy(TcConvPlan* p);
 int tc_conv_launch(const TcConvPlan* p, cudaStream_t s);
 int64_t tc_conv_flops(const TcConvPlan* p);

@@ -813,7 +813,10 @@ int launch_inst(const TcConvPlan* pl, cudaStream_t s) {
 }
 }  // namespace
 
-TcConvPlan* tc_conv_plan_create(const TcConvDesc& d) {
+TcConvPlan* tc_conv_plan_create(const TcConvDesc& d, int* rc) {
+    int rc_local;
+    if (!rc) rc = &rc_local;
+    *rc = H3D_EINVAL;   // every early return below is an illegal descriptor
     if (d.Cin_pad % BK != 0 || d.Cout_pad % 64 != 0 || (d.k != 1 && d.k != 3 && d.k != 5 && d.k != 7) || (d.passes != 1 && d.passes != 3 && d.passes != 4)) {
         set_error("tc_conv: unsupported geometry (Cin_pad=%d Cout_pad=%d k=%d passes=%d)", d.Cin_pad, d.Cout_pad, d.k, d.passes);
         return nullptr;
@@ -833,6 +836,7 @@ TcConvPlan* tc_conv_plan_create(const TcConvDesc& d) {
     if (d.passes == 4 && d.y.hi && (!d.y.l8 || !d.y.h8)) { set_error("tc_conv: fp8-correction mode needs l8/h8 output planes"); return nullptr; }
     if (d.passes == 4 && d.y.hi && ((d.Cy_total % 16) || (d.cy_off % 16))) { set_error("tc_conv: fp8 planes need 16-channel aligned offsets"); return nullptr; }
     if (d.pool && ((d.H | d.W) & 1)) { set_error("tc_conv: fused max-pool / stride 2 needs even H and W"); return nullptr; }
+    *rc = H3D_ECUDA;    // from here on only a tensor-map encode can fail
     TcConvPlan* pl = new TcConvPlan();
     pl->d = d;
     const TcTuning& tune = tc_tuning();
@@ -881,6 +885,7 @@ TcConvPlan* tc_conv_plan_create(const TcConvDesc& d) {
     if (ok && d.passes == 1) { pl->map_x_lo = pl->map_x_hi; pl->map_w_lo = pl->map_w_hi; }
     if (ok && d.passes != 4) { pl->map_x_h8 = pl->map_x_hi; pl->map_w_l8 = pl->map_w_hi; }
     if (!ok) { delete pl; return nullptr; }
+    *rc = H3D_OK;
     return pl;
 }
 

@@ -307,6 +307,57 @@ class Context:
                                               PRECISIONS[precision], _stream()), "h3d_conv2d_tc_dev")
         return y
 
+    # plane canaries of conv_layer: NaN bit patterns in every format, which no layer output of finite operands takes
+    CANARY16, CANARY8, CANARY32 = 0x7FA5, 0x7F, 0x7FC0A5A5
+
+    def conv_layer(self, x, w_host, b_host, precision, route=0, pool=0, leaky=True, perm=None, planes=True, Cy_total=None, cy_off=0,
+                   yf=False, Cyf_total=None, cyf_off=0, out=None):
+        """One network layer as the stage entries build it (h3d_conv2d_layer_planes): x fp32 [B,H,W,Cx] on the device, host weights
+        HWIO [k,k,Cin,Cout].  Returns {"hi", "lo", "l8", "h8", "yf"}: the raw planes (uint16 / uint8 [B,Ho,Wo,Cy_total], all four
+        whatever the precision, so a test can see which ones were written) and the fp32 output [B,Ho,Wo,Cyf_total], each None when not
+        requested.  Buffers come from `out` (a dict of the same keys) or are filled with the CANARY* patterns."""
+        x = _chk_f32(x, "x", 4)
+        w = np.ascontiguousarray(w_host, np.float32); b = np.ascontiguousarray(b_host, np.float32)
+        B, H, W, Cx = x.shape
+        k, _, Cin, Cout = w.shape
+        Ho, Wo = (H // 2, W // 2) if pool else (H, W)
+        Cout_pad = -(-Cout // 64) * 64
+        out = dict(out or {})
+        dev = x.device
+
+        def buf(key, C, dtype, fill):
+            if out.get(key) is None:
+                t = torch.empty((B, Ho, Wo, C), dtype=dtype, device=dev)
+                t.view(torch.int32 if dtype == torch.float32 else dtype).fill_(fill)
+                out[key] = t
+            return out[key]
+        if planes:
+            Cy_total = Cout_pad if Cy_total is None else Cy_total
+            for key in ("hi", "lo"):
+                buf(key, Cy_total, torch.int16, self.CANARY16)
+            for key in ("l8", "h8"):
+                buf(key, Cy_total, torch.uint8, self.CANARY8)
+        else:
+            Cy_total = 0
+            for key in ("hi", "lo", "l8", "h8"):
+                out[key] = None
+        if yf:
+            Cyf_total = Cout if Cyf_total is None else Cyf_total
+            buf("yf", Cyf_total, torch.float32, self.CANARY32)
+        else:
+            Cyf_total, out["yf"] = 0, None
+        p = None
+        if perm is not None:
+            p = np.ascontiguousarray(perm, np.int32)
+            if p.shape != (-(-Cin // 64) * 64,):
+                raise ValueError("conv_layer: perm must have align_up(Cin, 64) = %d entries, got %s" % (-(-Cin // 64) * 64, p.shape))
+        _lib.check(self.lib.h3d_conv2d_layer_planes(
+            self.h, _ptr(x), B, H, W, Cx, w.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p), k, Cin, Cout,
+            None if p is None else p.ctypes.data_as(C.c_void_p), int(pool), int(bool(leaky)), PRECISIONS[precision], int(route),
+            _ptr(out["hi"]), _ptr(out["lo"]), _ptr(out["l8"]), _ptr(out["h8"]), int(Cy_total), int(cy_off), _ptr(out["yf"]),
+            int(Cyf_total), int(cyf_off), _stream()), "h3d_conv2d_layer_planes")
+        return out
+
     def conv2d_tc_backward(self, x, y, dy, w, stride=1, leaky=False, precision="bf16x3", need_dx=True, need_dw=True, need_db=True):
         """Gradients (dx, dw, db) of y = act(conv_SAME(x, w, stride) + b); outputs not needed come back as None.  y (the forward
         output) is read only with leaky, x only for dw, w only for dx."""

@@ -14,7 +14,7 @@
  *     workspace arena of the stage entry points; operator entry points borrow scratch from a context-owned buffer that only
  *     ever grows (old blocks are retired until h3d_destroy), so consecutive operator calls on one context must be ordered by
  *     the caller when they run on different streams.  Documented exceptions: h3d_load_weight, h3d_pack_conv_weights and the
- *     host-weight convenience entry h3d_conv2d_tc(_strided) upload weights (allocate + copy);
+ *     host-weight convenience entries h3d_conv2d_tc(_strided) and h3d_conv2d_layer_planes upload weights (allocate + copy);
  *   - return 0 on success, negative H3D_E* on failure; h3d_last_error() gives a thread-local message;
  *   - one h3d_ctx per device, used from one host thread at a time (one rank <-> one GPU); every entry makes the context's device
  *     current for the duration of the call and restores the caller's device;
@@ -173,6 +173,24 @@ H3D_API int h3d_conv2d_tc_packed(h3d_ctx* ctx, const float* x, const h3d_packed_
  * h3d_conv2d_tc_packed for the same weights.  precision: bf16x3, fp16x3, fp16 or bf16. */
 H3D_API int h3d_conv2d_tc_dev(h3d_ctx* ctx, const float* x, const float* w_hwio, const float* bias, float* y, int B, int H, int W,
                               int Cin, int Cout, int ksize, int stride, int leaky, int precision, void* stream);
+/* One network layer as the stage entries build it, with its raw output planes (for tests of the layer paths the stage plans use).
+ * x fp32 [B,H,W,Cx]; host_w_hwio [k,k,Cin,Cout] and host_bias [Cout] are HOST pointers.  precision: a tensor-core mode.
+ * route 0: the wgmma layer.  x is split on the device into the precision's planes with Cin_total = Cx (Cx % 16 == 0); the layer reads
+ *   channels [0, Cin_pad), Cin_pad = align_up(Cin, 64) <= Cx.  host_perm (NULL = identity) is host int32 [Cin_pad]: packed input
+ *   channel j takes weight row host_perm[j], -1 = a zero row (PoseNet2D's conv6_1 / conv7_1 read the concat planes this way).
+ *   pool: 0, 1 = fused 2x2 max-pool, 2 = stride 2; outputs are [B,H/2,W/2,.] when pool != 0.
+ * route 1: the CUDA-core layer; a 3x3, 3 -> 64 layer runs the first-layer kernels (the tensor-core one when only planes are
+ *   requested, the FFMA one with yf, with the c3_ffma switch, or in fp16_f8c).  pool must be 0 and host_perm NULL.
+ * Outputs (each optional, at least one): planes [B,Ho,Wo,Cy_total] at channel offset cy_off, y_hi (uint16) always, y_lo (uint16) in
+ * bf16x3 / fp16x3, y_l8 and y_h8 (uint8) in fp16_f8c; plane pointers the precision does not use are never written.  Route 0 writes
+ * Cout_pad = align_up(Cout, 64) plane channels, the padding ones as zeros; yf fp32 [B,Ho,Wo,Cyf_total] gets Cout channels at cyf_off.
+ * Descriptor errors (alignment of the offsets, pool with Cout % 32 != 0 or odd H / W, ...) return H3D_EINVAL.  Like h3d_conv2d_tc, the
+ * call uploads the host weights and frees them afterwards (the free waits for the kernel); the input planes live in the operator
+ * scratch. */
+H3D_API int h3d_conv2d_layer_planes(h3d_ctx* ctx, const float* x, int B, int H, int W, int Cx, const float* host_w_hwio,
+                                    const float* host_bias, int ksize, int Cin, int Cout, const int32_t* host_perm, int pool, int leaky,
+                                    int precision, int route, void* y_hi, void* y_lo, void* y_l8, void* y_h8, int Cy_total, int cy_off,
+                                    float* yf, int Cyf_total, int cyf_off, void* stream);
 /* Gradients of y = act(conv_SAME(x, w, stride) + b) (act: identity, or leaky ReLU 0.01 when leaky), the TF Conv2DBackpropInput,
  * Conv2DBackpropFilter, BiasAddGrad and Maximum gradients that AdamOptimizer.minimize evaluates (training_posenet.py:67,
  * training_handsegnet.py).  x [B,H,W,Cin], y and dy [B,H/stride,W/stride,Cout], w_hwio [k,k,Cin,Cout], all fp32 device tensors;
