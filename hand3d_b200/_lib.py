@@ -105,6 +105,8 @@ AUG_UV_NOISE, AUG_CENTER_NOISE, AUG_SCALE, AUG_OFFSET_NOISE, AUG_HUE_DELTA, AUG_
 READER_QUEUE_CAPACITY, READER_STATE_COUNT, READER_STATE_NEXT, READER_STATE_SLOTS, READER_STATE_WORDS, READER_MAX_GATHER = 100, 0, 1, 2, 102, 4096
 # camera frames (H3D_FRAME_*): the largest frame side and output side of h3d_resize_frames
 FRAME_MAX_SIDE, FRAME_MAX_OUT = 4096, 512
+# the largest image side of h3d_pipeline_forward and h3d_seg_postprocess (H3D_PIPELINE_MAX_SIDE)
+PIPELINE_MAX_SIDE = 2048
 # device evaluation store (H3D_EVAL_*): dtypes, the header layout, the limits and the layout of a stats row
 EVAL_FLOAT32, EVAL_FLOAT64 = 0, 1
 EVAL_KEPT, EVAL_DROPPED, EVAL_TICKET, EVAL_COUNT, EVAL_HEADER_WORDS = 0, 1, 2, 8, 72

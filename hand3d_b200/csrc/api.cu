@@ -969,7 +969,7 @@ static int check_device() {
 extern "C" {
 
 const char* h3d_last_error(void) { return g_err; }
-int h3d_version(void) { return 106; }
+int h3d_version(void) { return 107; }
 
 int h3d_device_available(void) {
     int n = 0;
@@ -1234,6 +1234,8 @@ int h3d_pipeline_forward(h3d_ctx* ctx, const float* image, const float* hand_sid
     DeviceGuard guard_(ctx ? ctx->device : 0);
     H3D_REQUIRE(ctx && image && B > 0, "h3d_pipeline_forward: bad argument");
     H3D_REQUIRE(!with_pose3d || (hand_side && keypoint_coord3d), "h3d_pipeline_forward: hand_side / keypoint_coord3d required with pose3d");
+    H3D_REQUIRE(H >= 1 && W >= 1 && H <= H3D_PIPELINE_MAX_SIDE && W <= H3D_PIPELINE_MAX_SIDE,
+                "h3d_pipeline_forward: images must be 1..%d pixels a side (H3D_PIPELINE_MAX_SIDE), got %dx%d", H3D_PIPELINE_MAX_SIDE, H, W);
     cudaStream_t s = (cudaStream_t)stream;
     int rc;
     if ((rc = ensure_layout_covers(ctx, B, H, W, 256, 256))) return rc;
@@ -1639,6 +1641,9 @@ int h3d_seg_postprocess(h3d_ctx* ctx, const float* logits, int B, int H, int W, 
                         float* crop_size, float* scale_crop, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(logits && center && scale_crop, "h3d_seg_postprocess: logits, center and scale_crop are required");
+    H3D_REQUIRE(B > 0 && H >= 1 && W >= 1 && H <= H3D_PIPELINE_MAX_SIDE && W <= H3D_PIPELINE_MAX_SIDE,
+                "h3d_seg_postprocess: maps must be 1..%d pixels a side (H3D_PIPELINE_MAX_SIDE), got B=%d %dx%d", H3D_PIPELINE_MAX_SIDE, B, H,
+                W);
     char* scratch = nullptr;
     int rc = op_scratch(ctx, seg_scratch_bytes(B, H, W), &scratch);
     if (rc) return rc;

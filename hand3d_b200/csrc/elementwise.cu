@@ -5,6 +5,8 @@
 // All arithmetic that feeds a discrete decision or an interpolated output uses explicit
 // __fmul_rn/__fadd_rn/__fsub_rn so that nvcc cannot contract to FMA: the TF-1.3 CPU kernels the
 // oracle restates use separate multiply and add (SURVEY.md section 9).
+#include <cooperative_groups.h>
+
 #include "common.cuh"
 #include "split_fmt.cuh"
 
@@ -587,11 +589,225 @@ mask_grow_kernel(const unsigned long long* __restrict__ key, const uint32_t* __r
     }
 }
 
+// Kernel 2' (mask_grow_cluster_kernel, max(H, W) > 512): the same passes on one thread-block cluster per image.  CTA `rank` owns the
+// band of rows [row0, row0 + n) (H split evenly over the cluster, every band >= 16 rows when the cluster has more than one CTA) and keeps
+// that band's det, obj and hor words in its own shared memory.  A pass is the single-CTA pass: the horizontal widening into hor, a
+// cluster barrier, the 10 hor rows above and below the band copied from the neighbouring CTAs' shared memory (distributed shared memory)
+// into the band's padding rows, the vertical OR AND det; every CTA ORs its "changed" vote into word pass & 1 of rank 0 and a second
+// cluster barrier publishes it.  Rank 0 clears the other vote word after the first barrier of a pass: all CTAs have read it (after the
+// second barrier of the previous pass), and nobody writes it before the first barrier of the next pass.  Every CTA reads the same word
+// at the same point, so all leave the loop together.  Bounding boxes are reduced into rank 0 and the last access to a peer's shared
+// memory precedes the final cluster barrier, so no CTA exits while a peer may still read it.
+constexpr int kGrowClusterMax = 8;      // portable cluster size
+constexpr int kGrowBandMinRows = 16;    // >= the 10-row halo: a band's halo comes from its two neighbours only
+__host__ __device__ inline int grow_cluster_size(int H) {
+    const int c = H / kGrowBandMinRows;
+    return c < 1 ? 1 : c > kGrowClusterMax ? kGrowClusterMax : c;
+}
+// shared memory of one CTA: det, obj [bp][Ww] and hor [10 + bp + 17][Ww] for the largest band (bp = rows rounded up to 8)
+__host__ __device__ inline size_t grow_cluster_smem_bytes(int H, int Ww) {
+    const int cs = grow_cluster_size(H);
+    return grow_smem_bytes((H + cs - 1) / cs, Ww);
+}
+
+__global__ void __launch_bounds__(kGrowThreads, 1)
+mask_grow_cluster_kernel(const unsigned long long* __restrict__ key, const uint32_t* __restrict__ det_g, int H, int W, int Ww,
+                         int num_passes, uint8_t* __restrict__ hand_mask, int32_t* __restrict__ max_loc, float* __restrict__ center,
+                         float* __restrict__ crop_size, float* __restrict__ scale_crop) {
+    namespace cg = cooperative_groups;
+    cg::cluster_group cluster = cg::this_cluster();
+    extern __shared__ uint32_t sm[];
+    __shared__ int s_box[4];                 // rmin, rmax, cmin, cmax: the CTA's band, then (rank 0) the image's
+    __shared__ unsigned int s_vote[2];       // rank 0's are the cluster's
+    const int cs = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
+    const int b = blockIdx.x / cs;
+    const int tid = threadIdx.x;
+    const int base_rows = H / cs, extra = H - base_rows * cs;
+    const int n = base_rows + (rank < extra ? 1 : 0);                      // rows of this band
+    const int row0 = rank * base_rows + min(rank, extra);
+    const int n_up = rank > 0 ? base_rows + (rank - 1 < extra ? 1 : 0) : 0;
+    const int n_dn = rank + 1 < cs ? base_rows + (rank + 1 < extra ? 1 : 0) : 0;
+    const int np = grow_rows_padded(n);
+    const int Bp = grow_rows_padded((H + cs - 1) / cs);                    // the layout every CTA of the launch shares
+    uint32_t* det = sm;                                                    // [np][Ww], rows >= n zero
+    uint32_t* obj = sm + Bp * Ww;                                          // [np][Ww]
+    uint32_t* hor_p = sm + 2 * Bp * Ww;                                    // [10 + np + 17][Ww]: band row y is row y + 10
+    uint32_t* hor = hor_p + kGrowPadTop * Ww;
+    const int64_t words = (int64_t)H * Ww;
+
+    const unsigned long long k = key[b];
+    const int seed_idx = (int)(0xFFFFFFFFu - (uint32_t)(k & 0xFFFFFFFFull));
+    const int sy = seed_idx / W, sx = seed_idx - sy * W;
+    const uint32_t* det_b = det_g + (int64_t)b * words + (int64_t)row0 * Ww;
+    for (int i = tid; i < np * Ww; i += kGrowThreads) {
+        det[i] = i < n * Ww ? det_b[i] : 0u;
+        obj[i] = 0u;
+    }
+    for (int i = tid; i < (kGrowPadTop + np + kGrowPadBot) * Ww; i += kGrowThreads) hor_p[i] = 0u;
+    if (tid == 0) {
+        s_box[0] = 1 << 30; s_box[1] = -1; s_box[2] = 1 << 30; s_box[3] = -1;
+        s_vote[0] = 0u; s_vote[1] = 0u;
+        if (rank == 0 && max_loc) { max_loc[2 * b] = sy; max_loc[2 * b + 1] = sx; }
+    }
+    __syncthreads();
+    if (tid == 0 && sy >= row0 && sy < row0 + n) obj[(sy - row0) * Ww + (sx >> 5)] = 1u << (sx & 31);   // one-hot seed
+    unsigned int* vote0 = cluster.map_shared_rank(s_vote, 0);
+    int* box0 = cluster.map_shared_rank(s_box, 0);
+    const uint32_t* hor_up = rank > 0 ? cluster.map_shared_rank(hor, rank - 1) : nullptr;
+    const uint32_t* hor_dn = rank + 1 < cs ? cluster.map_shared_rank(hor, rank + 1) : nullptr;
+    const int halo_up = min(kGrowPadTop, n_up), halo_dn = min(kGrowPadTop, n_dn);
+    cluster.sync();   // every CTA's votes, box and seed are initialised before any peer touches them
+
+    const int segs = (Ww + kGrowSeg - 1) / kGrowSeg;
+    const int h_tasks = n * segs;
+    const int v_tasks = (np / kGrowRows) * Ww;
+    for (int pass = 0; pass < num_passes; ++pass) {
+        for (int t = tid; t < h_tasks; t += kGrowThreads) {   // horizontal phase: as in mask_grow_kernel
+            const int y = t / segs, sg = t - y * segs;
+            const int x0 = sg * kGrowSeg, base = y * Ww + x0;
+            uint32_t w[kGrowSeg + 2];
+#pragma unroll
+            for (int i = 0; i < kGrowSeg + 2; ++i) {
+                const int xw = x0 - 1 + i;
+                w[i] = (xw >= 0 && xw < Ww) ? obj[base - 1 + i] : 0u;
+            }
+#pragma unroll
+            for (int step = 0; step < 4; ++step) {
+                const int sft = step == 0 ? 1 : step == 1 ? 2 : step == 2 ? 4 : 3;
+                uint32_t r[kGrowSeg + 2];
+#pragma unroll
+                for (int i = 0; i < kGrowSeg + 2; ++i) {
+                    const uint32_t lo = i > 0 ? w[i - 1] : 0u, hi = i + 1 < kGrowSeg + 2 ? w[i + 1] : 0u;
+                    r[i] = w[i] | __funnelshift_l(lo, w[i], sft) | __funnelshift_r(w[i], hi, sft);
+                }
+#pragma unroll
+                for (int i = 0; i < kGrowSeg + 2; ++i) w[i] = r[i];
+            }
+#pragma unroll
+            for (int i = 0; i < kGrowSeg; ++i)
+                if (x0 + i < Ww) hor[base + i] = w[i + 1];
+        }
+        cluster.sync();   // every band's hor is complete
+        if (rank == 0 && tid == 0) s_vote[(pass + 1) & 1] = 0u;
+        // halo: the last rows of the band above go to rows -10 .. -1, the first rows of the band below to rows n .. n + 9 (rows past
+        // the image stay zero)
+        for (int i = tid; i < (halo_up + halo_dn) * Ww; i += kGrowThreads) {
+            const int r = i / Ww, xw = i - r * Ww;
+            if (r < halo_up) hor[(r - halo_up) * Ww + xw] = hor_up[(n_up - halo_up + r) * Ww + xw];
+            else hor[(n + r - halo_up) * Ww + xw] = hor_dn[(r - halo_up) * Ww + xw];
+        }
+        __syncthreads();
+        int changed = 0;
+        for (int t = tid; t < v_tasks; t += kGrowThreads) {   // vertical phase + combine: as in mask_grow_kernel
+            const int g = t / Ww, xw = t - g * Ww;
+            const int vb = g * kGrowRows * Ww + xw;
+            uint32_t v[kGrowRows + 20];
+#pragma unroll
+            for (int i = 0; i < kGrowRows + 20; ++i) v[i] = hor_p[vb + i * Ww];
+            uint32_t core = v[kGrowRows - 1];
+#pragma unroll
+            for (int i = kGrowRows; i <= 20; ++i) core |= v[i];
+            uint32_t lo[kGrowRows], hi[kGrowRows];
+            lo[0] = 0u; hi[0] = 0u;
+#pragma unroll
+            for (int kk = 1; kk < kGrowRows; ++kk) { lo[kk] = lo[kk - 1] | v[kGrowRows - 1 - kk]; hi[kk] = hi[kk - 1] | v[20 + kk]; }
+#pragma unroll
+            for (int j = 0; j < kGrowRows; ++j) {
+                const int i = vb + j * Ww;
+                const uint32_t r = (core | lo[kGrowRows - 1 - j] | hi[j]) & det[i];
+                changed |= (r != obj[i]);
+                obj[i] = r;
+            }
+        }
+        if (__syncthreads_or(changed) && tid == 0) atomicOr(vote0 + (pass & 1), 1u);
+        cluster.sync();   // every vote is in
+        unsigned int any = 0u;
+        if ((tid & 31) == 0) any = *(volatile unsigned int*)(vote0 + (pass & 1));
+        if (!__shfl_sync(0xFFFFFFFFu, any, 0)) break;   // fixed point, seen by every CTA of the cluster
+    }
+
+    // bounding box of the band (utils/general.py:294-300): X = row index, Y = column index
+    int rmin = 1 << 30, rmax = -1, cmin = 1 << 30, cmax = -1;
+    for (int i = tid; i < n * Ww; i += kGrowThreads) {
+        const uint32_t v = obj[i];
+        if (v) {
+            const int y = row0 + i / Ww, xw = i % Ww;
+            rmin = min(rmin, y); rmax = max(rmax, y);
+            cmin = min(cmin, xw * 32 + __ffs(v) - 1);
+            cmax = max(cmax, xw * 32 + 31 - __clz(v));
+        }
+    }
+    if (rmax >= 0) {
+        atomicMin(&s_box[0], rmin); atomicMax(&s_box[1], rmax);
+        atomicMin(&s_box[2], cmin); atomicMax(&s_box[3], cmax);
+    }
+    if (hand_mask) {
+        uint8_t* hm = hand_mask + (int64_t)b * H * W + (int64_t)row0 * W;
+        for (int i = tid; i < n * W; i += kGrowThreads) {
+            const int y = i / W, x = i - y * W;
+            hm[i] = (obj[y * Ww + (x >> 5)] >> (x & 31)) & 1u;
+        }
+    }
+    __syncthreads();
+    if (tid == 0 && rank != 0 && s_box[1] >= 0) {
+        atomicMin(box0 + 0, s_box[0]); atomicMax(box0 + 1, s_box[1]);
+        atomicMin(box0 + 2, s_box[2]); atomicMax(box0 + 3, s_box[3]);
+    }
+    cluster.sync();   // the last access to a peer's shared memory is above
+    if (rank == 0 && tid == 0) {
+        float c0, c1, sz;
+        if (s_box[1] < 0) {         // empty mask: the reference's written fallbacks (utils/general.py:311-312,319-320)
+            c0 = 160.0f; c1 = 160.0f; sz = 100.0f;
+        } else {
+            const float xmin = (float)s_box[0], xmax = (float)s_box[1], ymin = (float)s_box[2], ymax = (float)s_box[3];
+            c0 = __fmul_rn(0.5f, __fadd_rn(xmax, xmin));
+            c1 = __fmul_rn(0.5f, __fadd_rn(ymax, ymin));
+            sz = fmaxf(__fsub_rn(xmax, xmin), __fsub_rn(ymax, ymin));
+        }
+        center[2 * b] = c0; center[2 * b + 1] = c1;
+        if (crop_size) crop_size[b] = sz;
+        const float best = __fmul_rn(sz, 1.25f);                                   // nets/...:84
+        scale_crop[b] = fminf(fmaxf(__fdiv_rn(256.0f, best), 0.25f), 5.0f);         // nets/...:85 (size 0 -> inf -> 5)
+    }
+}
+
+static int launch_mask_grow_cluster(const unsigned long long* key, const uint32_t* det, int B, int H, int W, int Ww, int num_passes,
+                                    uint8_t* hand_mask, int32_t* max_loc, float* center, float* crop_size, float* scale_crop,
+                                    cudaStream_t s) {
+    const int cs = grow_cluster_size(H);
+    const size_t smem = grow_cluster_smem_bytes(H, Ww);
+    H3D_REQUIRE(smem <= 227 * 1024, "seg_postprocess: %dx%d needs %zu bytes of shared memory per CTA", H, W, smem);
+    static bool attr_set[64] = {};   // per device
+    int dev = 0;
+    H3D_CUDA(cudaGetDevice(&dev));
+    if (!attr_set[dev & 63]) {
+        H3D_CUDA(cudaFuncSetAttribute(mask_grow_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)grow_cluster_smem_bytes(H3D_PIPELINE_MAX_SIDE, seg_words(H3D_PIPELINE_MAX_SIDE))));
+        attr_set[dev & 63] = true;
+    }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(B * cs));
+    cfg.blockDim = dim3(kGrowThreads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)cs;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    H3D_CUDA(cudaLaunchKernelEx(&cfg, mask_grow_cluster_kernel, key, det, H, W, Ww, num_passes, hand_mask, max_loc, center, crop_size,
+                                scale_crop));
+    return H3D_OK;
+}
+
 // low != nullptr: fused form for the pipeline - `low` [B,LH,LW,2] is up-sampled to `logits` [B,H,W,2] (written) and classified in one pass
 int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scratch, uint8_t* hand_mask, int32_t* max_loc,
                            float* center, float* crop_size, float* scale_crop, cudaStream_t s, int* n_launch, const float* low, int LH,
                            int LW) {
-    H3D_REQUIRE(H <= 512 && W <= 512 && H > 0 && W > 0, "seg_postprocess: H, W must be in [1, 512]");
+    H3D_REQUIRE(H > 0 && W > 0 && H <= H3D_PIPELINE_MAX_SIDE && W <= H3D_PIPELINE_MAX_SIDE,
+                "seg_postprocess: H, W must be in [1, %d] (H3D_PIPELINE_MAX_SIDE), got %dx%d", H3D_PIPELINE_MAX_SIDE, H, W);
     const int Ww = seg_words(W);
     unsigned long long* key = (unsigned long long*)scratch;
     uint32_t* det = (uint32_t*)((char*)scratch + align_up((int64_t)B * 8, 256));
@@ -605,6 +821,12 @@ int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scrat
     else
         seg_prob_kernel<false><<<grid, 256, 0, s>>>((const float2*)(low ? low : logits), nullptr, 0, 0, 0.f, 0.f, H, W, Ww, key, det);
     H3D_CHECK_LAUNCH();
+    const int num_passes = std::max(H, W) / (21 / 2);   // utils/general.py:256
+    if (std::max(H, W) > 512) {   // one CTA's shared memory holds the masks up to 512 x 512; larger images are banded over a cluster
+        const int rc = launch_mask_grow_cluster(key, det, B, H, W, Ww, num_passes, hand_mask, max_loc, center, crop_size, scale_crop, s);
+        if (rc == H3D_OK && n_launch) *n_launch += 2;
+        return rc;
+    }
     const size_t smem = grow_smem_bytes(H, Ww);    // det, obj, hor (+ zero padding rows)
     static bool attr_set[64] = {};   // per device (one process may drive several GPUs)
     int dev = 0;
@@ -613,7 +835,6 @@ int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scrat
         H3D_CUDA(cudaFuncSetAttribute(mask_grow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)grow_smem_bytes(512, 16)));
         attr_set[dev & 63] = true;
     }
-    const int num_passes = std::max(H, W) / (21 / 2);   // utils/general.py:256
     mask_grow_kernel<<<B, kGrowThreads, smem, s>>>(key, det, H, W, Ww, num_passes, hand_mask, max_loc, center, crop_size,
                                                    scale_crop);
     H3D_CHECK_LAUNCH();

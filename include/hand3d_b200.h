@@ -131,7 +131,9 @@ H3D_API int h3d_lifting_forward(h3d_ctx* ctx, const float* scoremap32, const flo
  * Outputs (device, caller-owned, any of the large ones may be NULL to skip the copy-out):
  *   hand_scoremap [B,H,W,2], image_crop [B,256,256,3], scale_crop [B,1], center [B,2],
  *   keypoints_scoremap [B,256,256,21], keypoint_coord3d [B,21,3], keypoints_uv [B,21,2] int32 (row,col),
- *   hand_mask [B,H,W] uint8 (optional). */
+ *   hand_mask [B,H,W] uint8 (optional).
+ * 1 <= H, W <= H3D_PIPELINE_MAX_SIDE; a larger image returns H3D_EINVAL before anything is enqueued. */
+#define H3D_PIPELINE_MAX_SIDE 2048
 H3D_API int h3d_pipeline_forward(h3d_ctx* ctx, const float* image, const float* hand_side, int B, int H, int W,
                          int with_pose3d, const float* force_center, const float* force_scale,
                          float* hand_scoremap, float* image_crop, float* scale_crop, float* center,
@@ -219,7 +221,9 @@ H3D_API int h3d_avgpool8(h3d_ctx* ctx, const float* x, float* y, int B, int H, i
 /* single_obj_scoremap + calc_center_bb + crop-scale glue (utils/general.py:233-328,
  * nets/ColorHandPose3DNetwork.py:83-85).  logits [B,H,W,2] -> hand_mask [B,H,W] uint8 (optional),
  * max_loc [B,2] int32 (optional, find_max_location), center [B,2], crop_size [B,1] (raw, optional),
- * scale_crop [B,1].  H,W <= 512, W % 32 == 0 not required. */
+ * scale_crop [B,1].  1 <= H, W <= H3D_PIPELINE_MAX_SIDE (a larger map returns H3D_EINVAL before anything is enqueued),
+ * W % 32 == 0 not required.  Up to 512 a side one CTA grows the mask; larger maps are split into row bands over a thread-block
+ * cluster, with the same result. */
 H3D_API int h3d_seg_postprocess(h3d_ctx* ctx, const float* logits, int B, int H, int W, uint8_t* hand_mask,
                         int32_t* max_loc, float* center, float* crop_size, float* scale_crop, void* stream);
 /* calc_center_bb (utils/general.py:271-328) on an arbitrary mask [B,H,W] fp32 (pixels with int(mask) == 1 count):
