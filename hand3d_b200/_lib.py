@@ -50,6 +50,8 @@ SIGNATURES = {
     "h3d_conv2d_tc_dev": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
     "h3d_conv2d_tc_backward": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
     "h3d_conv2d_layer_planes": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _i, _i, _i, _p, _i, _i, _i, _i, _p, _p, _p, _p, _i, _i, _p, _i, _i, _p]),
+    "h3d_conv2d_tc_geometry": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(_i)]),
+    "h3d_conv2d_wgrad_geometry": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(_i)]),
     "h3d_leaky_relu_f32": (_i, [_p, _p, _p, _i64, _p]),
     "h3d_maxpool2x2_f32": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),
     "h3d_maxpool2x2_backward_f32": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _p]),

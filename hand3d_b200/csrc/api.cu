@@ -1499,6 +1499,21 @@ int h3d_conv2d_tc_backward(h3d_ctx* ctx, const float* x, const float* y, const f
     return H3D_OK;
 }
 
+int h3d_conv2d_tc_geometry(int B, int H, int W, int Cout, int pool, int precision, int* out) {
+    H3D_REQUIRE(out && B > 0 && H > 0 && W > 0 && Cout > 0, "h3d_conv2d_tc_geometry: bad argument");
+    H3D_REQUIRE(pool >= 0 && pool <= 2, "h3d_conv2d_tc_geometry: pool must be 0 (none), 1 (max-pool) or 2 (stride 2)");
+    H3D_REQUIRE(precision >= H3D_PREC_BF16X3 && precision <= H3D_PREC_FP16_F8C, "h3d_conv2d_tc_geometry: precision must be a tensor-core mode");
+    tc_conv_geometry(B, H, W, (int)align_up(Cout, 64), pool, passes_of(precision), out);
+    return H3D_OK;
+}
+
+int h3d_conv2d_wgrad_geometry(int B, int H, int W, int ksize, int Cin, int Cout, int* out) {
+    H3D_REQUIRE(out && B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0, "h3d_conv2d_wgrad_geometry: bad argument");
+    H3D_REQUIRE(ksize == 1 || ksize == 3 || ksize == 5 || ksize == 7, "h3d_conv2d_wgrad_geometry: ksize must be 1, 3, 5 or 7");
+    conv_wgrad_geometry(B, H, W, ksize, (int)align_up(Cin, 64), (int)align_up(Cout, 64), out);
+    return H3D_OK;
+}
+
 int h3d_conv2d_tc(h3d_ctx* ctx, const float* x, const float* host_w_hwio, const float* host_bias, float* y, int B, int H, int W,
                   int Cin, int Cout, int ksize, int leaky, int precision, void* stream) {
     return h3d_conv2d_tc_strided(ctx, x, host_w_hwio, host_bias, y, B, H, W, Cin, Cout, ksize, 1, leaky, precision, stream);

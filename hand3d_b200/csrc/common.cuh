@@ -268,6 +268,8 @@ void tc_conv_plan_destroy(TcConvPlan* p);
 int tc_conv_launch(const TcConvPlan* p, cudaStream_t s);
 int64_t tc_conv_flops(const TcConvPlan* p);
 int tc_num_sms();
+// The pixel tile and N tile tc_conv_plan_create gives a layer: out = {TW, TH, TB, BN}.  Host only, launches nothing.
+void tc_conv_geometry(int B, int H, int W, int Cout_pad, int pool, int passes, int out[4]);
 
 // ---------------------------------------------------------------- kernels (conv_wgrad.cu): backward of the tensor-core convolution
 // HWIO fp32 device weights -> 16-bit hi (/ lo) planes: forward [Cout_pad][k][k][Cin_pad] (as pack_conv_weights) or, with dgrad, the
@@ -290,6 +292,8 @@ struct WgradDesc {
     int* err_flag;
 };
 int64_t conv_wgrad_partial_floats(int B, int H, int W, int k, int Cin_pad, int Cout_pad);
+// The geometry launch_conv_wgrad gives a layer: out = {TW, TH, TB, BN, num_tiles, splits}.  Host only, launches nothing.
+void conv_wgrad_geometry(int B, int H, int W, int k, int Cin_pad, int Cout_pad, int out[6]);
 int launch_conv_wgrad(const WgradDesc& d, cudaStream_t s);
 
 // ---------------------------------------------------------------- kernels (train.cu): resize gradient, training losses, Adam

@@ -802,6 +802,19 @@ int tc_set_tuning(const char* key, int value) {
 }
 
 namespace {
+// N = 128 tiles where Cout allows (each A tile feeds twice the output channels).  Small maps (lifting pyramids from 16x16
+// down, 1x1 layers over batch rows) have too few pixel tiles to fill the machine with wide tiles, so N = 64 tiles spread the
+// work over twice the SMs.  The rule depends on the layer geometry only, never on the batch size: the arithmetic of an image
+// must not depend on how a batch is cut (tests/test_gpu_properties.py: bit-identical results under sharding).
+int choose_bn(int H, int W, int Cout_pad, int passes) {
+    const TcTuning& tune = tc_tuning();
+    int BN = Cout_pad % 128 == 0 ? 128 : 64;
+    if ((int64_t)H * W <= 256) BN = 64;
+    if ((tune.bn == 64 || tune.bn == 128) && Cout_pad % tune.bn == 0) BN = tune.bn;
+    if (passes == 4) BN = 64;   // the separate e4m3 accumulator: three fragments of BN / 2 registers per thread
+    return BN;
+}
+
 template <int BN, int PASSES, bool FP16>
 int launch_inst(const TcConvPlan* pl, cudaStream_t s) {
     constexpr int smem = smem_bytes(BN, PASSES);
@@ -840,14 +853,7 @@ TcConvPlan* tc_conv_plan_create(const TcConvDesc& d, int* rc) {
     TcConvPlan* pl = new TcConvPlan();
     pl->d = d;
     const TcTuning& tune = tc_tuning();
-    // N = 128 tiles where Cout allows (each A tile feeds twice the output channels).  Small maps (lifting pyramids from 16x16
-    // down, 1x1 layers over batch rows) have too few pixel tiles to fill the machine with wide tiles, so N = 64 tiles spread the
-    // work over twice the SMs.  The rule depends on the layer geometry only, never on the batch size: the arithmetic of an image
-    // must not depend on how a batch is cut (tests/test_gpu_properties.py: bit-identical results under sharding).
-    int BN = d.Cout_pad % 128 == 0 ? 128 : 64;
-    if ((int64_t)d.H * d.W <= 256) BN = 64;
-    if ((tune.bn == 64 || tune.bn == 128) && d.Cout_pad % tune.bn == 0) BN = tune.bn;
-    if (d.passes == 4) BN = 64;   // the separate e4m3 accumulator: three fragments of BN / 2 registers per thread
+    const int BN = choose_bn(d.H, d.W, d.Cout_pad, d.passes);
     int TW, TH, TB;
     choose_tile(d.B, d.H, d.W, &TW, &TH, &TB, d.pool == 1);
     pl->BN = BN;
@@ -890,6 +896,11 @@ TcConvPlan* tc_conv_plan_create(const TcConvDesc& d, int* rc) {
 }
 
 void tc_conv_plan_destroy(TcConvPlan* p) { delete p; }
+
+void tc_conv_geometry(int B, int H, int W, int Cout_pad, int pool, int passes, int out[4]) {
+    choose_tile(B, H, W, &out[0], &out[1], &out[2], pool == 1);
+    out[3] = choose_bn(H, W, Cout_pad, passes);
+}
 
 int64_t tc_conv_flops(const TcConvPlan* p) {
     return 2ll * p->d.B * p->d.H * p->d.W * p->d.k * p->d.k * (int64_t)p->d.Cin_pad * p->d.Cout_pad;

@@ -350,6 +350,11 @@ int64_t conv_wgrad_partial_floats(int B, int H, int W, int k, int Cin_pad, int C
     return (int64_t)g.splits * g.num_tiles * 64 * g.BN;
 }
 
+void conv_wgrad_geometry(int B, int H, int W, int k, int Cin_pad, int Cout_pad, int out[6]) {
+    const WgradGeom g = wgrad_geometry(B, H, W, k, Cin_pad, Cout_pad);
+    out[0] = g.TW; out[1] = g.TH; out[2] = g.TB; out[3] = g.BN; out[4] = g.num_tiles; out[5] = g.splits;
+}
+
 int launch_conv_wgrad(const WgradDesc& d, cudaStream_t s) {
     H3D_REQUIRE(d.passes == 1 || d.passes == 3, "conv_wgrad: 1 or 3 passes");
     H3D_REQUIRE(d.Cin_pad % 64 == 0 && d.Cout_pad % 64 == 0 && d.dy.hi && d.x.hi && (d.passes == 1 || (d.dy.lo && d.x.lo)),

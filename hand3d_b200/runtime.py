@@ -915,6 +915,20 @@ class PackedConv:
             pass
 
 
+def conv2d_tc_geometry(B, H, W, Cout, pool=0, precision="bf16x3"):
+    """(TW, TH, TB, BN) the tensor-core convolution runs this layer on (h3d_conv2d_tc_geometry; pool 2 = stride 2).  Needs no device."""
+    out = (C.c_int * 4)()
+    _lib.check(_lib.load().h3d_conv2d_tc_geometry(B, H, W, Cout, int(pool), PRECISIONS[precision], out), "h3d_conv2d_tc_geometry")
+    return tuple(out)
+
+
+def conv2d_wgrad_geometry(B, H, W, ksize, Cin, Cout):
+    """(TW, TH, TB, BN, num_tiles, splits) of the weight-gradient kernel (h3d_conv2d_wgrad_geometry).  Needs no device."""
+    out = (C.c_int * 6)()
+    _lib.check(_lib.load().h3d_conv2d_wgrad_geometry(B, H, W, ksize, Cin, Cout, out), "h3d_conv2d_wgrad_geometry")
+    return tuple(out)
+
+
 _default = {}
 
 

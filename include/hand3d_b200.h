@@ -203,6 +203,17 @@ H3D_API int h3d_conv2d_layer_planes(h3d_ctx* ctx, const float* x, int B, int H, 
 H3D_API int h3d_conv2d_tc_backward(h3d_ctx* ctx, const float* x, const float* y, const float* dy, const float* w_hwio, float* dx,
                                    float* dw_hwio, float* db, int B, int H, int W, int Cin, int Cout, int ksize, int stride, int leaky,
                                    int precision, void* stream);
+/* Which tile the tensor-core convolution runs a layer on, from the library's own choosers (host only: no context, no device, nothing
+ * is launched; without a device the SM count is taken as 132).  For tests and tools that must know which kernel geometry a shape
+ * exercises.  out[4] = TW, TH, TB, BN: a pixel tile of TW x TH pixels of TB images (TW * TH * TB = 128 rows) and the N tile (64 or 128
+ * output channels), for x [B,H,W,.] -> Cout channels with pool as in h3d_conv2d_layer_planes (stride 2 of the operator entries is
+ * pool = 2), under the current "tc_bn" tuning.  The data gradient of h3d_conv2d_tc_backward is this geometry with Cout = the layer's
+ * Cin and pool = 0. */
+H3D_API int h3d_conv2d_tc_geometry(int B, int H, int W, int Cout, int pool, int precision, int* out);
+/* The weight-gradient kernel's geometry for h3d_conv2d_tc_backward on x [B,H,W,Cin] (H, W of the layer's input at either stride):
+ * out[6] = TW, TH, TB (a 64-pixel box), BN (64 or 128 input channels per tile), num_tiles (ksize^2 x Cout tiles x Cin tiles) and
+ * splits (CTAs that share one tile's pixel blocks). */
+H3D_API int h3d_conv2d_wgrad_geometry(int B, int H, int W, int ksize, int Cin, int Cout, int* out);
 /* NetworkOps.leaky_relu (utils/general.py:31-33): y = max(x, 0.01 x), n elements, 16-byte aligned pointers. */
 H3D_API int h3d_leaky_relu_f32(h3d_ctx* ctx, const float* x, float* y, int64_t n, void* stream);
 /* NetworkOps.max_pool (utils/general.py:62-65): 2x2 / 2 VALID. */
