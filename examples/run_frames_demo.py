@@ -46,6 +46,9 @@ def main():
     ap.add_argument("--width", type=int, default=1920)
     ap.add_argument("--weights", default=None, help="directory of the reference's pickles (default: synthetic weights)")
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--track", action="store_true", help="follow the hand from frame to frame; HandSegNet only to (re-)acquire it")
+    ap.add_argument("--redetect-every", type=int, default=None, help="with --track: also detect on every N-th batch")
+    ap.add_argument("--min-score", type=float, default=None, help="with --track: a slot whose key-point score is lower is lost")
     args = ap.parse_args()
 
     from hand3d_b200 import runtime, weights as Wt
@@ -70,14 +73,18 @@ def main():
         hw = (args.height, args.width)
         batches = synthetic_batches(args.batches, args.batch, hw[0], hw[1], args.seed)
 
-    runner = FrameRunner(ctx, args.batch, hw)
+    runner = FrameRunner(ctx, args.batch, hw, track=args.track, redetect_every=args.redetect_every, min_score=args.min_score)
     t0 = time.perf_counter()
     n = 0
     for i, r in enumerate(runner.stream(batches)):
         n += args.batch
         kp = r["keypoints_frame"][0]
-        print("batch %d: frame 0 key-points (row, col) in %dx%d pixels: wrist %s, index tip %s" % (i, hw[0], hw[1], np.round(kp[0], 1),
-                                                                                               np.round(kp[8], 1)))
+        track = ""
+        if args.track:
+            track = " [%s, score %.4g%s]" % ("detect" if r["detected"] else "track", r["track_score"][0],
+                                             ", lost" if r["track_lost"][0] else "")
+        print("batch %d: frame 0 key-points (row, col) in %dx%d pixels: wrist %s, index tip %s%s" % (i, hw[0], hw[1], np.round(kp[0], 1),
+                                                                                                 np.round(kp[8], 1), track))
     dt = time.perf_counter() - t0
     print("%d frames in %.3f s: %.1f frames/s" % (n, dt, n / dt if dt > 0 else 0.0))
 

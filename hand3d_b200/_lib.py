@@ -41,6 +41,9 @@ SIGNATURES = {
     "h3d_lifting_forward": (_i, [_p, _p, _p, _i, _i, _p, _p, _p, _p]),
     "h3d_pipeline_forward": (_i, [_p, _p, _p, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "h3d_pose2d_forward": (_i, [_p, _p, _i, _i, _i, _p, _p, _p]),
+    "h3d_track_state_bytes": (_i64, [_i]),
+    "h3d_track_step": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _f, _f, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "h3d_track_update": (_i, [_p, _p, _p, _p, _p, _i, _f, _f, _p, _p]),
     "h3d_conv2d_f32": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
     "h3d_conv2d_tc": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
     "h3d_conv2d_tc_strided": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
@@ -109,6 +112,8 @@ READER_QUEUE_CAPACITY, READER_STATE_COUNT, READER_STATE_NEXT, READER_STATE_SLOTS
 FRAME_MAX_SIDE, FRAME_MAX_OUT = 4096, 512
 # the largest image side of h3d_pipeline_forward and h3d_seg_postprocess (H3D_PIPELINE_MAX_SIDE)
 PIPELINE_MAX_SIDE = 2048
+# tracking state (H3D_TRACK_*): the word offset of each array, in units of B words
+TRACK_CENTER, TRACK_SCALE, TRACK_SCORE, TRACK_LOST, TRACK_STATE_WORDS = 0, 2, 3, 4, 5
 # device evaluation store (H3D_EVAL_*): dtypes, the header layout, the limits and the layout of a stats row
 EVAL_FLOAT32, EVAL_FLOAT64 = 0, 1
 EVAL_KEPT, EVAL_DROPPED, EVAL_TICKET, EVAL_COUNT, EVAL_HEADER_WORDS = 0, 1, 2, 8, 72

@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libhand3d_b200.so")
 STAMP = os.path.join(HERE, ".libhand3d_b200.stamp")
 SOURCES = ["api.cu", "elementwise.cu", "reader.cu", "reader_aug.cu", "conv_direct.cu", "conv_wgmma.cu", "conv_wgrad.cu", "train.cu", "train_lift.cu",
-           "frames.cu", "eval.cu"]
+           "frames.cu", "eval.cu", "track.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--cudart=static", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",

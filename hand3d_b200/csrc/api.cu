@@ -1227,35 +1227,13 @@ int h3d_lifting_forward(h3d_ctx* ctx, const float* scoremap32, const float* hand
     return run_plan(ctx, ctx->lift.get(), e, (cudaStream_t)stream);
 }
 
-int h3d_pipeline_forward(h3d_ctx* ctx, const float* image, const float* hand_side, int B, int H, int W, int with_pose3d,
-                         const float* force_center, const float* force_scale, float* hand_scoremap, float* image_crop,
-                         float* scale_crop, float* center, float* keypoints_scoremap, float* keypoint_coord3d,
-                         int32_t* keypoints_uv, uint8_t* hand_mask, void* stream) {
-    DeviceGuard guard_(ctx ? ctx->device : 0);
-    H3D_REQUIRE(ctx && image && B > 0, "h3d_pipeline_forward: bad argument");
-    H3D_REQUIRE(!with_pose3d || (hand_side && keypoint_coord3d), "h3d_pipeline_forward: hand_side / keypoint_coord3d required with pose3d");
-    H3D_REQUIRE(H >= 1 && W >= 1 && H <= H3D_PIPELINE_MAX_SIDE && W <= H3D_PIPELINE_MAX_SIDE,
-                "h3d_pipeline_forward: images must be 1..%d pixels a side (H3D_PIPELINE_MAX_SIDE), got %dx%d", H3D_PIPELINE_MAX_SIDE, H, W);
+// The pipeline after the crop parameters (cen, scl) are known: crop, PoseNet2D, up-sampling + key-points, lifting.  Shared by
+// h3d_pipeline_forward and the track steps of h3d_track_step, which differ only in where (cen, scl) come from.
+static int pipeline_tail(h3d_ctx* ctx, const float* image, const float* hand_side, int B, int H, int W, int with_pose3d, const float* cen,
+                         const float* scl, float* crop, float* kps, float* keypoint_coord3d, int32_t* keypoints_uv, void* stream) {
     cudaStream_t s = (cudaStream_t)stream;
-    int rc;
-    if ((rc = ensure_layout_covers(ctx, B, H, W, 256, 256))) return rc;
     h3d_ctx::Layout& L = ctx->lay;
-    float* seg = hand_scoremap ? hand_scoremap : L.hand_scoremap;
-    float* crop = image_crop ? image_crop : L.image_crop;
-    float* kps = keypoints_scoremap ? keypoints_scoremap : L.kp_scoremap;
-    float* cen = center ? center : L.center;
-    float* scl = scale_crop ? scale_crop : L.scale;
-    // HandSegNet (nets/...:78-79)
-    // (its x8 up-sampling, nets/...:166, is fused into the next kernel: the 0.82 MB / image hand_scoremap is written once, not re-read)
-    const bool fuse_up = !tc_tuning().no_seg_fusion;
-    if ((rc = run_handsegnet(ctx, image, B, H, W, fuse_up ? nullptr : seg, stream))) return rc;
-    // single_obj_scoremap + calc_center_bb + scale (nets/...:82-85)
-    int nl = 0;
-    if ((rc = launch_seg_postprocess(seg, B, H, W, L.seg_scratch, hand_mask, nullptr, cen, L.crop_size, scl, s, &nl,
-                                     fuse_up ? L.seg_low : nullptr, H / 8, W / 8))) return rc;
-    ctx->launches += nl;
-    if (force_center) H3D_CUDA(cudaMemcpyAsync(cen, force_center, (size_t)B * 8, cudaMemcpyDeviceToDevice, s));
-    if (force_scale) H3D_CUDA(cudaMemcpyAsync(scl, force_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
+    int rc = H3D_OK, nl = 0;
     // crop_image_from_xy (nets/...:86)
     if ((rc = launch_crop_image(image, cen, scl, crop, B, H, W, 3, 256, s))) return rc;
     ctx->launches += 1;
@@ -1289,6 +1267,89 @@ int h3d_pipeline_forward(h3d_ctx* ctx, const float* image, const float* hand_sid
         rc = h3d_lifting_forward(ctx, L.s[2], hand_side, B, H3D_VARIANT_PROPOSED, keypoint_coord3d, nullptr, nullptr, stream);
     if (overlap) H3D_CUDA(cudaStreamWaitEvent(s, ctx->ev_join2, 0));   // join even when the lifting stage failed
     if (rc) return rc;
+    return H3D_OK;
+}
+
+#define H3D_PIPELINE_CHECKS(fn)                                                                                                       \
+    H3D_REQUIRE(ctx && image && B > 0, fn ": bad argument");                                                                          \
+    H3D_REQUIRE(!with_pose3d || (hand_side && keypoint_coord3d), fn ": hand_side / keypoint_coord3d required with pose3d");           \
+    H3D_REQUIRE(H >= 1 && W >= 1 && H <= H3D_PIPELINE_MAX_SIDE && W <= H3D_PIPELINE_MAX_SIDE,                                         \
+                fn ": images must be 1..%d pixels a side (H3D_PIPELINE_MAX_SIDE), got %dx%d", H3D_PIPELINE_MAX_SIDE, H, W)
+
+int h3d_pipeline_forward(h3d_ctx* ctx, const float* image, const float* hand_side, int B, int H, int W, int with_pose3d,
+                         const float* force_center, const float* force_scale, float* hand_scoremap, float* image_crop,
+                         float* scale_crop, float* center, float* keypoints_scoremap, float* keypoint_coord3d,
+                         int32_t* keypoints_uv, uint8_t* hand_mask, void* stream) {
+    DeviceGuard guard_(ctx ? ctx->device : 0);
+    H3D_PIPELINE_CHECKS("h3d_pipeline_forward");
+    cudaStream_t s = (cudaStream_t)stream;
+    int rc;
+    if ((rc = ensure_layout_covers(ctx, B, H, W, 256, 256))) return rc;
+    h3d_ctx::Layout& L = ctx->lay;
+    float* seg = hand_scoremap ? hand_scoremap : L.hand_scoremap;
+    float* cen = center ? center : L.center;
+    float* scl = scale_crop ? scale_crop : L.scale;
+    // HandSegNet (nets/...:78-79)
+    // (its x8 up-sampling, nets/...:166, is fused into the next kernel: the 0.82 MB / image hand_scoremap is written once, not re-read)
+    const bool fuse_up = !tc_tuning().no_seg_fusion;
+    if ((rc = run_handsegnet(ctx, image, B, H, W, fuse_up ? nullptr : seg, stream))) return rc;
+    // single_obj_scoremap + calc_center_bb + scale (nets/...:82-85)
+    int nl = 0;
+    if ((rc = launch_seg_postprocess(seg, B, H, W, L.seg_scratch, hand_mask, nullptr, cen, L.crop_size, scl, s, &nl,
+                                     fuse_up ? L.seg_low : nullptr, H / 8, W / 8))) return rc;
+    ctx->launches += nl;
+    if (force_center) H3D_CUDA(cudaMemcpyAsync(cen, force_center, (size_t)B * 8, cudaMemcpyDeviceToDevice, s));
+    if (force_scale) H3D_CUDA(cudaMemcpyAsync(scl, force_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
+    return pipeline_tail(ctx, image, hand_side, B, H, W, with_pose3d, cen, scl, image_crop ? image_crop : L.image_crop,
+                         keypoints_scoremap ? keypoints_scoremap : L.kp_scoremap, keypoint_coord3d, keypoints_uv, stream);
+}
+
+int64_t h3d_track_state_bytes(int B) {
+    if (B < 1) return H3D_EINVAL;
+    return (int64_t)H3D_TRACK_STATE_WORDS * 4 * B;
+}
+
+#define H3D_TRACK_CHECKS(fn)                                                                                                         \
+    H3D_REQUIRE(state != nullptr && ((uintptr_t)state & 7) == 0, fn ": state must be a non-NULL, 8-byte aligned device pointer");    \
+    H3D_REQUIRE(std::isfinite(margin) && margin >= 0.25f, fn ": margin must be finite and >= 0.25, got %g", (double)margin);         \
+    H3D_REQUIRE(!std::isinf(min_score), fn ": min_score must be finite, or NaN for no score test")
+
+int h3d_track_update(h3d_ctx* ctx, const float* scoremap32, const int32_t* keypoints_uv, const float* center, const float* scale_crop,
+                     int B, float margin, float min_score, void* state, void* stream) {
+    DeviceGuard guard_(ctx ? ctx->device : 0);
+    H3D_REQUIRE(ctx && scoremap32 && keypoints_uv && center && scale_crop && B > 0, "h3d_track_update: bad argument");
+    H3D_TRACK_CHECKS("h3d_track_update");
+    int rc = launch_track_update(scoremap32, keypoints_uv, center, scale_crop, B, margin, min_score, state, (cudaStream_t)stream);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+
+int h3d_track_step(h3d_ctx* ctx, const float* image, const float* hand_side, int B, int H, int W, int with_pose3d, int detect,
+                   float margin, float min_score, void* state, float* image_crop, float* scale_crop, float* center,
+                   float* keypoints_scoremap, float* keypoint_coord3d, int32_t* keypoints_uv, void* stream) {
+    DeviceGuard guard_(ctx ? ctx->device : 0);
+    H3D_PIPELINE_CHECKS("h3d_track_step");
+    H3D_TRACK_CHECKS("h3d_track_step");
+    cudaStream_t s = (cudaStream_t)stream;
+    int rc;
+    if ((rc = ensure_layout_covers(ctx, B, H, W, 256, 256))) return rc;
+    h3d_ctx::Layout& L = ctx->lay;
+    float* cen = center ? center : L.center;
+    float* scl = scale_crop ? scale_crop : L.scale;
+    int32_t* uv = keypoints_uv ? keypoints_uv : L.kp_uv;   // the update needs the key-points even when the caller does not
+    if (detect) {
+        rc = h3d_pipeline_forward(ctx, image, hand_side, B, H, W, with_pose3d, nullptr, nullptr, nullptr, image_crop, scl, cen,
+                                  keypoints_scoremap, keypoint_coord3d, uv, nullptr, stream);
+    } else {
+        const float* st = (const float*)state;
+        H3D_CUDA(cudaMemcpyAsync(cen, st + (int64_t)H3D_TRACK_CENTER * B, (size_t)B * 8, cudaMemcpyDeviceToDevice, s));
+        H3D_CUDA(cudaMemcpyAsync(scl, st + (int64_t)H3D_TRACK_SCALE * B, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
+        rc = pipeline_tail(ctx, image, hand_side, B, H, W, with_pose3d, cen, scl, image_crop ? image_crop : L.image_crop,
+                           keypoints_scoremap ? keypoints_scoremap : L.kp_scoremap, keypoint_coord3d, uv, stream);
+    }
+    if (rc) return rc;
+    if ((rc = launch_track_update(L.s[2], uv, cen, scl, B, margin, min_score, state, s))) return rc;
+    ctx->launches += 1;
     return H3D_OK;
 }
 

@@ -176,6 +176,12 @@ int launch_eval_feed(void* store, int K, int N, int dtype, const void* gt, const
                      cudaStream_t s);
 int launch_eval_stats(const void* store, int K, int N, int dtype, const double* thr, int nthr, int64_t* out, cudaStream_t s);
 
+// ---------------------------------------------------------------- kernels (track.cu): the next crop of a tracked stream
+// map32 [B,32,32,21] (the last PoseNet2D stage), uv [B,21,2] int32, center [B,2], scale [B] -> state (include/hand3d_b200.h,
+// H3D_TRACK_*); min_score NaN = no score test.  One kernel.
+int launch_track_update(const float* map32, const int32_t* uv, const float* center, const float* scale, int B, float margin,
+                        float min_score, void* state, cudaStream_t s);
+
 // ---------------------------------------------------------------- kernels (conv_direct.cu)
 struct DirectConvArgs {
     const float* x;       // [B,H,W,Cin_total] fp32, channels [cin_off, cin_off+Cin) are read

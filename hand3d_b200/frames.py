@@ -113,13 +113,29 @@ class FrameRunner:
     hand_side [B,2] (run.py's constant [[1, 0]] when None) goes with each batch.
 
     stream(batches) is the overlapped loop: it submits batch i + 1 before it reads back batch i, and yields the host results of
-    every batch in order (numpy dicts owned by the caller)."""
+    every batch in order (numpy dicts owned by the caller).
+
+    track=True follows the hand from batch to batch instead of detecting it in every frame (Context.track_step, DESIGN.md section
+    4.14): each batch slot is one camera stream, and a track step crops frame t where the key-points of frame t - 1 put the hand,
+    without HandSegNet.  It captures a detect graph and a track graph per input buffer around one TrackState, which the graphs
+    update in stream order, so no step waits on the host for its crop.  Step t detects when t == 0, when redetect_every is set and
+    t % redetect_every == 0, or when any slot was lost at step t - 2 (min_score: the lowest trusted score; None = no score test).
+    The choice is made on the host from step t - 2's lost flags: stream() has them already; submit() waits for step t - 2 to finish.
+    So a slot lost at step t is re-acquired by a detect step at t + 2 at the latest.  The results gain detected (bool, the step's
+    kind), track_score [B] float32 and track_lost [B] bool."""
 
     RESULT_KEYS = ("keypoints_frame", "keypoints_uv", "keypoint_coord3d", "center", "scale_crop")
+    TRACK_KEYS = ("track_score", "track_lost")
 
-    def __init__(self, ctx, batch, frame_hw, size=NETWORK_SIZE, outputs="keypoints"):
+    def __init__(self, ctx, batch, frame_hw, size=NETWORK_SIZE, outputs="keypoints", track=False, redetect_every=None, min_score=None,
+                 track_margin=1.5):
         self.ctx, self.B = ctx, int(batch)
         self.frame_hw, self.size = (int(frame_hw[0]), int(frame_hw[1])), (int(size[0]), int(size[1]))
+        self.track = bool(track)
+        if redetect_every is not None and int(redetect_every) < 1:
+            raise ValueError("FrameRunner: redetect_every must be None or >= 1, got %r" % (redetect_every,))
+        self.redetect_every = None if redetect_every is None else int(redetect_every)
+        self.min_score, self.track_margin = min_score, float(track_margin)
         dev = ctx.device
         Hf, Wf = self.frame_hw
         h, w = self.size
@@ -139,27 +155,58 @@ class FrameRunner:
         self._i = 0
         ctx.ensure_workspace(self.B, h, w)
 
-        def body(k):
+        if self.track:
+            self._state = runtime.TrackState(self.B, dev)
+            self._lost_host = [torch.zeros(self.B, dtype=torch.bool).pin_memory() for _ in range(2)]   # step t's lost flags
+            self._lost_ready = [torch.cuda.Event() for _ in range(2)]
+            self._detected = [True, True]
+
+        def body(k, detect=True):
             ctx.resize_frames(self._frames[k], h, w, normalize=True, out=self._image[k])
-            r = ctx.pipeline(self._image[k], self._hs[k], True, outputs=outputs)
+            if self.track:
+                r = ctx.track_step(self._image[k], self._hs[k], self._state, detect, margin=self.track_margin, min_score=self.min_score,
+                                   outputs=outputs)
+                r["track_score"] = self._state.score.clone()
+                r["track_lost"] = self._state.lost != 0
+            else:
+                r = ctx.pipeline(self._image[k], self._hs[k], True, outputs=outputs)
             r["keypoints_frame"] = frame_coords(trafo_coords(r["keypoints_uv"], r["center"], r["scale_crop"], 256), self.frame_hw, self.size)
             return r
 
+        kinds = (True, False) if self.track else (True,)
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):       # warm-up outside capture: builds the resize and stage plans, packs weights
             for k in range(2):
-                body(k)
+                for detect in kinds:
+                    body(k, detect)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize(dev)
-        self._graphs, self._results = [], []
+        self._graphs, self._results = [], []   # [buffer][kind]: kind 0 = detect, 1 = track
         for k in range(2):
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                r = body(k)
-            ctx._graphs_captured = getattr(ctx, "_graphs_captured", 0) + 1   # the graphs bake in workspace pointers
-            self._graphs.append(g)
-            self._results.append(r)
+            gs, rs = [], []
+            for detect in kinds:
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g):
+                    r = body(k, detect)
+                ctx._graphs_captured = getattr(ctx, "_graphs_captured", 0) + 1   # the graphs bake in workspace pointers
+                gs.append(g)
+                rs.append(r)
+            self._graphs.append(gs)
+            self._results.append(rs)
+        if self.track:
+            self._state.reset()             # forget the warm-up's steps
+            torch.cuda.synchronize(dev)
+
+    def _detect_now(self, t):
+        """The host's detect / track choice for step t (deterministic: t, redetect_every and step t - 2's lost flags)."""
+        if t == 0 or (self.redetect_every is not None and t % self.redetect_every == 0):
+            return True
+        if t < 2:
+            return False
+        k = t & 1                                   # step t - 2 used the same buffer
+        self._lost_ready[k].synchronize()
+        return bool(self._lost_host[k].any())
 
     def _check_frames(self, frames):
         shape = (self.B,) + self.frame_hw + (3,)
@@ -167,7 +214,10 @@ class FrameRunner:
             raise ValueError("FrameRunner: frames must be %s, got %s" % (shape, tuple(frames.shape)))
 
     def submit(self, frames, hand_side=None):
-        k = self._i & 1
+        """Enqueues one batch; returns its device result tensors (see the class notes), and in track mode also detected (bool)."""
+        t = self._i
+        k = t & 1
+        detect = self._detect_now(t) if self.track else True
         self._i += 1
         cur = torch.cuda.current_stream(self.ctx.device)
         cur.wait_event(self._d2h_done[k])           # stream() may still be reading this buffer's previous results
@@ -196,9 +246,17 @@ class FrameRunner:
                 self._hs[k].copy_(self._stage_hs[k], non_blocking=True)
                 self._uploaded[k].record(self._copy)
             cur.wait_event(self._uploaded[k])
-        self._graphs[k].replay()
+        kind = 0 if detect else 1
+        self._graphs[k][kind].replay()
         self._consumed[k].record(cur)
-        return {n: self._results[k][n] for n in self.RESULT_KEYS}
+        res = {n: self._results[k][kind][n] for n in self.RESULT_KEYS}
+        if self.track:
+            res.update({n: self._results[k][kind][n] for n in self.TRACK_KEYS})
+            self._lost_host[k].copy_(res["track_lost"], non_blocking=True)   # read by step t + 2's choice
+            self._lost_ready[k].record(cur)
+            self._detected[k] = detect
+            res["detected"] = detect
+        return res
 
     def stream(self, batches):
         """batches: iterable of frames, or of (frames, hand_side) -> yields one numpy dict per batch, in order."""
@@ -206,6 +264,7 @@ class FrameRunner:
         for item in batches:
             frames, hs = item if isinstance(item, tuple) else (item, None)
             res = self.submit(frames, hs)
+            res.pop("detected", None)       # a host value: _collect adds it
             k = (self._i - 1) & 1
             if self._host[k] is None:
                 self._host[k] = {n: torch.empty(t.shape, dtype=t.dtype).pin_memory() for n, t in res.items()}
@@ -222,4 +281,7 @@ class FrameRunner:
 
     def _collect(self, k):
         self._d2h_done[k].synchronize()             # the read-back the caller asked for
-        return {n: t.numpy().copy() for n, t in self._host[k].items()}
+        out = {n: t.numpy().copy() for n, t in self._host[k].items()}
+        if self.track:
+            out["detected"] = self._detected[k]
+        return out

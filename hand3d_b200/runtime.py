@@ -251,6 +251,55 @@ class Context:
         """Declares every graph returned by capture_pipeline() dead (the caller must drop them); the workspace may grow again."""
         self._graphs_captured = 0
 
+    def track_step(self, image, hand_side, state, detect, margin=1.5, min_score=None, outputs="all", with_pose3d=True):
+        """One step of a tracked stream per batch slot (h3d_track_step, DESIGN.md section 4.14).  detect=True runs pipeline() (no
+        forced crop); detect=False crops at state.center / state.scale and skips HandSegNet and the mask post-processing.  Either way
+        the step then updates `state` (a TrackState of the same batch) from its key-points: the next crop, the score and the lost
+        flag.  min_score None turns the score test off.  Returns image_crop, scale_crop, center (the crop this step used),
+        keypoints_scoremap, keypoint_coord3d and keypoints_uv as pipeline() does; outputs="keypoints" leaves the large ones in the
+        workspace.  Enqueue-only: a call on fixed tensors can be captured into a CUDA graph."""
+        image = _chk_f32(image, "image", 4)
+        B, H, W, _ = image.shape
+        dev = image.device
+        if with_pose3d:
+            hand_side = _chk_f32(hand_side, "hand_side", 2)
+        if not isinstance(state, TrackState) or state.B != B or state.buffer.device != dev:
+            raise ValueError("state must be a TrackState of batch %d on %s" % (B, dev))
+        self.ensure_workspace(B, H, W)
+        f32 = dict(dtype=torch.float32, device=dev)
+        big = outputs == "all"
+        r = {
+            "image_crop": torch.empty((B, 256, 256, 3), **f32) if big else None,
+            "scale_crop": torch.empty((B, 1), **f32),
+            "center": torch.empty((B, 2), **f32),
+            "keypoints_scoremap": torch.empty((B, 256, 256, 21), **f32) if big else None,
+            "keypoint_coord3d": torch.empty((B, 21, 3), **f32) if with_pose3d else None,
+            "keypoints_uv": torch.empty((B, 21, 2), dtype=torch.int32, device=dev),
+        }
+        _lib.check(self.lib.h3d_track_step(
+            self.h, _ptr(image), _ptr(hand_side if with_pose3d else None), B, H, W, int(bool(with_pose3d)), int(bool(detect)),
+            float(margin), float("nan") if min_score is None else float(min_score), _ptr(state.buffer),
+            _ptr(r["image_crop"]), _ptr(r["scale_crop"]), _ptr(r["center"]), _ptr(r["keypoints_scoremap"]),
+            _ptr(r["keypoint_coord3d"]), _ptr(r["keypoints_uv"]), _stream()), "h3d_track_step")
+        return r
+
+    def track_update(self, scoremap32, keypoints_uv, center, scale_crop, state, margin=1.5, min_score=None):
+        """track_step's update alone (h3d_track_update): scoremap32 [B,32,32,21], keypoints_uv [B,21,2] int32, center [B,2] and
+        scale_crop [B] or [B,1] of the crop the key-points were found in -> `state` (a TrackState of batch B)."""
+        scoremap32 = _chk_f32(scoremap32, "scoremap32", 4)
+        B = scoremap32.shape[0]
+        if tuple(scoremap32.shape[1:]) != (32, 32, 21):
+            raise ValueError("track_update expects a [B,32,32,21] score map, got %s" % (tuple(scoremap32.shape),))
+        center = _chk_f32(center, "center").reshape(B, 2)
+        scale_crop = _chk_f32(scale_crop, "scale_crop").reshape(B)
+        if keypoints_uv.dtype != torch.int32 or tuple(keypoints_uv.shape) != (B, 21, 2) or not keypoints_uv.is_cuda:
+            raise ValueError("keypoints_uv must be a CUDA int32 [%d,21,2] tensor" % B)
+        if not isinstance(state, TrackState) or state.B != B:
+            raise ValueError("state must be a TrackState of batch %d" % B)
+        _lib.check(self.lib.h3d_track_update(self.h, _ptr(scoremap32), _ptr(keypoints_uv.contiguous()), _ptr(center), _ptr(scale_crop),
+                                             B, float(margin), float("nan") if min_score is None else float(min_score),
+                                             _ptr(state.buffer), _stream()), "h3d_track_update")
+
     # ---- operators ---------------------------------------------------------------------------
     def conv2d(self, x, w, b, stride=1, leaky=False):
         x = _chk_f32(x, "x", 4); w = _chk_f32(w, "w", 4); b = _chk_f32(b, "b", 1)
@@ -913,6 +962,33 @@ class PackedConv:
             self.h = None
         except Exception:
             pass
+
+
+class TrackState:
+    """The device state of B tracked streams (include/hand3d_b200.h, H3D_TRACK_*): one float32 buffer of h3d_track_state_bytes(B)
+    bytes and views of it: center [B,2] and scale [B] (the crop the next track step uses), score [B] float32 and lost [B] int32.
+    A new state holds the reference's fall-back crop (centre (160, 160), crop size 100 at its margin 1.25) in every slot, a NaN
+    score and lost = 1: nothing has been found yet.  reset() restores that."""
+
+    def __init__(self, B, device=None):
+        self.B = int(B)
+        words = int(_lib.load().h3d_track_state_bytes(self.B))
+        if words < 0:
+            _lib.check(words, "h3d_track_state_bytes")
+        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.buffer = torch.empty(words // 4, dtype=torch.float32, device=dev)
+        B = self.B
+        self.center = self.buffer[_lib.TRACK_CENTER * B:(_lib.TRACK_CENTER + 2) * B].view(B, 2)
+        self.scale = self.buffer[_lib.TRACK_SCALE * B:(_lib.TRACK_SCALE + 1) * B]
+        self.score = self.buffer[_lib.TRACK_SCORE * B:(_lib.TRACK_SCORE + 1) * B]
+        self.lost = self.buffer[_lib.TRACK_LOST * B:(_lib.TRACK_LOST + 1) * B].view(torch.int32)
+        self.reset()
+
+    def reset(self):
+        self.center.fill_(160.0)
+        self.scale.fill_(float(np.float32(256.0) / (np.float32(100.0) * np.float32(1.25))))
+        self.score.fill_(float("nan"))
+        self.lost.fill_(1)
 
 
 def conv2d_tc_geometry(B, H, W, Cout, pool=0, precision="bf16x3"):

@@ -146,6 +146,41 @@ H3D_API int h3d_pipeline_forward(h3d_ctx* ctx, const float* image, const float* 
 H3D_API int h3d_pose2d_forward(h3d_ctx* ctx, const float* image_crop, int B, int Hc, int Wc, float* keypoints_scoremap,
                                int32_t* keypoints_uv, void* stream);
 
+/* ---- Tracking across camera frames (extends nets/ColorHandPose3DNetwork.py:61-129 and utils/general.py:271-328,347-357) ----
+ * Batch slot b is one camera stream.  A track state is caller-owned DEVICE memory of h3d_track_state_bytes(B) bytes: arrays of B x
+ * 32-bit words (center takes two), the array H3D_TRACK_<name> starting at word H3D_TRACK_<name> * B:
+ *   center [B,2] fp32 (row, col) and scale [B] fp32: the crop the next track step uses;
+ *   score [B] fp32: (sum over k of the peak of channel k of the last PoseNet2D stage's 32x32 map) / 21 (NaN if the map holds NaN);
+ *   lost [B] int32: 1 when the step's key-points were not trusted; a lost slot keeps the crop it had.
+ * The caller initialises center and scale before a first track step (a detect step writes them for every slot it does not lose). */
+#define H3D_TRACK_CENTER 0
+#define H3D_TRACK_SCALE 2
+#define H3D_TRACK_SCORE 3
+#define H3D_TRACK_LOST 4
+#define H3D_TRACK_STATE_WORDS 5
+/* Bytes of a track state of B slots (H3D_TRACK_STATE_WORDS * 4 * B), or H3D_EINVAL for B < 1. */
+H3D_API int64_t h3d_track_state_bytes(int B);
+/* One step of a tracked stream.  detect != 0: h3d_pipeline_forward's computation (no forced crop, no hand_scoremap / hand_mask).
+ * detect == 0: the crop (center, scale) is read from `state`, and HandSegNet, the mask post-processing and the bounding box are not
+ * enqueued; the crop, PoseNet2D, the x8 up-sampling + key-point detection and the lifting stage follow as in h3d_pipeline_forward.
+ * Either way the step ends with track_update_kernel, which derives the next crop from this step's key-points (fp32, round to nearest,
+ * no contraction):
+ *   p[k] = (float(uv[k]) - 128) / scale + center per axis; center' = 0.5 (max_k p + min_k p); size = max(extent_row, extent_col);
+ *   if center' or size is not finite: center' = (160, 160), size = 100, and the slot is lost;
+ *   scale' = min(max(256 / (size * margin), 0.25), 5);
+ *   lost also when min_score is not NaN and !(score >= min_score).  A slot that is not lost takes (center', scale').
+ * Outputs as h3d_pipeline_forward's (any may be NULL except where with_pose3d needs keypoint_coord3d).  Enqueue-only, allocates
+ * nothing, capturable into a CUDA graph.  A track step adds fewer kernels to h3d_launch_count than a detect step by exactly
+ * HandSegNet and the mask post-processing.  H3D_EINVAL before anything is enqueued unless 1 <= H, W <= H3D_PIPELINE_MAX_SIDE, B >= 1,
+ * state is 8-byte aligned, margin is finite and >= 0.25, and min_score is finite or NaN (NaN = no score test). */
+H3D_API int h3d_track_step(h3d_ctx* ctx, const float* image, const float* hand_side, int B, int H, int W, int with_pose3d, int detect,
+                           float margin, float min_score, void* state, float* image_crop, float* scale_crop, float* center,
+                           float* keypoints_scoremap, float* keypoint_coord3d, int32_t* keypoints_uv, void* stream);
+/* The update alone (the operator form of h3d_track_step's last kernel): scoremap32 [B,32,32,21] (the last PoseNet2D stage),
+ * keypoints_uv [B,21,2] int32, center [B,2] and scale_crop [B] of the crop they were found in -> state.  Same argument rules. */
+H3D_API int h3d_track_update(h3d_ctx* ctx, const float* scoremap32, const int32_t* keypoints_uv, const float* center,
+                             const float* scale_crop, int B, float margin, float min_score, void* state, void* stream);
+
 /* ---- operator entry points (utils/general.py) ------------------------------------------------- */
 /* NetworkOps.conv / conv_relu (utils/general.py:36-59): tf.nn.conv2d SAME + bias (+ leaky 0.01).
  * fp32 CUDA-core kernel; x [B,H,W,Cin], w HWIO [k,k,Cin,Cout] (device), y [B,ceil(H/s),ceil(W/s),Cout]. */
