@@ -36,6 +36,7 @@ SIGNATURES = {
     "h3d_scope_ready": (_i, [_p, C.c_char_p]),
     "h3d_workspace_bytes": (_i64, [_p, _i, _i, _i]),
     "h3d_set_workspace": (_i, [_p, _p, _i64]),
+    "h3d_fill_scratch": (_i, [_p, _i, _p]),
     "h3d_handsegnet_forward": (_i, [_p, _p, _i, _i, _i, _p, _p]),
     "h3d_posenet_forward": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _p]),
     "h3d_lifting_forward": (_i, [_p, _p, _p, _i, _i, _p, _p, _p, _p]),

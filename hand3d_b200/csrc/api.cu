@@ -969,7 +969,7 @@ static int check_device() {
 extern "C" {
 
 const char* h3d_last_error(void) { return g_err; }
-int h3d_version(void) { return 107; }
+int h3d_version(void) { return 108; }
 
 int h3d_device_available(void) {
     int n = 0;
@@ -1160,6 +1160,16 @@ int h3d_set_workspace(h3d_ctx* ctx, void* dev_ptr, int64_t bytes) {
     ctx->drop_plans();
     memset(&ctx->lay, 0, sizeof(ctx->lay));
     ctx->ws = (char*)dev_ptr; ctx->ws_bytes = bytes;
+    return H3D_OK;
+}
+
+int h3d_fill_scratch(h3d_ctx* ctx, int byte, void* stream) {
+    H3D_REQUIRE(ctx != nullptr, "h3d_fill_scratch: ctx is NULL");
+    H3D_REQUIRE(byte >= 0 && byte <= 255, "h3d_fill_scratch: byte must be 0..255, got %d", byte);
+    DeviceGuard guard_(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (ctx->op_scratch) H3D_CUDA(cudaMemsetAsync(ctx->op_scratch, byte, (size_t)ctx->op_scratch_bytes, s));
+    if (ctx->ws && ctx->ws_bytes > 0) H3D_CUDA(cudaMemsetAsync(ctx->ws, byte, (size_t)ctx->ws_bytes, s));
     return H3D_OK;
 }
 

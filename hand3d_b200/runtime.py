@@ -152,6 +152,11 @@ class Context:
         _lib.check(self.lib.h3d_set_workspace(self.h, C.c_void_p(base), need), "h3d_set_workspace")
         self._ws_key = (kB, kH, kW)
 
+    def fill_scratch(self, byte):
+        """Fills the workspace and the operator scratch with one byte value on the current stream (h3d_fill_scratch): no result may
+        depend on what they held before a call.  For tests; the scratch grows on demand, so size it with one call first."""
+        _lib.check(self.lib.h3d_fill_scratch(self.h, int(byte), _stream()), "h3d_fill_scratch")
+
     # ---- stages ----------------------------------------------------------------------------
     def handsegnet(self, image):
         image = _chk_f32(image, "image", 4)

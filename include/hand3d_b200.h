@@ -104,9 +104,18 @@ H3D_API int h3d_load_weight(h3d_ctx* ctx, const char* name, const float* host_da
 /* 1 if every variable of `scope` ("HandSegNet", "PoseNet2D", "PosePrior", "ViewpointNet") is loaded. */
 H3D_API int h3d_scope_ready(const h3d_ctx* ctx, const char* scope);
 
-/* Workspace arena for the stage entry points (activations of one batch). */
+/* Workspace arena for the stage entry points (activations of one batch).
+ * The workspace and the context's operator scratch carry no state between calls and need no initialisation: every entry writes
+ * each byte of them it reads earlier in the same call (padding channels, keys of the arg-max reductions and split-K partial sums
+ * included), so any content a previous call, another context or the allocator left there never reaches a result, an address or a
+ * loop bound.  State that outlives a call lives only in caller-owned buffers named as such: the Adam state, the reader queue, the
+ * h3d_eval_* store and the track state. */
 H3D_API int64_t h3d_workspace_bytes(const h3d_ctx* ctx, int B, int H, int W);
 H3D_API int h3d_set_workspace(h3d_ctx* ctx, void* dev_ptr, int64_t bytes);
+/* Fills the current operator scratch and the workspace (when one is set) with `byte` (0..255): one cudaMemsetAsync each on `stream`,
+ * enqueue-only, allocates nothing, capturable.  For tests of the contract above; the scratch grows on demand, so a test sizes it with
+ * one call of the entry under test before filling it. */
+H3D_API int h3d_fill_scratch(h3d_ctx* ctx, int byte, void* stream);
 
 /* ---- stage entry points (fixed layer schedules) --------------------------------------------- */
 /* ColorHandPose3DNetwork.inference_detection (nets/ColorHandPose3DNetwork.py:131-168).
