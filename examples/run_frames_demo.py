@@ -49,6 +49,9 @@ def main():
     ap.add_argument("--track", action="store_true", help="follow the hand from frame to frame; HandSegNet only to (re-)acquire it")
     ap.add_argument("--redetect-every", type=int, default=None, help="with --track: also detect on every N-th batch")
     ap.add_argument("--min-score", type=float, default=None, help="with --track: a slot whose key-point score is lower is lost")
+    ap.add_argument("--detect", default="batch", choices=["batch", "slots"],
+                    help="with --track: re-detect the whole batch when a slot is lost (batch), or only the lost slots, chosen on the "
+                         "device one step after the loss (slots)")
     args = ap.parse_args()
 
     from hand3d_b200 import runtime, weights as Wt
@@ -73,7 +76,8 @@ def main():
         hw = (args.height, args.width)
         batches = synthetic_batches(args.batches, args.batch, hw[0], hw[1], args.seed)
 
-    runner = FrameRunner(ctx, args.batch, hw, track=args.track, redetect_every=args.redetect_every, min_score=args.min_score)
+    runner = FrameRunner(ctx, args.batch, hw, track=args.track, redetect_every=args.redetect_every, min_score=args.min_score,
+                         detect=args.detect)
     t0 = time.perf_counter()
     n = 0
     for i, r in enumerate(runner.stream(batches)):
@@ -81,7 +85,8 @@ def main():
         kp = r["keypoints_frame"][0]
         track = ""
         if args.track:
-            track = " [%s, score %.4g%s]" % ("detect" if r["detected"] else "track", r["track_score"][0],
+            detected = r["track_detected"][0] if args.detect == "slots" else r["detected"]
+            track = " [%s, score %.4g%s]" % ("detect" if detected else "track", r["track_score"][0],
                                              ", lost" if r["track_lost"][0] else "")
         print("batch %d: frame 0 key-points (row, col) in %dx%d pixels: wrist %s, index tip %s%s" % (i, hw[0], hw[1], np.round(kp[0], 1),
                                                                                                  np.round(kp[8], 1), track))

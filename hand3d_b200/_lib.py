@@ -45,6 +45,7 @@ SIGNATURES = {
     "h3d_track_state_bytes": (_i64, [_i]),
     "h3d_track_step": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _f, _f, _p, _p, _p, _p, _p, _p, _p, _p]),
     "h3d_track_update": (_i, [_p, _p, _p, _p, _p, _i, _f, _f, _p, _p]),
+    "h3d_track_step_slots": (_i, [_p, _p, _p, _i, _i, _i, _i, _f, _f, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "h3d_conv2d_f32": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
     "h3d_conv2d_tc": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
     "h3d_conv2d_tc_strided": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p]),

@@ -123,6 +123,10 @@ struct StagePlan {
     int cur_lane = 0;                   // lane given to steps as they are appended (see seal())
     int B = 0, H = 0, W = 0, variant = -1;
     int64_t flops = 0;
+    // counted plan (HandSegNet for the slots a slots step re-detects): every kernel computes only images [0, *count), and the first layer
+    // reads image b of its input at slots[b]; both device pointers are context-owned.  NULL: the whole batch, in order.
+    const int* count = nullptr;
+    const int* slots = nullptr;
     ~StagePlan() {
         for (auto* p : tc) tc_conv_plan_destroy(p);
         for (auto* p : fc) fc_chain_plan_destroy(p);
@@ -149,6 +153,7 @@ struct h3d_ctx {
     float* vp_head_w = nullptr; float* vp_head_b = nullptr;   // fused fc_vp_ux/uy/uz [128,3]
     char* ws = nullptr; int64_t ws_bytes = 0;
     std::unique_ptr<StagePlan> seg, pose, lift;
+    std::unique_ptr<StagePlan> seg_counted;   // HandSegNet's counted plan (h3d_track_step_slots), built on first use beside `seg`
     // persistent buffers inside the workspace (laid out by layout())
     struct Layout {
         int B = 0, H = 0, W = 0;
@@ -158,7 +163,7 @@ struct h3d_ctx {
         float *seg_low, *s[3];
         int64_t seg_off, pose_off, lift_off, total;
     } lay;
-    void drop_plans() { seg.reset(); pose.reset(); lift.reset(); }
+    void drop_plans() { seg.reset(); pose.reset(); lift.reset(); seg_counted.reset(); }
     // independent branches (PosePrior || ViewpointNet, x8 up-sampling || lifting) run on two private streams that fork from
     // and join back into the caller's stream with events (capturable into a CUDA graph)
     cudaStream_t side = nullptr, side2 = nullptr;
@@ -168,6 +173,10 @@ struct h3d_ctx {
     // after the trap has poisoned the CUDA context (h3d_check_errors).
     int* err_flag = nullptr;
     unsigned int* fc_counter = nullptr;      // ticket of the FC-chain kernel ("last cluster applies the rotation epilogue"), zero between launches
+    // Slot selection of h3d_track_step_slots for up to track_cap slots, outside the workspace: track_sel = [count | slots[B] | pos[B]]
+    // (launch_track_select), track_crop = [center [B,2] | scale [B]] of the selected slots in compact order.  Grown (old blocks retired)
+    // when the counted plan is built, so a step itself never allocates.
+    int32_t* track_sel = nullptr; float* track_crop = nullptr; int track_cap = 0;
     // Operator entry points borrow scratch from here instead of allocating per call: grown geometrically on demand, old blocks
     // are retired (not freed) until h3d_destroy, so no call ever synchronises or frees.
     char* op_scratch = nullptr; int64_t op_scratch_bytes = 0;
@@ -433,6 +442,8 @@ static int add_direct(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, con
     a.B = B; a.H = H; a.W = W; a.Cin = l.cin; a.Cout = l.cout; a.k = l.k; a.stride = l.stride; a.leaky = l.leaky;
     a.splitk_scratch = splitk_scratch; a.splitk_scratch_floats = splitk_scratch ? kConvSplitKScratchFloats : 0;
     a.err_flag = ctx->err_flag;
+    a.count = pl->count;
+    a.slots = x ? nullptr : pl->slots;   // the plan's external input is indexed through the slot list
     pl->steps.push_back([a](const Ext& e, cudaStream_t s) {
         DirectConvArgs aa = a;
         if (!aa.x) aa.x = e.in;
@@ -460,6 +471,7 @@ static int add_tc(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, const L
     d.corr_scale = pw->corr_scale;
     d.pool = pool;
     d.err_flag = ctx->err_flag;
+    d.count = pl->count;
     TcConvPlan* tp = tc_conv_plan_create(d, &rc);
     if (!tp) return rc;
     pl->tc.push_back(tp);
@@ -506,8 +518,9 @@ static int build_trunk(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, co
             const Act src = in;
             const int hh = h, ww = w, cc = l.cout;
             if (tc && lo == 4) { set_error("fp16_f8c: max-pool must be fused into the convolution (even H, W required)"); return H3D_EINVAL; }
-            if (tc) pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_maxpool_split(src.s, pooled.s, B, hh, ww, cc, half, s); });
-            else pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_maxpool_f32(src.f, pooled.f, B, hh, ww, cc, s); });
+            const int* cnt = pl->count;
+            if (tc) pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_maxpool_split(src.s, pooled.s, B, hh, ww, cc, half, s, cnt); });
+            else pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_maxpool_f32(src.f, pooled.f, B, hh, ww, cc, s, cnt); });
             pl->launches.push_back(1);
             in = pooled; cur ^= 1; h /= 2; w /= 2;
         }
@@ -516,10 +529,12 @@ static int build_trunk(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, co
     return H3D_OK;
 }
 
-static int build_handsegnet(h3d_ctx* ctx, int B, int H, int W) {
+// count != NULL: the counted plan (ctx->seg_counted), with the same (B, H, W) tiling as ctx->seg; otherwise ctx->seg
+static int build_handsegnet(h3d_ctx* ctx, int B, int H, int W, const int* count = nullptr, const int* slots = nullptr) {
     H3D_REQUIRE(H % 8 == 0 && W % 8 == 0, "HandSegNet: H and W must be multiples of 8 (got %dx%d)", H, W);
     auto pl = std::make_unique<StagePlan>();
     pl->B = B; pl->H = H; pl->W = W;
+    pl->count = count; pl->slots = slots;
     const bool tc = is_tc(ctx->precision);
     char* r = ctx->ws + ctx->lay.seg_off;
     const int64_t se = slot_elems_seg(B, H, W);
@@ -539,9 +554,10 @@ static int build_handsegnet(h3d_ctx* ctx, int B, int H, int W) {
         if ((rc = add_direct(ctx, pl.get(), "HandSegNet", kHandSeg[15], B, h, w, f512, 512, 0, low, 2, 0, Split(), 0, 0))) return rc;
     }
     // e.out == nullptr (pipeline): the x8 up-sampling is fused into the mask post-processing (launch_seg_postprocess reads seg_low)
-    pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return e.out ? launch_resize_bilinear_tf1(low, e.out, B, h, w, 2, H, W, s) : H3D_OK; });
+    const int* cnt = pl->count;
+    pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return e.out ? launch_resize_bilinear_tf1(low, e.out, B, h, w, 2, H, W, s, cnt) : H3D_OK; });
     pl->launches.push_back(1);
-    ctx->seg = std::move(pl);
+    (count ? ctx->seg_counted : ctx->seg) = std::move(pl);
     return H3D_OK;
 }
 
@@ -969,7 +985,7 @@ static int check_device() {
 extern "C" {
 
 const char* h3d_last_error(void) { return g_err; }
-int h3d_version(void) { return 108; }
+int h3d_version(void) { return 109; }
 
 int h3d_device_available(void) {
     int n = 0;
@@ -1047,6 +1063,8 @@ int h3d_destroy(h3d_ctx* ctx) {
     for (void* p : ctx->retired) cudaFree(p);
     if (ctx->err_flag) cudaFreeHost(ctx->err_flag);
     if (ctx->fc_counter) cudaFree(ctx->fc_counter);
+    if (ctx->track_sel) cudaFree(ctx->track_sel);
+    if (ctx->track_crop) cudaFree(ctx->track_crop);
     for (auto& kv : ctx->frame_plans) frame_plan_destroy(kv.second);
     delete ctx;
     return H3D_OK;
@@ -1358,6 +1376,66 @@ int h3d_track_step(h3d_ctx* ctx, const float* image, const float* hand_side, int
                            keypoints_scoremap ? keypoints_scoremap : L.kp_scoremap, keypoint_coord3d, uv, stream);
     }
     if (rc) return rc;
+    if ((rc = launch_track_update(L.s[2], uv, cen, scl, B, margin, min_score, state, s))) return rc;
+    ctx->launches += 1;
+    return H3D_OK;
+}
+
+// HandSegNet's counted plan for (B, H, W) and the selection memory it reads: built outside any step that could be captured mid-way (a
+// failure here enqueues nothing).  A grown selection block retires the old one: graphs captured earlier may still point into it.
+static int ensure_counted_seg(h3d_ctx* ctx, int B, int H, int W) {
+    if (ctx->track_cap < B) {
+        int32_t* sel = nullptr; float* crop = nullptr;
+        H3D_CUDA(cudaMalloc(&sel, (size_t)(1 + 2 * B) * sizeof(int32_t)));
+        if (cudaMalloc(&crop, (size_t)3 * B * sizeof(float)) != cudaSuccess) {
+            cudaFree(sel);
+            return cuda_fail(cudaGetLastError(), "cudaMalloc(track_crop)", __FILE__, __LINE__);
+        }
+        if (ctx->track_sel) { ctx->retired.push_back(ctx->track_sel); ctx->retired.push_back(ctx->track_crop); }
+        ctx->track_sel = sel; ctx->track_crop = crop; ctx->track_cap = B;
+        ctx->seg_counted.reset();   // it points into the old block
+    }
+    const StagePlan* p = ctx->seg_counted.get();
+    if (p && p->B == B && p->H == H && p->W == W && p->count == ctx->track_sel) return H3D_OK;
+    return build_handsegnet(ctx, B, H, W, ctx->track_sel, ctx->track_sel + 1);
+}
+
+int h3d_track_step_slots(h3d_ctx* ctx, const float* image, const float* hand_side, int B, int H, int W, int with_pose3d, float margin,
+                         float min_score, void* state, const int32_t* force, int32_t* detected, float* image_crop, float* scale_crop,
+                         float* center, float* keypoints_scoremap, float* keypoint_coord3d, int32_t* keypoints_uv, void* stream) {
+    DeviceGuard guard_(ctx ? ctx->device : 0);
+    H3D_PIPELINE_CHECKS("h3d_track_step_slots");
+    H3D_TRACK_CHECKS("h3d_track_step_slots");
+    cudaStream_t s = (cudaStream_t)stream;
+    int rc;
+    if ((rc = ensure_layout_covers(ctx, B, H, W, 256, 256))) return rc;
+    if ((rc = ensure_counted_seg(ctx, B, H, W))) return rc;
+    h3d_ctx::Layout& L = ctx->lay;
+    float* cen = center ? center : L.center;
+    float* scl = scale_crop ? scale_crop : L.scale;
+    int32_t* uv = keypoints_uv ? keypoints_uv : L.kp_uv;
+    const int32_t* count = ctx->track_sel;
+    float* cen_c = ctx->track_crop;
+    float* scl_c = ctx->track_crop + 2 * B;
+    // 1. the slots to re-detect, from the lost flags the previous step's update wrote (stream order) and the caller's mask
+    if ((rc = launch_track_select(state, force, B, ctx->track_sel, detected, s))) return rc;
+    ctx->launches += 1;
+    // 2. HandSegNet and the mask post-processing on the selected slots only, in compact order (slot slots[i] -> image i); the x8
+    //    up-sampling fused into the post-processing or on its own, as in h3d_pipeline_forward
+    const bool fuse_up = !tc_tuning().no_seg_fusion;
+    Ext e; e.in = image; e.out = fuse_up ? nullptr : L.hand_scoremap;
+    if ((rc = run_plan(ctx, ctx->seg_counted.get(), e, s))) return rc;
+    if (fuse_up) ctx->launches -= 1;   // the skipped up-sampling step
+    int nl = 0;
+    if ((rc = launch_seg_postprocess(L.hand_scoremap, B, H, W, L.seg_scratch, nullptr, nullptr, cen_c, L.crop_size, scl_c, s, &nl,
+                                     fuse_up ? L.seg_low : nullptr, H / 8, W / 8, count))) return rc;
+    ctx->launches += nl;
+    // 3. the step's crop: detected for the selected slots, the state's for the others
+    if ((rc = launch_track_merge(state, ctx->track_sel, cen_c, scl_c, B, cen, scl, s))) return rc;
+    ctx->launches += 1;
+    // 4. the rest of the pipeline on every slot, then the update
+    if ((rc = pipeline_tail(ctx, image, hand_side, B, H, W, with_pose3d, cen, scl, image_crop ? image_crop : L.image_crop,
+                            keypoints_scoremap ? keypoints_scoremap : L.kp_scoremap, keypoint_coord3d, uv, stream))) return rc;
     if ((rc = launch_track_update(L.s[2], uv, cen, scl, B, margin, min_score, state, s))) return rc;
     ctx->launches += 1;
     return H3D_OK;

@@ -109,19 +109,23 @@ struct LaunchCounter {
 };
 
 // ---------------------------------------------------------------- kernels (elementwise.cu)
-int launch_resize_bilinear_tf1(const float* x, float* y, int B, int H, int W, int C, int oh, int ow, cudaStream_t s);
-int launch_maxpool_f32(const float* x, float* y, int B, int H, int W, int C, cudaStream_t s);
+// count (optional, device int): only images [0, *count) are resized (needs a size change)
+int launch_resize_bilinear_tf1(const float* x, float* y, int B, int H, int W, int C, int oh, int ow, cudaStream_t s,
+                               const int* count = nullptr);
+// count (optional, device int): only images [0, *count) are pooled (HandSegNet's counted plan)
+int launch_maxpool_f32(const float* x, float* y, int B, int H, int W, int C, cudaStream_t s, const int* count = nullptr);
 // gradient of the 2x2 / 2 VALID max-pool: dy [B,H/2,W/2,C] -> dx [B,H,W,C], each window's gradient to its first maximum (row-major)
 int launch_maxpool_backward_f32(const float* x, const float* dy, float* dx, int B, int H, int W, int C, cudaStream_t s);
-int launch_maxpool_split(Split x, Split y, int B, int H, int W, int C, Half16 t, cudaStream_t s);
+int launch_maxpool_split(Split x, Split y, int B, int H, int W, int C, Half16 t, cudaStream_t s, const int* count = nullptr);
 int launch_avgpool8(const float* x, float* y, int B, int H, int W, int C, cudaStream_t s);
 int launch_f32_to_split(const float* x, Split y, int64_t rows, int C, int Cpad, Half16 t, cudaStream_t s);
 int launch_split_to_f32(Split x, float* y, int64_t rows, int C, int Cpad, Half16 t, cudaStream_t s);
-// seg post-process: scratch must hold seg_scratch_bytes(B,H,W) bytes (zeroed by the launcher).
+// seg post-process: scratch must hold seg_scratch_bytes(B,H,W) bytes (zeroed by the launcher).  count (optional, device int): only
+// images [0, *count) are processed; the blocks of the others exit at once.
 int64_t seg_scratch_bytes(int B, int H, int W);
 int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scratch, uint8_t* hand_mask,
                            int32_t* max_loc, float* center, float* crop_size, float* scale_crop, cudaStream_t s,
-                           int* n_launch, const float* low = nullptr, int LH = 0, int LW = 0);
+                           int* n_launch, const float* low = nullptr, int LH = 0, int LW = 0, const int* count = nullptr);
 int launch_crop_image(const float* image, const float* center, const float* scale, float* out, int B, int H, int W,
                       int C, int crop, cudaStream_t s);
 int64_t argmax_scratch_bytes(int B, int C);
@@ -181,6 +185,13 @@ int launch_eval_stats(const void* store, int K, int N, int dtype, const double* 
 // H3D_TRACK_*); min_score NaN = no score test.  One kernel.
 int launch_track_update(const float* map32, const int32_t* uv, const float* center, const float* scale, int B, float margin,
                         float min_score, void* state, cudaStream_t s);
+// The slots a slots step re-detects (h3d_track_step_slots): slot b is selected when state lost[b] != 0 or force[b] != 0 (force may be
+// NULL).  sel = [count | slots[B] | pos[B]]: count = n, slots[0..n) the selected slots in ascending order, pos[b] = the compact index
+// of slot b or -1; detected [B] (optional) = 1 for a selected slot.  One CTA, positions by prefix sum.
+int launch_track_select(const void* state, const int32_t* force, int B, int32_t* sel, int32_t* detected, cudaStream_t s);
+// center [B,2] / scale [B] of the step: the compact detection (cen_c, scl_c at pos[b]) for a selected slot, the state's crop otherwise.
+int launch_track_merge(const void* state, const int32_t* sel, const float* cen_c, const float* scl_c, int B, float* center, float* scale,
+                       cudaStream_t s);
 
 // ---------------------------------------------------------------- kernels (conv_direct.cu)
 struct DirectConvArgs {
@@ -197,6 +208,10 @@ struct DirectConvArgs {
     float* splitk_scratch = nullptr;        // optional: enables deterministic split-K for layers with too few tiles
     int64_t splitk_scratch_floats = 0;
     int* err_flag = nullptr;                // forwarded to the tensor-core first-layer kernel (bounded barrier waits)
+    // counted batch (HandSegNet's second plan): only images [0, *count) are computed (device int, read in stream order); with slots,
+    // image b of the input x is image slots[b] of it.  Counted layers never split K.
+    const int* count = nullptr;
+    const int* slots = nullptr;
 };
 constexpr int64_t kConvSplitKScratchFloats = 600ll * 64 * 64;   // upper bound used by launch_conv_direct's split-K policy
 int launch_conv_direct(const DirectConvArgs& a, cudaStream_t s);
@@ -213,8 +228,9 @@ int launch_concat_handside_split(const float* feat, const float* hand_side, Spli
 
 // ---------------------------------------------------------------- kernels (conv_wgmma.cu)
 // first layer (Cin = 3, 3x3, 64 output channels) on the tensor cores, writing split planes (hi, lo optional)
+// (count, slots: as DirectConvArgs)
 int launch_conv_c3_tc(const float* x, const float* w, const float* bias, Split y, int Cs_total, int cs_off, int B, int H, int W, int leaky,
-                      Half16 half, cudaStream_t s, int* err_flag = nullptr);
+                      Half16 half, cudaStream_t s, int* err_flag = nullptr, const int* count = nullptr, const int* slots = nullptr);
 struct TcConvPlan;  // opaque: tensor maps + launch geometry of one tensor-core conv layer
 struct TcConvDesc {
     // input activations (split planes) [B,H,W,Cin_total]; channels [0,Cin_pad) are read (Cin_pad % 64 == 0)
@@ -236,6 +252,7 @@ struct TcConvDesc {
     Half16 half;
     int pool = 0;  // 1: fuse the following 2x2/2 max-pool; 2: stride-2 'SAME' convolution (even H, W); outputs are [B, H/2, W/2, C]
     int* err_flag = nullptr;   // device int: a barrier wait that times out stores its code here before trapping (h3d_ctx owns it)
+    const int* count = nullptr;   // device int (optional): only images [0, *count) are computed, read after the grid-dependency wait
 };
 // Tuning switches: initialised from the environment once (H3D_TC_BN, H3D_FC_CHAIN, ...), changed only through tc_set_tuning().
 struct TcTuning {

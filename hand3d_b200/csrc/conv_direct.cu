@@ -33,6 +33,8 @@ struct ConvGeom {
     uint8_t* yl8; uint8_t* yh8;   // fp16_f8c planes (see split_fmt.cuh); yhi then holds fp16
     int k_per_split;     // reduction range handled by one blockIdx.z (multiple of KC); == Ktot when not split
     float* partial;      // split-K: raw partial sums [gridDim.z][M][Cout]
+    const int* count;    // counted batch: only images [0, *count) (DirectConvArgs::count); never with split-K
+    const int* slots;    // image b of the launch is image slots[b] of x (DirectConvArgs::slots)
 };
 
 // VEC: Cin % 16 == 0 and 16-byte aligned input channels -> one tap per K chunk, float4 gathers.
@@ -44,8 +46,9 @@ conv_direct_kernel(const float* __restrict__ x, const float* __restrict__ w, con
     __shared__ __align__(16) float Bs[KC][TN + 4];
     const int t = threadIdx.x;
     const int tx = t & 15, ty = t >> 4;
-    const int64_t M = (int64_t)g.B * g.Ho * g.Wo;
+    const int64_t M = (int64_t)(g.count ? min(*g.count, g.B) : g.B) * g.Ho * g.Wo;
     const int64_t m0 = (int64_t)blockIdx.x * TM;
+    if (m0 >= M) return;   // counted batch: the whole CTA lies past the last image
     const int n0 = blockIdx.y * TN;
     const int Ktot = g.k * g.k * g.Cin;
 
@@ -60,7 +63,7 @@ conv_direct_kernel(const float* __restrict__ x, const float* __restrict__ w, con
         ab = (int)(am / ((int64_t)g.Wo * g.Ho));
     }
     const int iy0 = aoy * g.stride - g.pad_t, ix0 = aox * g.stride - g.pad_l;
-    const float* xb = x + (int64_t)ab * g.H * g.W * g.Cin_total + g.cin_off;
+    const float* xb = x + (int64_t)(g.slots && a_valid ? g.slots[ab] : ab) * g.H * g.W * g.Cin_total + g.cin_off;
 
     float acc[4][4];
 #pragma unroll
@@ -209,19 +212,20 @@ template <bool FP16>
 __global__ void __launch_bounds__(256, 2)
 conv3x3_c3_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias, float* __restrict__ y,
                   uint16_t* __restrict__ yhi, uint16_t* __restrict__ ylo, uint8_t* __restrict__ yl8, uint8_t* __restrict__ yh8, int B, int H,
-                  int W, int Cy_total, int cy_off, int Cs_total, int cs_off, int leaky) {
+                  int W, int Cy_total, int cy_off, int Cs_total, int cs_off, int leaky, const int* __restrict__ count,
+                  const int* __restrict__ slots) {
     __shared__ __align__(16) float ws[27][64];
     __shared__ __align__(16) float xs[3][C3_TH + 2][C3_LD];
     const int t = threadIdx.x;
     const int tiles_w = (W + C3_TW - 1) / C3_TW, tiles_h = (H + C3_TH - 1) / C3_TH;
-    const int num_tiles = tiles_w * tiles_h * B;
+    const int num_tiles = tiles_w * tiles_h * (count ? min(*count, B) : B);   // images are the slowest tile index
     for (int i = t; i < 27 * 64; i += 256) (&ws[0][0])[i] = __ldg(w + i);      // weights staged once per CTA
     for (int i = t; i < 3 * (C3_TH + 2) * C3_LD; i += 256) (&xs[0][0][0])[i] = 0.f;   // alignment padding columns stay zero
     for (int tile = blockIdx.x * C3_TILES_PER_CTA; tile < min(num_tiles, (blockIdx.x + 1) * C3_TILES_PER_CTA); ++tile) {
     const int tw = tile % tiles_w, th = (tile / tiles_w) % tiles_h, b = tile / (tiles_w * tiles_h);
     const int x0 = tw * C3_TW, y0 = th * C3_TH;
     __syncthreads();                                                            // previous tile fully consumed (and ws visible)
-    const float* xb = x + (int64_t)b * H * W * 3;
+    const float* xb = x + (int64_t)(slots ? slots[b] : b) * H * W * 3;
     for (int i = t; i < (C3_TH + 2) * (C3_TW + 2) * 3; i += 256) {              // haloed input tile (contiguous (x, c) reads), zero outside the image
         const int r = i / ((C3_TW + 2) * 3), rem = i - r * ((C3_TW + 2) * 3);
         const int c = rem / 3, ci = rem - c * 3;
@@ -320,6 +324,7 @@ static void plan_direct(const DirectConvArgs& a, ConvGeom* gp, dim3* gridp, int*
     g.Cin_total = a.Cin_total; g.cin_off = a.cin_off; g.Cout_total = a.Cout_total; g.cout_off = a.cout_off;
     g.Cs_total = a.Cs_total; g.cs_off = a.cs_off; g.leaky = a.leaky;
     g.yl8 = a.ys.l8; g.yh8 = a.ys.h8;
+    g.count = a.count; g.slots = a.slots;
     const int64_t M = (int64_t)g.B * g.Ho * g.Wo;
     dim3 grid((unsigned)ceil_div64(M, TM), (unsigned)ceil_div(a.Cout, TN));
     const int Ktot = a.k * a.k * a.Cin;
@@ -327,7 +332,7 @@ static void plan_direct(const DirectConvArgs& a, ConvGeom* gp, dim3* gridp, int*
     g.partial = nullptr;
     int ksplit = 1;
     const int ctas = (int)(grid.x * grid.y);
-    if (a.splitk_scratch && a.y && !a.ys.hi && ctas < 296 && Ktot >= 256) {
+    if (a.splitk_scratch && !a.count && a.y && !a.ys.hi && ctas < 296 && Ktot >= 256) {
         // tiny spatial maps (the stride-2 lifting pyramids): too few tiles to fill 132 SMs -> split the reduction
         ksplit = std::min(ceil_div(Ktot, 128), std::max(1, 592 / ctas));
         if (ksplit > 1 && (int64_t)ksplit * M * a.Cout <= a.splitk_scratch_floats) {
@@ -351,13 +356,13 @@ int conv_direct_num_launches(const DirectConvArgs& a) {
 int launch_conv_direct(const DirectConvArgs& a, cudaStream_t s) {
     H3D_REQUIRE(a.k >= 1 && a.stride >= 1 && a.Cin >= 1 && a.Cout >= 1, "conv_direct: bad geometry");
     if (is_c3_case(a) && !a.y && a.ys.hi && !a.ys.l8 && !tc_tuning().c3_ffma)   // split planes only: tensor-core version
-        return launch_conv_c3_tc(a.x, a.w, a.bias, a.ys, a.Cs_total, a.cs_off, a.B, a.H, a.W, a.leaky, a.half, s, a.err_flag);
+        return launch_conv_c3_tc(a.x, a.w, a.bias, a.ys, a.Cs_total, a.cs_off, a.B, a.H, a.W, a.leaky, a.half, s, a.err_flag, a.count, a.slots);
     if (is_c3_case(a)) {
         const int tiles = ceil_div(ceil_div(a.W, C3_TW) * ceil_div(a.H, C3_TH) * a.B, C3_TILES_PER_CTA);
         if (a.half == Half16::FP16)
-            conv3x3_c3_kernel<true><<<tiles, 256, 0, s>>>(a.x, a.w, a.bias, a.y, a.ys.hi, a.ys.lo, a.ys.l8, a.ys.h8, a.B, a.H, a.W, a.Cout_total, a.cout_off, a.Cs_total, a.cs_off, a.leaky);
+            conv3x3_c3_kernel<true><<<tiles, 256, 0, s>>>(a.x, a.w, a.bias, a.y, a.ys.hi, a.ys.lo, a.ys.l8, a.ys.h8, a.B, a.H, a.W, a.Cout_total, a.cout_off, a.Cs_total, a.cs_off, a.leaky, a.count, a.slots);
         else
-            conv3x3_c3_kernel<false><<<tiles, 256, 0, s>>>(a.x, a.w, a.bias, a.y, a.ys.hi, a.ys.lo, a.ys.l8, a.ys.h8, a.B, a.H, a.W, a.Cout_total, a.cout_off, a.Cs_total, a.cs_off, a.leaky);
+            conv3x3_c3_kernel<false><<<tiles, 256, 0, s>>>(a.x, a.w, a.bias, a.y, a.ys.hi, a.ys.lo, a.ys.l8, a.ys.h8, a.B, a.H, a.W, a.Cout_total, a.cout_off, a.Cs_total, a.cs_off, a.leaky, a.count, a.slots);
         H3D_CHECK_LAUNCH();
         return H3D_OK;
     }

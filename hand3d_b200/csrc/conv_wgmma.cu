@@ -73,7 +73,15 @@ struct TcParams {
     int leaky;
     int* err_flag;
     const float* w_scale;   // fp16 weight planes (PASSES 1 / 3): [Cout_pad] 2^-s per output channel (split_fmt.cuh)
+    const int* count;       // NULL, or a device int: only images [0, *count) are computed (read after the grid-dependency wait)
 };
+
+// The tile-loop bound and the image bound of a (possibly counted) launch.  The image-group index varies slowest in the tile index, so
+// the tiles of the first n images are the prefix [0, ceil(n / TB) * tiles_w * tiles_h * n_tiles) of [0, num_tiles).
+__device__ __forceinline__ int counted_images(const TcParams& p) { return p.count ? min(*p.count, p.B) : p.B; }
+__device__ __forceinline__ int counted_tiles(const TcParams& p, int nb) {
+    return p.count ? min(p.num_tiles, (nb + p.TB - 1) / p.TB * p.tiles_w * p.tiles_h * p.n_tiles) : p.num_tiles;
+}
 
 // bias + leaky ReLU + store of 32 consecutive output channels [n, n+32) of one pixel (fp32 and / or hi-lo split planes).
 // w_scale (fp16 weight planes): [n, n+32) per-channel factors 2^-s that un-do the weight shift, in global memory (read through the
@@ -373,12 +381,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_consta
     __syncthreads();
     pdl_launch_dependents();
     pdl_wait();
+    const int nb = counted_images(p), num_tiles = counted_tiles(p, nb);   // the producer and the consumers walk the same tiles
 
     if (wg == 0) {
         setmaxnreg_dec<kProducerRegs>();
         if (warp == 0) {
             // ================================ TMA producer (whole warp, one elected lane issues) ================================
-            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
                 const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h, tb = mt / (p.tiles_w * p.tiles_h);
                 const int w0 = tw * p.TW - p.pad, h0 = th * p.TH - p.pad, b0 = tb * p.TB, n0 = nt * BN;
@@ -395,14 +404,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_consta
         // ================================ wgmma + epilogue (warpgroups 1 and 2) ================================
         const int ct = threadIdx.x - 128;
         float racc[BN / 2];
-        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
             const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h, tb = mt / (p.tiles_w * p.tiles_h);
             mma_tile<BN, PASSES, FP16>(ring, kblocks, p.chunk_kb, racc, ct >> 7, lane, p.err_flag);
             store_tile<BN, PASSES, FP16>(p, racc, stg, ct, nt * BN, [&](int row, int64_t& pix, bool& valid) {
                 const int w_l = row % p.TW, h_l = (row / p.TW) % p.TH, b_l = row / (p.TW * p.TH);
                 const int w = tw * p.TW + w_l, h = th * p.TH + h_l, b = tb * p.TB + b_l;
-                valid = (w < p.W) && (h < p.H) && (b < p.B);
+                valid = (w < p.W) && (h < p.H) && (b < nb);
                 pix = ((int64_t)b * p.H + h) * p.W + w;
                 if (p.pool) {   // 1: pooled output pixel, the even-(w, h) lane of each 2x2 window stores; 2: stride-2 'SAME' conv on an
                                 // even-sized map = the stride-1 result at the odd pixels (TF pads 0 before / 1 after, SURVEY.md 9.1)
@@ -430,9 +439,11 @@ constexpr int C3T_PW = C3_TW + 2, C3T_PH = C3_TH + 2;
 constexpr int C3T_PATCH_FLOATS = C3T_PH * C3T_PW * 3;   // 540
 constexpr int C3T_SMEM = C3T_B_BYTES + 2 * A_TILE_BYTES + STG_BYTES + C3T_PATCH_FLOATS * 4 + 64 * 4 + 1024 /*align*/;
 
-template <bool FP16>
+// COUNTED (p.count set): only images [0, *p.count) are computed, and with slots image b of the launch is image slots[b] of x (the counted
+// plan's first layer reads the selected slots in place).  The uncounted instances are the kernel as it was before the count existed.
+template <bool FP16, bool COUNTED>
 __global__ void __launch_bounds__(C3T_THREADS, 2)
-conv_c3_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, const TcParams p) {
+conv_c3_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, const TcParams p, const int* __restrict__ slots) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* bsm = smem;                                   // [W_hi 64 rows ; W_lo 64 rows] x 128 B
@@ -468,15 +479,16 @@ conv_c3_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, cons
     }
     pdl_launch_dependents();
     pdl_wait();
+    const int num_tiles = COUNTED ? counted_tiles(p, counted_images(p)) : p.num_tiles;   // TB = 1: whole images
 
     const uint32_t sb = smem_u32(bsm), sa = smem_u32(asm_);
     const uint64_t b_hi = desc_sw128(sb), b_lo = desc_sw128(sb + 64 * 128);
     const uint64_t a_hi = desc_sw128(sa + wg * 64 * 128), a_lo = desc_sw128(sa + A_TILE_BYTES + wg * 64 * 128);
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int tw = tile % p.tiles_w, th = (tile / p.tiles_w) % p.tiles_h, b = tile / (p.tiles_w * p.tiles_h);
         {   // haloed input patch, zero outside the image ('SAME' padding)
             const int x0 = tw * C3_TW - 1, y0 = th * C3_TH - 1;
-            const float* xb = x + (int64_t)b * p.H * p.W * 3;
+            const float* xb = x + (int64_t)(COUNTED && slots ? slots[b] : b) * p.H * p.W * 3;
             for (int i = t; i < C3T_PATCH_FLOATS; i += C3T_THREADS) {
                 const int r = i / (C3T_PW * 3), rem = i - r * (C3T_PW * 3);
                 const int gy = y0 + r, gx = x0 + rem / 3;
@@ -873,6 +885,7 @@ TcConvPlan* tc_conv_plan_create(const TcConvDesc& d, int* rc) {
     p.pool = d.pool;
     p.err_flag = d.err_flag;
     p.w_scale = d.w_scale;
+    p.count = d.count;
     // <= ~108 accumulating tensor-core steps per partial sum (9 K blocks x 4 K steps x 3 passes)
     p.chunk_kb = d.passes >= 3 ? 9 : 27;
     if (tune.chunk_kb > 0) p.chunk_kb = tune.chunk_kb;
@@ -924,7 +937,7 @@ int tc_conv_launch(const TcConvPlan* pl, cudaStream_t s) {
 // conv1_1 (3 -> 64 channels, 3x3, stride 1) on the tensor cores: x fp32 [B,H,W,3], w fp32 HWIO [3,3,3,64] and bias [64] on the
 // device, output split planes y (hi, and lo when present) [B,H,W,Cs_total] at channel offset cs_off.
 int launch_conv_c3_tc(const float* x, const float* w, const float* bias, Split y, int Cs_total, int cs_off, int B, int H, int W, int leaky,
-                      Half16 half, cudaStream_t s, int* err_flag) {
+                      Half16 half, cudaStream_t s, int* err_flag, const int* count, const int* slots) {
     H3D_REQUIRE(x && w && bias && y.hi && !y.l8 && (Cs_total % 8) == 0 && (cs_off % 8) == 0, "conv_c3_tc: bad argument");
     TcParams p{};
     p.bias = bias;
@@ -934,13 +947,16 @@ int launch_conv_c3_tc(const float* x, const float* w, const float* bias, Split y
     p.TW = C3_TW; p.TH = C3_TH; p.TB = 1;
     p.tiles_w = ceil_div(W, C3_TW); p.tiles_h = ceil_div(H, C3_TH); p.n_tiles = 1;
     p.num_tiles = p.tiles_w * p.tiles_h * B;
-    p.n_valid = 64; p.pool = 0; p.chunk_kb = 1; p.leaky = leaky; p.err_flag = err_flag;
+    p.n_valid = 64; p.pool = 0; p.chunk_kb = 1; p.leaky = leaky; p.err_flag = err_flag; p.count = count;
     const int grid = std::min(p.num_tiles, 2 * tc_num_sms());   // two co-resident CTAs per SM
-    static bool attr_h[kMaxDevices] = {}, attr_b[kMaxDevices] = {};
-    if (int rc = smem_opt_in(conv_c3_tc_kernel<true>, C3T_SMEM, attr_h)) return rc;
-    if (int rc = smem_opt_in(conv_c3_tc_kernel<false>, C3T_SMEM, attr_b)) return rc;
-    if (half == Half16::FP16) H3D_CUDA(launch_pdl(conv_c3_tc_kernel<true>, dim3(grid), dim3(C3T_THREADS), (size_t)C3T_SMEM, s, x, w, p));
-    else H3D_CUDA(launch_pdl(conv_c3_tc_kernel<false>, dim3(grid), dim3(C3T_THREADS), (size_t)C3T_SMEM, s, x, w, p));
+    static bool attr[4][kMaxDevices] = {};
+    if (int rc = smem_opt_in(conv_c3_tc_kernel<true, false>, C3T_SMEM, attr[0])) return rc;
+    if (int rc = smem_opt_in(conv_c3_tc_kernel<false, false>, C3T_SMEM, attr[1])) return rc;
+    if (int rc = smem_opt_in(conv_c3_tc_kernel<true, true>, C3T_SMEM, attr[2])) return rc;
+    if (int rc = smem_opt_in(conv_c3_tc_kernel<false, true>, C3T_SMEM, attr[3])) return rc;
+    auto* k = half == Half16::FP16 ? (count ? conv_c3_tc_kernel<true, true> : conv_c3_tc_kernel<true, false>)
+                                   : (count ? conv_c3_tc_kernel<false, true> : conv_c3_tc_kernel<false, false>);
+    H3D_CUDA(launch_pdl(k, dim3(grid), dim3(C3T_THREADS), (size_t)C3T_SMEM, s, x, w, p, slots));
     return H3D_OK;
 }
 

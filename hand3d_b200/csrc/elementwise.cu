@@ -24,7 +24,8 @@ __device__ __forceinline__ float lerp_tf(float a, float b, float t) {
 // CT > 0: channel count known at compile time (2 and 21 on the hot path) -> the per-element e / C becomes a multiply-shift.
 template <int CT>
 __global__ void resize_bilinear_tf1_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W,
-                                           int C_rt, int oh, int ow, float hscale, float wscale) {
+                                           int C_rt, int oh, int ow, float hscale, float wscale, const int* __restrict__ count) {
+    if (count) B = min(*count, B);   // counted batch: only images [0, *count)
     const int C = CT > 0 ? CT : C_rt;
     const int row_elems = ow * C;
     const int vec_per_row = (row_elems + 3) >> 2;
@@ -69,7 +70,8 @@ __global__ void resize_bilinear_tf1_kernel(const float* __restrict__ x, float* _
     }
 }
 
-int launch_resize_bilinear_tf1(const float* x, float* y, int B, int H, int W, int C, int oh, int ow, cudaStream_t s) {
+int launch_resize_bilinear_tf1(const float* x, float* y, int B, int H, int W, int C, int oh, int ow, cudaStream_t s, const int* count) {
+    H3D_REQUIRE(!count || !(H == oh && W == ow), "resize_bilinear_tf1: a counted batch needs a size change");
     if (H == oh && W == ow) {  // TF returns the input unchanged when the size already matches
         H3D_CUDA(cudaMemcpyAsync(y, x, (size_t)B * H * W * C * sizeof(float), cudaMemcpyDeviceToDevice, s));
         return H3D_OK;
@@ -78,9 +80,9 @@ int launch_resize_bilinear_tf1(const float* x, float* y, int B, int H, int W, in
     const int64_t total = (int64_t)B * oh * ((ow * C + 3) / 4);
     const int threads = 256;
     const int blocks = (int)std::min<int64_t>(ceil_div64(total, threads), 132 * 32);
-    if (C == 21) resize_bilinear_tf1_kernel<21><<<blocks, threads, 0, s>>>(x, y, B, H, W, C, oh, ow, hscale, wscale);
-    else if (C == 2) resize_bilinear_tf1_kernel<2><<<blocks, threads, 0, s>>>(x, y, B, H, W, C, oh, ow, hscale, wscale);
-    else resize_bilinear_tf1_kernel<0><<<blocks, threads, 0, s>>>(x, y, B, H, W, C, oh, ow, hscale, wscale);
+    if (C == 21) resize_bilinear_tf1_kernel<21><<<blocks, threads, 0, s>>>(x, y, B, H, W, C, oh, ow, hscale, wscale, count);
+    else if (C == 2) resize_bilinear_tf1_kernel<2><<<blocks, threads, 0, s>>>(x, y, B, H, W, C, oh, ow, hscale, wscale, count);
+    else resize_bilinear_tf1_kernel<0><<<blocks, threads, 0, s>>>(x, y, B, H, W, C, oh, ow, hscale, wscale, count);
     H3D_CHECK_LAUNCH();
     return H3D_OK;
 }
@@ -88,7 +90,9 @@ int launch_resize_bilinear_tf1(const float* x, float* y, int B, int H, int W, in
 // =============================================================================================
 // NetworkOps.max_pool 2x2/2 VALID (utils/general.py:62-65)
 // =============================================================================================
-__global__ void maxpool_f32_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W, int C) {
+// count (optional): only images [0, *count) are pooled
+__global__ void maxpool_f32_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W, int C, const int* __restrict__ count) {
+    if (count) B = min(*count, B);
     const int Ho = H >> 1, Wo = W >> 1;
     const int C4 = C >> 2;
     const int64_t total = (int64_t)B * Ho * Wo * C4;
@@ -108,7 +112,9 @@ __global__ void maxpool_f32_kernel(const float* __restrict__ x, float* __restric
     }
 }
 
-__global__ void maxpool_f32_scalar_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W, int C) {
+__global__ void maxpool_f32_scalar_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W, int C,
+                                          const int* __restrict__ count) {
+    if (count) B = min(*count, B);
     const int Ho = H >> 1, Wo = W >> 1;
     const int64_t total = (int64_t)B * Ho * Wo * C;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -121,14 +127,14 @@ __global__ void maxpool_f32_scalar_kernel(const float* __restrict__ x, float* __
     }
 }
 
-int launch_maxpool_f32(const float* x, float* y, int B, int H, int W, int C, cudaStream_t s) {
+int launch_maxpool_f32(const float* x, float* y, int B, int H, int W, int C, cudaStream_t s, const int* count) {
     const int threads = 256;
     if ((C & 3) == 0) {
         const int64_t total = (int64_t)B * (H / 2) * (W / 2) * (C / 4);
-        maxpool_f32_kernel<<<(int)std::min<int64_t>(ceil_div64(total, threads), 132 * 32), threads, 0, s>>>(x, y, B, H, W, C);
+        maxpool_f32_kernel<<<(int)std::min<int64_t>(ceil_div64(total, threads), 132 * 32), threads, 0, s>>>(x, y, B, H, W, C, count);
     } else {
         const int64_t total = (int64_t)B * (H / 2) * (W / 2) * C;
-        maxpool_f32_scalar_kernel<<<(int)std::min<int64_t>(ceil_div64(total, threads), 132 * 32), threads, 0, s>>>(x, y, B, H, W, C);
+        maxpool_f32_scalar_kernel<<<(int)std::min<int64_t>(ceil_div64(total, threads), 132 * 32), threads, 0, s>>>(x, y, B, H, W, C, count);
     }
     H3D_CHECK_LAUNCH();
     return H3D_OK;
@@ -184,7 +190,8 @@ __device__ __forceinline__ uint16_t f32_to_h16(float v) {
 // (hi, lo) pair is carried through unchanged, so the pooled value is exactly one of the inputs.
 template <bool FP16, bool HAS_LO>
 __global__ void maxpool_split_kernel(const uint4* __restrict__ xh, const uint4* __restrict__ xl, uint4* __restrict__ yh,
-                                     uint4* __restrict__ yl, int B, int H, int W, int C8) {
+                                     uint4* __restrict__ yl, int B, int H, int W, int C8, const int* __restrict__ count) {
+    if (count) B = min(*count, B);   // counted batch: only images [0, *count)
     const int Ho = H >> 1, Wo = W >> 1;
     const int64_t total = (int64_t)B * Ho * Wo * C8;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -215,7 +222,7 @@ __global__ void maxpool_split_kernel(const uint4* __restrict__ xh, const uint4* 
     }
 }
 
-int launch_maxpool_split(Split x, Split y, int B, int H, int W, int C, Half16 t, cudaStream_t s) {
+int launch_maxpool_split(Split x, Split y, int B, int H, int W, int C, Half16 t, cudaStream_t s, const int* count) {
     H3D_REQUIRE((C & 7) == 0, "maxpool_split: C %% 8 != 0");
     const int threads = 256;
     const int64_t total = (int64_t)B * (H / 2) * (W / 2) * (C / 8);
@@ -224,11 +231,11 @@ int launch_maxpool_split(Split x, Split y, int B, int H, int W, int C, Half16 t,
     uint4 *yh = (uint4*)y.hi, *yl = (uint4*)y.lo;
     const bool lo = x.lo != nullptr;
     if (t == Half16::FP16) {
-        if (lo) maxpool_split_kernel<true, true><<<blocks, threads, 0, s>>>(xh, xl, yh, yl, B, H, W, C / 8);
-        else maxpool_split_kernel<true, false><<<blocks, threads, 0, s>>>(xh, xl, yh, yl, B, H, W, C / 8);
+        if (lo) maxpool_split_kernel<true, true><<<blocks, threads, 0, s>>>(xh, xl, yh, yl, B, H, W, C / 8, count);
+        else maxpool_split_kernel<true, false><<<blocks, threads, 0, s>>>(xh, xl, yh, yl, B, H, W, C / 8, count);
     } else {
-        if (lo) maxpool_split_kernel<false, true><<<blocks, threads, 0, s>>>(xh, xl, yh, yl, B, H, W, C / 8);
-        else maxpool_split_kernel<false, false><<<blocks, threads, 0, s>>>(xh, xl, yh, yl, B, H, W, C / 8);
+        if (lo) maxpool_split_kernel<false, true><<<blocks, threads, 0, s>>>(xh, xl, yh, yl, B, H, W, C / 8, count);
+        else maxpool_split_kernel<false, false><<<blocks, threads, 0, s>>>(xh, xl, yh, yl, B, H, W, C / 8, count);
     }
     H3D_CHECK_LAUNCH();
     return H3D_OK;
@@ -375,8 +382,9 @@ int64_t seg_scratch_bytes(int B, int H, int W) {
 template <bool UPS>
 __global__ void __launch_bounds__(256)
 seg_prob_kernel(const float2* __restrict__ logits, float2* __restrict__ up, int LH, int LW, float hscale, float wscale, int H, int W,
-                int Ww, unsigned long long* __restrict__ key, uint32_t* __restrict__ det) {
+                int Ww, unsigned long long* __restrict__ key, uint32_t* __restrict__ det, const int* __restrict__ count) {
     const int b = blockIdx.y;
+    if (count && b >= *count) return;   // counted batch: the blocks of images past the count exit together
     const int lane = threadIdx.x & 31;
     const int warps_per_block = blockDim.x >> 5;
     const int words = H * Ww;
@@ -446,7 +454,8 @@ __host__ __device__ inline size_t grow_smem_bytes(int H, int Ww) {
 __global__ void __launch_bounds__(kGrowThreads, 1)
 mask_grow_kernel(const unsigned long long* __restrict__ key, const uint32_t* __restrict__ det_g, int H, int W, int Ww,
                  int num_passes, uint8_t* __restrict__ hand_mask, int32_t* __restrict__ max_loc, float* __restrict__ center,
-                 float* __restrict__ crop_size, float* __restrict__ scale_crop) {
+                 float* __restrict__ crop_size, float* __restrict__ scale_crop, const int* __restrict__ count) {
+    if (count && (int)blockIdx.x >= *count) return;   // counted batch: one CTA per image, images past the count exit at once
     extern __shared__ uint32_t sm[];
     const int Hp = grow_rows_padded(H);
     uint32_t* det = sm;                                   // [Hp][Ww]
@@ -613,7 +622,7 @@ __host__ __device__ inline size_t grow_cluster_smem_bytes(int H, int Ww) {
 __global__ void __launch_bounds__(kGrowThreads, 1)
 mask_grow_cluster_kernel(const unsigned long long* __restrict__ key, const uint32_t* __restrict__ det_g, int H, int W, int Ww,
                          int num_passes, uint8_t* __restrict__ hand_mask, int32_t* __restrict__ max_loc, float* __restrict__ center,
-                         float* __restrict__ crop_size, float* __restrict__ scale_crop) {
+                         float* __restrict__ crop_size, float* __restrict__ scale_crop, const int* __restrict__ count) {
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
     extern __shared__ uint32_t sm[];
@@ -621,6 +630,7 @@ mask_grow_cluster_kernel(const unsigned long long* __restrict__ key, const uint3
     __shared__ unsigned int s_vote[2];       // rank 0's are the cluster's
     const int cs = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
     const int b = blockIdx.x / cs;
+    if (count && b >= *count) return;        // counted batch: the whole cluster of an image past the count exits, before any barrier
     const int tid = threadIdx.x;
     const int base_rows = H / cs, extra = H - base_rows * cs;
     const int n = base_rows + (rank < extra ? 1 : 0);                      // rows of this band
@@ -773,7 +783,7 @@ mask_grow_cluster_kernel(const unsigned long long* __restrict__ key, const uint3
 
 static int launch_mask_grow_cluster(const unsigned long long* key, const uint32_t* det, int B, int H, int W, int Ww, int num_passes,
                                     uint8_t* hand_mask, int32_t* max_loc, float* center, float* crop_size, float* scale_crop,
-                                    cudaStream_t s) {
+                                    cudaStream_t s, const int* count) {
     const int cs = grow_cluster_size(H);
     const size_t smem = grow_cluster_smem_bytes(H, Ww);
     H3D_REQUIRE(smem <= 227 * 1024, "seg_postprocess: %dx%d needs %zu bytes of shared memory per CTA", H, W, smem);
@@ -798,14 +808,14 @@ static int launch_mask_grow_cluster(const unsigned long long* key, const uint32_
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     H3D_CUDA(cudaLaunchKernelEx(&cfg, mask_grow_cluster_kernel, key, det, H, W, Ww, num_passes, hand_mask, max_loc, center, crop_size,
-                                scale_crop));
+                                scale_crop, count));
     return H3D_OK;
 }
 
 // low != nullptr: fused form for the pipeline - `low` [B,LH,LW,2] is up-sampled to `logits` [B,H,W,2] (written) and classified in one pass
 int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scratch, uint8_t* hand_mask, int32_t* max_loc,
                            float* center, float* crop_size, float* scale_crop, cudaStream_t s, int* n_launch, const float* low, int LH,
-                           int LW) {
+                           int LW, const int* count) {
     H3D_REQUIRE(H > 0 && W > 0 && H <= H3D_PIPELINE_MAX_SIDE && W <= H3D_PIPELINE_MAX_SIDE,
                 "seg_postprocess: H, W must be in [1, %d] (H3D_PIPELINE_MAX_SIDE), got %dx%d", H3D_PIPELINE_MAX_SIDE, H, W);
     const int Ww = seg_words(W);
@@ -817,13 +827,13 @@ int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scrat
     dim3 grid(std::max(1, std::min(ceil_div(words, 8), ceil_div(132 * 8, B))), B);
     if (low && !(LH == H && LW == W))
         seg_prob_kernel<true><<<grid, 256, 0, s>>>((const float2*)low, (float2*)const_cast<float*>(logits), LH, LW, (float)LH / (float)H,
-                                                   (float)LW / (float)W, H, W, Ww, key, det);
+                                                   (float)LW / (float)W, H, W, Ww, key, det, count);
     else
-        seg_prob_kernel<false><<<grid, 256, 0, s>>>((const float2*)(low ? low : logits), nullptr, 0, 0, 0.f, 0.f, H, W, Ww, key, det);
+        seg_prob_kernel<false><<<grid, 256, 0, s>>>((const float2*)(low ? low : logits), nullptr, 0, 0, 0.f, 0.f, H, W, Ww, key, det, count);
     H3D_CHECK_LAUNCH();
     const int num_passes = std::max(H, W) / (21 / 2);   // utils/general.py:256
     if (std::max(H, W) > 512) {   // one CTA's shared memory holds the masks up to 512 x 512; larger images are banded over a cluster
-        const int rc = launch_mask_grow_cluster(key, det, B, H, W, Ww, num_passes, hand_mask, max_loc, center, crop_size, scale_crop, s);
+        const int rc = launch_mask_grow_cluster(key, det, B, H, W, Ww, num_passes, hand_mask, max_loc, center, crop_size, scale_crop, s, count);
         if (rc == H3D_OK && n_launch) *n_launch += 2;
         return rc;
     }
@@ -836,7 +846,7 @@ int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scrat
         attr_set[dev & 63] = true;
     }
     mask_grow_kernel<<<B, kGrowThreads, smem, s>>>(key, det, H, W, Ww, num_passes, hand_mask, max_loc, center, crop_size,
-                                                   scale_crop);
+                                                   scale_crop, count);
     H3D_CHECK_LAUNCH();
     if (n_launch) *n_launch += 2;
     return H3D_OK;

@@ -70,7 +70,72 @@ __global__ void __launch_bounds__(kTrackThreads) track_update_kernel(const float
     reinterpret_cast<int32_t*>(state)[(int64_t)H3D_TRACK_LOST * B + b] = lost ? 1 : 0;
 }
 
+// Slot selection of a slots step (h3d_track_step_slots): one CTA walks the B slots in chunks of kSelThreads; a chunk's positions are an
+// exclusive prefix sum of its flags (warp ballots, then the warp totals), added to the running count of the chunks before it.  So the
+// selected slots land in ascending order and no atomic decides a position.  Reads the lost flags the previous step's update wrote.
+constexpr int kSelThreads = 256;
+
+__global__ void __launch_bounds__(kSelThreads) track_select_kernel(const int32_t* __restrict__ lost, const int32_t* __restrict__ force,
+                                                                   int B, int32_t* __restrict__ sel, int32_t* __restrict__ detected) {
+    __shared__ int s_warp[kSelThreads / 32];
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    int32_t* slots = sel + 1;
+    int32_t* pos = sel + 1 + B;
+    int base = 0;
+    for (int c0 = 0; c0 < B; c0 += kSelThreads) {
+        const int b = c0 + t;
+        const bool on = b < B && (lost[b] != 0 || (force && force[b] != 0));
+        const unsigned m = __ballot_sync(0xFFFFFFFFu, on);
+        if (lane == 0) s_warp[warp] = __popc(m);
+        __syncthreads();
+        int before = base, total = base;
+        for (int w = 0; w < kSelThreads / 32; ++w) {
+            if (w < warp) before += s_warp[w];
+            total += s_warp[w];
+        }
+        const int p = before + __popc(m & ((1u << lane) - 1u));
+        if (b < B) {
+            pos[b] = on ? p : -1;
+            if (on) slots[p] = b;
+            if (detected) detected[b] = on ? 1 : 0;
+        }
+        base = total;
+        __syncthreads();   // s_warp is rewritten by the next chunk
+    }
+    if (t == 0) sel[0] = base;
+}
+
+// The crop of a slots step: a selected slot takes the one its mask produced (compact index pos[b]), every other slot its state's crop.
+__global__ void track_merge_kernel(const float* __restrict__ state, const int32_t* __restrict__ sel, const float* __restrict__ cen_c,
+                                   const float* __restrict__ scl_c, int B, float* __restrict__ center, float* __restrict__ scale) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const int p = sel[1 + B + b];
+    const float* st_center = state + (int64_t)H3D_TRACK_CENTER * B;
+    if (p >= 0) {
+        center[2 * b] = cen_c[2 * p]; center[2 * b + 1] = cen_c[2 * p + 1];
+        scale[b] = scl_c[p];
+    } else {
+        center[2 * b] = st_center[2 * b]; center[2 * b + 1] = st_center[2 * b + 1];
+        scale[b] = state[(int64_t)H3D_TRACK_SCALE * B + b];
+    }
+}
+
 }  // namespace
+
+int launch_track_select(const void* state, const int32_t* force, int B, int32_t* sel, int32_t* detected, cudaStream_t s) {
+    const int32_t* lost = reinterpret_cast<const int32_t*>(state) + (int64_t)H3D_TRACK_LOST * B;
+    track_select_kernel<<<1, kSelThreads, 0, s>>>(lost, force, B, sel, detected);
+    H3D_CHECK_LAUNCH();
+    return H3D_OK;
+}
+
+int launch_track_merge(const void* state, const int32_t* sel, const float* cen_c, const float* scl_c, int B, float* center, float* scale,
+                       cudaStream_t s) {
+    track_merge_kernel<<<ceil_div(B, 128), 128, 0, s>>>((const float*)state, sel, cen_c, scl_c, B, center, scale);
+    H3D_CHECK_LAUNCH();
+    return H3D_OK;
+}
 
 int launch_track_update(const float* map32, const int32_t* uv, const float* center, const float* scale, int B, float margin,
                         float min_score, void* state, cudaStream_t s) {

@@ -95,6 +95,14 @@ def frame_coords(keypoints_hw, frame_hw, size=NETWORK_SIZE):
     return torch.stack([rows, cols], -1)
 
 
+def redetect_schedule(B, every):
+    """The staggered re-detection of FrameRunner(track=True, detect="slots", redetect_every=every): int32 [every, B], row p = the force
+    mask of the steps t with t % every == p; slot b is forced where (t + b) % every == 0, so each step forces about B / every slots."""
+    t = np.arange(int(every))[:, None]
+    b = np.arange(int(B))[None, :]
+    return ((t + b) % int(every) == 0).astype(np.int32)
+
+
 class FrameRunner:
     """Serves a stream of equal-size uint8 RGB frames through run.py's resize and ColorHandPose3DNetwork.inference.
 
@@ -122,16 +130,30 @@ class FrameRunner:
     t % redetect_every == 0, or when any slot was lost at step t - 2 (min_score: the lowest trusted score; None = no score test).
     The choice is made on the host from step t - 2's lost flags: stream() has them already; submit() waits for step t - 2 to finish.
     So a slot lost at step t is re-acquired by a detect step at t + 2 at the latest.  The results gain detected (bool, the step's
-    kind), track_score [B] float32 and track_lost [B] bool."""
+    kind), track_score [B] float32 and track_lost [B] bool.
+
+    track=True with detect="slots" re-detects per slot instead (Context.track_step_slots, DESIGN.md section 4.15): one graph per input
+    buffer runs HandSegNet on the slots the previous step lost, chosen on the device, and tracks the others.  The host reads nothing
+    back and submit() never waits on an earlier step, so a slot lost at step t is re-detected at step t + 1.  redetect_every = N forces
+    slot b at the steps t with (t + b) % N == 0, so that the re-detections are spread over the N steps; the step's force mask is copied
+    from a device table of the N phases before the replay.  The results gain track_detected [B] bool (the slots the step re-detected),
+    track_score and track_lost; detected is not given.  detect="batch" (the default) is the policy above; detect="slots" without
+    track=True is refused."""
 
     RESULT_KEYS = ("keypoints_frame", "keypoints_uv", "keypoint_coord3d", "center", "scale_crop")
     TRACK_KEYS = ("track_score", "track_lost")
+    SLOTS_KEYS = ("track_score", "track_lost", "track_detected")
 
     def __init__(self, ctx, batch, frame_hw, size=NETWORK_SIZE, outputs="keypoints", track=False, redetect_every=None, min_score=None,
-                 track_margin=1.5):
+                 track_margin=1.5, detect="batch"):
         self.ctx, self.B = ctx, int(batch)
         self.frame_hw, self.size = (int(frame_hw[0]), int(frame_hw[1])), (int(size[0]), int(size[1]))
         self.track = bool(track)
+        if detect not in ("batch", "slots"):
+            raise ValueError("FrameRunner: detect must be 'batch' or 'slots', got %r" % (detect,))
+        if detect == "slots" and not self.track:
+            raise ValueError("FrameRunner: detect='slots' re-detects tracked slots; it needs track=True")
+        self.slots = detect == "slots"
         if redetect_every is not None and int(redetect_every) < 1:
             raise ValueError("FrameRunner: redetect_every must be None or >= 1, got %r" % (redetect_every,))
         self.redetect_every = None if redetect_every is None else int(redetect_every)
@@ -155,6 +177,10 @@ class FrameRunner:
         self._i = 0
         ctx.ensure_workspace(self.B, h, w)
 
+        self._force, self._force_table = None, None
+        if self.slots and self.redetect_every is not None:
+            self._force_table = torch.from_numpy(redetect_schedule(self.B, self.redetect_every)).to(dev)   # [N, B]: phase t % N
+            self._force = [torch.zeros(self.B, dtype=torch.int32, device=dev) for _ in range(2)]
         if self.track:
             self._state = runtime.TrackState(self.B, dev)
             self._lost_host = [torch.zeros(self.B, dtype=torch.bool).pin_memory() for _ in range(2)]   # step t's lost flags
@@ -163,7 +189,12 @@ class FrameRunner:
 
         def body(k, detect=True):
             ctx.resize_frames(self._frames[k], h, w, normalize=True, out=self._image[k])
-            if self.track:
+            if self.slots:
+                r = ctx.track_step_slots(self._image[k], self._hs[k], self._state, None if self._force is None else self._force[k],
+                                         margin=self.track_margin, min_score=self.min_score, outputs=outputs)
+                r["track_score"] = self._state.score.clone()
+                r["track_lost"] = self._state.lost != 0
+            elif self.track:
                 r = ctx.track_step(self._image[k], self._hs[k], self._state, detect, margin=self.track_margin, min_score=self.min_score,
                                    outputs=outputs)
                 r["track_score"] = self._state.score.clone()
@@ -173,7 +204,7 @@ class FrameRunner:
             r["keypoints_frame"] = frame_coords(trafo_coords(r["keypoints_uv"], r["center"], r["scale_crop"], 256), self.frame_hw, self.size)
             return r
 
-        kinds = (True, False) if self.track else (True,)
+        kinds = (True, False) if self.track and not self.slots else (True,)
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):       # warm-up outside capture: builds the resize and stage plans, packs weights
@@ -217,7 +248,7 @@ class FrameRunner:
         """Enqueues one batch; returns its device result tensors (see the class notes), and in track mode also detected (bool)."""
         t = self._i
         k = t & 1
-        detect = self._detect_now(t) if self.track else True
+        detect = self._detect_now(t) if self.track and not self.slots else True
         self._i += 1
         cur = torch.cuda.current_stream(self.ctx.device)
         cur.wait_event(self._d2h_done[k])           # stream() may still be reading this buffer's previous results
@@ -247,10 +278,14 @@ class FrameRunner:
                 self._uploaded[k].record(self._copy)
             cur.wait_event(self._uploaded[k])
         kind = 0 if detect else 1
+        if self._force_table is not None:           # this step's phase of the staggered schedule (device to device, no host wait)
+            self._force[k].copy_(self._force_table[t % self.redetect_every])
         self._graphs[k][kind].replay()
         self._consumed[k].record(cur)
         res = {n: self._results[k][kind][n] for n in self.RESULT_KEYS}
-        if self.track:
+        if self.slots:
+            res.update({n: self._results[k][kind][n] for n in self.SLOTS_KEYS})
+        elif self.track:
             res.update({n: self._results[k][kind][n] for n in self.TRACK_KEYS})
             self._lost_host[k].copy_(res["track_lost"], non_blocking=True)   # read by step t + 2's choice
             self._lost_ready[k].record(cur)
@@ -282,6 +317,6 @@ class FrameRunner:
     def _collect(self, k):
         self._d2h_done[k].synchronize()             # the read-back the caller asked for
         out = {n: t.numpy().copy() for n, t in self._host[k].items()}
-        if self.track:
+        if self.track and not self.slots:
             out["detected"] = self._detected[k]
         return out

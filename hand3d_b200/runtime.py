@@ -288,6 +288,45 @@ class Context:
             _ptr(r["keypoint_coord3d"]), _ptr(r["keypoints_uv"]), _stream()), "h3d_track_step")
         return r
 
+    def track_step_slots(self, image, hand_side, state, force=None, margin=1.5, min_score=None, outputs="all", with_pose3d=True):
+        """A track step that re-detects only the slots that need it (h3d_track_step_slots, DESIGN.md section 4.15): slot b runs
+        HandSegNet and the mask post-processing when state.lost[b] (from the previous step) or force[b] (optional CUDA int32 or bool [B])
+        is set, and is cropped from the state otherwise.  The choice is made on the device: nothing is read back.  Returns track_step's
+        keys plus track_detected [B] bool (the slots this step re-detected).  Enqueue-only after the first call for a shape: a call on
+        fixed tensors can be captured into a CUDA graph."""
+        image = _chk_f32(image, "image", 4)
+        B, H, W, _ = image.shape
+        dev = image.device
+        if with_pose3d:
+            hand_side = _chk_f32(hand_side, "hand_side", 2)
+        if not isinstance(state, TrackState) or state.B != B or state.buffer.device != dev:
+            raise ValueError("state must be a TrackState of batch %d on %s" % (B, dev))
+        if force is not None:
+            if not isinstance(force, torch.Tensor) or not force.is_cuda or force.device != dev or force.numel() != B:
+                raise ValueError("force must be a CUDA tensor of %d elements on %s" % (B, dev))
+            if force.dtype != torch.int32:
+                force = force.to(torch.int32)
+            force = force.contiguous()
+        self.ensure_workspace(B, H, W)
+        f32 = dict(dtype=torch.float32, device=dev)
+        big = outputs == "all"
+        r = {
+            "image_crop": torch.empty((B, 256, 256, 3), **f32) if big else None,
+            "scale_crop": torch.empty((B, 1), **f32),
+            "center": torch.empty((B, 2), **f32),
+            "keypoints_scoremap": torch.empty((B, 256, 256, 21), **f32) if big else None,
+            "keypoint_coord3d": torch.empty((B, 21, 3), **f32) if with_pose3d else None,
+            "keypoints_uv": torch.empty((B, 21, 2), dtype=torch.int32, device=dev),
+        }
+        detected = torch.empty(B, dtype=torch.int32, device=dev)
+        _lib.check(self.lib.h3d_track_step_slots(
+            self.h, _ptr(image), _ptr(hand_side if with_pose3d else None), B, H, W, int(bool(with_pose3d)),
+            float(margin), float("nan") if min_score is None else float(min_score), _ptr(state.buffer), _ptr(force), _ptr(detected),
+            _ptr(r["image_crop"]), _ptr(r["scale_crop"]), _ptr(r["center"]), _ptr(r["keypoints_scoremap"]),
+            _ptr(r["keypoint_coord3d"]), _ptr(r["keypoints_uv"]), _stream()), "h3d_track_step_slots")
+        r["track_detected"] = detected != 0
+        return r
+
     def track_update(self, scoremap32, keypoints_uv, center, scale_crop, state, margin=1.5, min_score=None):
         """track_step's update alone (h3d_track_update): scoremap32 [B,32,32,21], keypoints_uv [B,21,2] int32, center [B,2] and
         scale_crop [B] or [B,1] of the crop the key-points were found in -> `state` (a TrackState of batch B)."""

@@ -185,6 +185,23 @@ H3D_API int64_t h3d_track_state_bytes(int B);
 H3D_API int h3d_track_step(h3d_ctx* ctx, const float* image, const float* hand_side, int B, int H, int W, int with_pose3d, int detect,
                            float margin, float min_score, void* state, float* image_crop, float* scale_crop, float* center,
                            float* keypoints_scoremap, float* keypoint_coord3d, int32_t* keypoints_uv, void* stream);
+/* A track step that re-detects only the slots that need it.  In stream order:
+ *   1. select: slot b is selected when the state's lost[b] != 0 (written by the previous step's update) or force[b] != 0 (force: optional
+ *      device int32 [B], NULL = none).  A fresh state (lost = 1 everywhere) selects every slot.  The count and the selected slots, in
+ *      ascending order, live in context-owned device memory, not in the workspace;
+ *   2. HandSegNet and the mask post-processing on the selected slots only: a device-counted batch whose first layer reads slot slots[i]
+ *      of `image` in place, every kernel bounded by the count on the device.  A slot's result has the same bits as in a detect step;
+ *   3. merge: a selected slot takes the crop its mask gives, every other slot its state's crop;
+ *   4. the crop, PoseNet2D, key-points and lifting on every slot, then the update, as in h3d_track_step.
+ * So every output of a selected slot equals h3d_track_step with detect != 0, and of any other slot detect == 0, bit for bit.
+ * detected (optional, device int32 [B]) receives 1 for the selected slots, 0 for the others.  The host never reads the selection, so a
+ * slot lost at step t is re-detected at step t + 1.  With no slot selected the counted kernels exit at once.  The first call for a
+ * (B, H, W) builds the counted plan (outside any graph capture); after that the entry only enqueues, allocates nothing and is
+ * capturable.  Argument rules as h3d_track_step's; a refused call enqueues nothing. */
+H3D_API int h3d_track_step_slots(h3d_ctx* ctx, const float* image, const float* hand_side, int B, int H, int W, int with_pose3d,
+                                 float margin, float min_score, void* state, const int32_t* force, int32_t* detected, float* image_crop,
+                                 float* scale_crop, float* center, float* keypoints_scoremap, float* keypoint_coord3d,
+                                 int32_t* keypoints_uv, void* stream);
 /* The update alone (the operator form of h3d_track_step's last kernel): scoremap32 [B,32,32,21] (the last PoseNet2D stage),
  * keypoints_uv [B,21,2] int32, center [B,2] and scale_crop [B] of the crop they were found in -> state.  Same argument rules. */
 H3D_API int h3d_track_update(h3d_ctx* ctx, const float* scoremap32, const int32_t* keypoints_uv, const float* center,
