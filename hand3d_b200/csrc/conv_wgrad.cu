@@ -35,8 +35,12 @@ constexpr int kWgProducerRegs = 40, kWgConsumerRegs = 232;   // as conv_tc_kerne
 
 // stage = [dy' hi | dy' lo | x hi (BN / 64 boxes) | x lo (BN / 64 boxes)]; PASSES 1 drops the lo planes
 __host__ __device__ constexpr int wg_stage_bytes(int BN, int PASSES) { return (PASSES == 3 ? 2 : 1) * (1 + BN / 64) * WG_BOX_BYTES; }
+// An even count, at most 8.  Warpgroup cw consumes the K blocks kb = cw, cw + 2, ... from stage kb % STAGES, so with an even count
+// each stage has one consumer, which has taken round r - 1 of its full barrier before it waits for round r.  With an odd count (7 at
+// BN = 64 in 3 passes) the two warpgroups alternate on a stage: one could wait for round r while the other's round r - 1 had not
+// landed, and the parity wait would pass at once on the stage's old contents.
 __host__ __device__ constexpr int wg_num_stages(int BN, int PASSES) {
-    return kWgSmemBudget / wg_stage_bytes(BN, PASSES) > 8 ? 8 : kWgSmemBudget / wg_stage_bytes(BN, PASSES);
+    return (kWgSmemBudget / wg_stage_bytes(BN, PASSES) > 8 ? 8 : kWgSmemBudget / wg_stage_bytes(BN, PASSES)) & ~1;
 }
 __host__ __device__ constexpr int wg_smem_bytes(int BN, int PASSES) { return wg_num_stages(BN, PASSES) * wg_stage_bytes(BN, PASSES) + 2048; }
 
@@ -85,6 +89,7 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid
     constexpr int X_PLANE = NBOX * WG_BOX_BYTES;
     constexpr int NR = BN / 2;
     static_assert(STAGES >= 4, "each consumer warpgroup holds two stages while the producer refills");
+    static_assert(STAGES % 2 == 0, "one consumer warpgroup per stage (wg_num_stages)");
     static_assert(STAGES * STAGE_BYTES >= 64 * BN * 4, "the epilogue reduces the two fragments through the ring");
     static_assert(wg_smem_bytes(BN, PASSES) <= 227 * 1024, "conv_wgrad_tc_kernel: shared memory budget");
 

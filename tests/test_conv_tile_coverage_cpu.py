@@ -1,15 +1,17 @@
 """Which tiles the shape tables of tests/test_gpu_conv_tiles.py reach, asked from the library's own choosers (h3d_conv2d_tc_geometry,
 h3d_conv2d_wgrad_geometry: host only, no device needed).  If a chooser changes and a candidate drops out of a table, or a shape stops
-being ragged where it claims to be, this fails without a GPU."""
+being ragged where it claims to be, this fails without a GPU.  The same holds for the training geometries of
+tests/test_gpu_conv_backward.py (TRAIN_CASES)."""
 import os
 import sys
 
 import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import test_gpu_conv_backward as Tb  # noqa: E402
 import test_gpu_conv_tiles as Tt  # noqa: E402
 from test_gpu_conv_layer_planes import POOL_LEGAL, TILE_SHAPES  # noqa: E402
-from hand3d_b200 import _lib, runtime  # noqa: E402
+from hand3d_b200 import _lib, arch, runtime  # noqa: E402
 
 # the candidate lists of choose_tile (conv_wgmma.cu) and wgrad_geometry (conv_wgrad.cu), TW x TH x TB
 FWD_TILES = [(16, 8, 1), (8, 16, 1), (32, 4, 1), (4, 32, 1), (64, 2, 1), (128, 1, 1), (8, 8, 2), (16, 4, 2), (4, 16, 2), (8, 4, 4),
@@ -175,3 +177,43 @@ def test_tables_hold_no_duplicates_and_stay_small(table):
     assert len(set(shapes)) == len(shapes)
     for B, H, W, Cin, Cout, k, s, _ in shapes:
         assert 2.0 * B * H * W * k * k * Cin * Cout < 2.5e9, "keep the fp64 reference of %s quick" % ((B, H, W, Cin, Cout, k),)
+
+
+def _training_layers(B=8, S=256):
+    """{scope/layer: (B, H, W, Cin, Cout, k, stride, leaky)} of every convolution of the HandSegNet and PoseNet2D training graphs at
+    B x S x S, from the variables' weight shapes and the number of pools before each layer."""
+    shapes = arch.variable_shapes()
+    out = {}
+    for scope, pool_after in (("HandSegNet", arch.HANDSEGNET_POOL_AFTER), ("PoseNet2D", arch.POSENET2D_POOL_AFTER)):
+        pools = 0
+        for name, _, stride, _, _, leaky in arch.NETS[scope]:
+            k, _, cin, cout = shapes["%s/%s/weights" % (scope, name)]
+            out["%s/%s" % (scope, name)] = (B, S >> pools, S >> pools, cin, cout, k, stride, leaky)
+            pools += name in pool_after
+    return out
+
+
+def _pixel_blocks_per_cta(shape):
+    tile, _, _, splits = wgrad_geometry(shape)
+    B, H, W = shape[:3]
+    return _cd(_cd(W, tile[0]) * _cd(H, tile[1]) * _cd(B, tile[2]), splits)
+
+
+def test_training_cases_hold_every_training_layer_geometry():
+    layers = _training_layers()
+    assert len(layers) == 16 + 31
+    missing = {n: s for n, s in layers.items() if s not in Tb.TRAIN_CASES}
+    assert not missing, "TRAIN_CASES leaves out %s" % missing
+    assert set(Tb.TRAIN_CASES) == set(layers.values()) and len(Tb.TRAIN_CASES) == 19
+    # and so every weight-gradient launch of the two graphs (tile, N tile, tiles, splits) runs in a per-layer GPU test
+    assert {wgrad_geometry(s) for s in layers.values()} == {wgrad_geometry(s) for s in Tb.TRAIN_CASES}
+
+
+def test_training_cases_reach_the_longest_weight_gradient_reduction():
+    """conv1_x at 256 x 256: 8192 pixel blocks in 44 splits, 187 per CTA (11 fp32 folds per warpgroup in bf16x3), against at most 47
+    in the other per-layer cases."""
+    layers = _training_layers()
+    longest = max(_pixel_blocks_per_cta(s) for s in layers.values())
+    assert longest == max(_pixel_blocks_per_cta(s) for s in Tb.TRAIN_CASES)
+    assert runtime.conv2d_wgrad_geometry(8, 256, 256, 3, 64, 64) == (8, 8, 1, 64, 9, 44) and longest == 187
+    assert longest > max(_pixel_blocks_per_cta(s) for s in Tb.CASES)

@@ -9,7 +9,9 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from hand3d_b200 import arch
 from oracle import tf1_grads as G
+from oracle import tf1_ops
 
 pytestmark = pytest.mark.gpu
 f32 = np.float32
@@ -30,6 +32,26 @@ CASES = [  # B, H, W, Cin, Cout, k, stride: the forward's operator cases (stride
 ]
 
 
+def training_cases(B=8, S=256):
+    """Every distinct layer geometry of the HandSegNet and PoseNet2D training graphs at B x S x S (training_handsegnet.py's
+    random_crop_size, training_posenet.py's crop_size): (B, H, W, Cin, Cout, k, stride, leaky), the map halved after each
+    *_POOL_AFTER layer.  Cin = 3 is conv1_1 (no dx), the linear 1x1 heads have Cout = 2 and 21."""
+    out = []
+    for layers, pool_after in ((arch.HANDSEGNET, arch.HANDSEGNET_POOL_AFTER), (arch.POSENET2D, arch.POSENET2D_POOL_AFTER)):
+        s = S
+        for name, k, stride, cin, cout, leaky in layers:
+            case = (B, s, s, cin, cout, k, stride, leaky)
+            if case not in out:
+                out.append(case)
+            if name in pool_after:
+                s //= 2
+    return out
+
+
+# B = 8 at 256 x 256: conv1_x run the longest weight-gradient splits any network layer runs (about 187 pixel blocks per CTA)
+TRAIN_CASES = training_cases()
+
+
 @pytest.fixture(scope="module")
 def ctx():
     from hand3d_b200 import runtime
@@ -41,7 +63,7 @@ def _err(g, ref):
 
 
 def _problem(case, seed=21):
-    B, H, W, Cin, Cout, k, s = case
+    B, H, W, Cin, Cout, k, s = case[:7]
     rng = np.random.default_rng(seed)
     x = rng.normal(size=(B, H, W, Cin)).astype(f32)
     w = (rng.normal(size=(k, k, Cin, Cout)) / np.sqrt(k * k * Cin)).astype(f32)
@@ -55,22 +77,45 @@ def _cu(a):
 
 
 @pytest.mark.parametrize("prec", ["bf16x3", "bf16"])
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", CASES + TRAIN_CASES)
 def test_conv_backward_vs_oracle(ctx, case, prec):
-    B, H, W, Cin, Cout, k, s = case
+    B, H, W, Cin, Cout, k, s = case[:7]
+    leaky = case[7] if len(case) > 7 else True
     x, w, b, dy = _problem(case)
     xg, wg, bg, dyg = _cu(x), _cu(w), _cu(b), _cu(dy)
-    y = ctx.conv2d_tc_dev(xg, wg, bg, stride=s, leaky=True, precision=prec)
+    y = ctx.conv2d_tc_dev(xg, wg, bg, stride=s, leaky=leaky, precision=prec)
     need_dx = Cin != 3
-    dx, dw, db = ctx.conv2d_tc_backward(xg, y, dyg, wg, stride=s, leaky=True, precision=prec, need_dx=need_dx)
-    rdx, rdw, rdb = G.conv_grads(x, w, b, dy, s, leaky=True, pre=y.cpu().numpy())
+    dx, dw, db = ctx.conv2d_tc_backward(xg, y, dyg, wg, stride=s, leaky=leaky, precision=prec, need_dx=need_dx)
+    rdx, rdw, rdb = G.conv_grads(x, w, b, dy, s, leaky=leaky, pre=y.cpu().numpy())
     errs = {"dw": _err(dw.cpu().numpy(), rdw), "db": _err(db.cpu().numpy(), rdb)}
     if need_dx:
         errs["dx"] = _err(dx.cpu().numpy(), rdx)
     else:
         assert dx is None
+    print("%s %s normwise errors: %s" % (case, prec, ", ".join("%s %.2e" % kv for kv in sorted(errs.items()))))
     for name, e in errs.items():
         assert e < TOL[prec][name], "%s normwise error %.3e (bound %.1e)" % (name, e, TOL[prec][name])
+
+
+@pytest.mark.parametrize("prec", ["bf16x3", "bf16"])
+@pytest.mark.parametrize("layer", [("HandSegNet", "conv1_2"), ("HandSegNet", "conv4_2"), ("PoseNet2D", "conv6_1")])
+def test_backward_is_power_of_two_equivariant(ctx, layer, prec):
+    """dy 2^e gives dx 2^e, dW 2^e, db 2^e bit for bit at e = -24 and +24: the split planes of dy' lose no bits at either end of
+    the range (real gradients are 1e-7 and smaller; the score-map loss gradient carries 1 / (H W) = 2^-16 at 256 x 256)."""
+    scope, name = layer
+    _, k, s, cin, cout, leaky = next(l for l in arch.NETS[scope] if l[0] == name)
+    case = next(c for c in TRAIN_CASES if c[3:8] == (cin, cout, k, s, leaky))
+    x, w, b, dy = _problem(case, seed=22)
+    xg, wg, bg = _cu(x), _cu(w), _cu(b)
+    y = ctx.conv2d_tc_dev(xg, wg, bg, stride=s, leaky=leaky, precision=prec)
+    base = ctx.conv2d_tc_backward(xg, y, _cu(dy), wg, stride=s, leaky=leaky, precision=prec)
+    assert all(torch.isfinite(g).all() and g.abs().max() > 0 for g in base)
+    for e in (-24, 24):
+        scaled = ctx.conv2d_tc_backward(xg, y, _cu(np.ldexp(dy, e)), wg, stride=s, leaky=leaky, precision=prec)
+        for what, g, g0 in zip(("dx", "dW", "db"), scaled, base):
+            want = g0 * 2.0 ** e                                      # exact: no element leaves the normal range
+            assert torch.equal(g, want), "%s at dy 2^%d: %d elements differ from 2^%d times the unscaled result" % (
+                what, e, int((g != want).sum()), e)
 
 
 def test_weight_gradient_canary_one_hot_dy(ctx):
@@ -119,6 +164,22 @@ def test_backward_is_bitwise_reproducible(ctx):
     c = ctx.conv2d_tc_backward(xg, y, dyg, wg, leaky=True)
     for u, v in zip(a, c):
         assert torch.equal(u, v)
+
+
+@pytest.mark.parametrize("case", [c for c in TRAIN_CASES if c[3] <= 64])
+def test_weight_gradient_reproducible_at_training_shapes(ctx, case):
+    """conv1_1, conv1_2 and conv2_1 at B = 8, 256 x 256 (Cin_pad = 64: the BN = 64 weight-gradient kernel, whose two consumer
+    warpgroups run the longest reductions of the networks): 40 bf16x3 weight gradients of the same operands are bit-identical.  This
+    kernel once ran an odd ring of 7 stages, so its two warpgroups shared stages; rarely, one read a stage before that stage's K
+    block had landed, and one tap tile changed (see wg_num_stages).  That race was rare enough that this check can pass without
+    catching it.  What rules it out is the even ring that wg_num_stages enforces."""
+    x, w, b, dy = _problem(case, seed=25)
+    xg, wg, bg, dyg = _cu(x), _cu(w), _cu(b), _cu(dy)
+    y = ctx.conv2d_tc_dev(xg, wg, bg, leaky=True)
+    first = ctx.conv2d_tc_backward(xg, y, dyg, wg, leaky=True, need_dx=False, need_db=False)[1]
+    for i in range(40):
+        dw = ctx.conv2d_tc_backward(xg, y, dyg, wg, leaky=True, need_dx=False, need_db=False)[1]
+        assert torch.equal(dw, first), "run %d: %d of %d weight-gradient elements differ" % (i + 1, int((dw != first).sum()), dw.numel())
 
 
 @pytest.mark.parametrize("stride", [1, 2])
@@ -191,6 +252,31 @@ def test_max_pool_backward_vs_oracle(ctx):
     dy = rng.normal(size=(2, 5, 6, 24)).astype(f32)
     dx = ctx.max_pool_backward(_cu(x), _cu(dy)).cpu().numpy()
     np.testing.assert_array_equal(dx, G.max_pool_grad(x, dy).astype(f32))
+
+
+@pytest.mark.parametrize("shape", [(8, 256, 256, 64), (8, 128, 128, 128), (8, 64, 64, 256)])
+def test_max_pool_at_training_shapes_vs_oracle(ctx, shape):
+    """The three pools of both training graphs at B = 8, 256 x 256, on a leaky-ReLU convolution output (about half of it negative and
+    small) with planted ties: forward and backward exact against TF's max-pool and MaxPoolGrad (first maximum of each window)."""
+    B, H, W, C = shape
+    x, w, b, _ = _problem((B, H, W, C, C, 3, 1), seed=23)
+    y = ctx.conv2d_tc_dev(_cu(x), _cu(w), _cu(b), leaky=True).cpu().numpy()
+    rng = np.random.default_rng(24)
+    win = y.reshape(B, H // 2, 2, W // 2, 2, C)                      # a view: the ties are planted in y
+    pick = rng.uniform(size=(B, H // 2, W // 2, C))
+    m = win.max(axis=(2, 4))
+    win[:, :, 1, :, 1][pick < 0.05] = m[pick < 0.05]                  # last entry ties the maximum
+    four = (pick >= 0.05) & (pick < 0.10)
+    for i in (0, 1):
+        for j in (0, 1):
+            win[:, :, i, :, j][four] = m[four]                       # all four entries equal
+    neg = (pick >= 0.10) & (pick < 0.15)
+    win[:, :, 0, :, 1][neg] = win[:, :, 1, :, 0][neg] = -np.abs(m[neg]) * 0.01   # a tie below zero, away from the first entry
+    win[:, :, 0, :, 0][neg] = win[:, :, 1, :, 1][neg] = -np.abs(m[neg]) * 0.02 - 1e-3
+    yg = _cu(y)
+    np.testing.assert_array_equal(ctx.max_pool(yg).cpu().numpy(), tf1_ops.max_pool_2x2(y))
+    dy = rng.normal(size=(B, H // 2, W // 2, C)).astype(f32)
+    np.testing.assert_array_equal(ctx.max_pool_backward(yg, _cu(dy)).cpu().numpy(), G.max_pool_grad(y, dy).astype(f32))
 
 
 # ---------------------------------------------------------------------------------------------- end to end through autograd.py
