@@ -212,6 +212,7 @@ __device__ __forceinline__ void produce_kblock(Ring& r, const CUtensorMap* x_hi,
                                                int a0, int a1, int a2, int a3, int kcol, int n0, int* err_flag) {
     using C = RingCfg<BN, PASSES>;
     mbar_wait(&r.empty[r.stage], r.phase ^ 1, err_flag, 1);
+    H3D_SKEW(SKEW_PRODUCER, r.stage + r.phase * C::STAGES);
     if (elect_one()) {
         uint8_t* st = r.base + r.stage * C::STAGE_BYTES;
         uint64_t* fb = &r.full[r.stage];
@@ -254,6 +255,7 @@ __device__ __forceinline__ void mma_tile(Ring& r, int kblocks, int chunk_kb, flo
         int pend = -1;
         for (int kb = kb0; kb < kb1; ++kb) {
             mbar_wait(&r.full[r.stage], r.phase, err_flag, 3);
+            H3D_SKEW(SKEW_CONSUMER, kb);
             const uint32_t sa = smem_u32(r.base + r.stage * C::STAGE_BYTES);
             const uint32_t a_rows = (uint32_t)wg * 64 * 128;   // this warpgroup's 64 rows of the A tile
             const uint64_t a_hi = desc_sw128(sa + a_rows);
@@ -288,6 +290,7 @@ __device__ __forceinline__ void mma_tile(Ring& r, int kblocks, int chunk_kb, flo
             wgmma_commit();
             fence_regs<NR>(acc);
             fence_regs<NR8>(acc8);
+            H3D_SKEW(SKEW_COMMIT, kb);
             wgmma_wait<1>();
             if (pend >= 0 && lane == 0) mbar_arrive(&r.empty[pend]);
             pend = r.stage;
@@ -325,6 +328,7 @@ __device__ __forceinline__ void store_tile(const TcParams& p, const float* racc,
     pix_of(row, pix, valid);
 #pragma unroll
     for (int rnd = 0; rnd < BN / STG_COLS; ++rnd) {
+        H3D_SKEW(SKEW_EPILOGUE, 2 * rnd);
         named_bar_sync(1, kConsumerThreads);   // the previous round's readers are done with the buffer
 #pragma unroll
         for (int j = 0; j < STG_COLS / 8; ++j) {
@@ -335,6 +339,7 @@ __device__ __forceinline__ void store_tile(const TcParams& p, const float* racc,
             stg[(r0 + 8) * STG_PITCH + c + 1] = racc[4 * jj + 3];
         }
         named_bar_sync(1, kConsumerThreads);
+        H3D_SKEW(SKEW_EPILOGUE, 2 * rnd + 1);
         float f[32];
 #pragma unroll
         for (int q = 0; q < 32; ++q) f[q] = stg[row * STG_PITCH + half * 32 + q];
@@ -380,6 +385,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_consta
     }
     __syncthreads();
     pdl_launch_dependents();
+    H3D_SKEW(SKEW_PDL_TAIL, 0);
     pdl_wait();
     const int nb = counted_images(p), num_tiles = counted_tiles(p, nb);   // the producer and the consumers walk the same tiles
 
@@ -478,6 +484,7 @@ conv_c3_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, cons
             *reinterpret_cast<uint4*>(bsm + sw128_chunk(t, c)) = make_uint4(pk[4 * c], pk[4 * c + 1], pk[4 * c + 2], pk[4 * c + 3]);
     }
     pdl_launch_dependents();
+    H3D_SKEW(SKEW_PDL_TAIL, 0);
     pdl_wait();
     const int num_tiles = COUNTED ? counted_tiles(p, counted_images(p)) : p.num_tiles;   // TB = 1: whole images
 
@@ -531,6 +538,7 @@ conv_c3_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, cons
             mma16<64, FP16>(acc, a_lo + koff, b_hi + koff, 1u);
         }
         wgmma_commit();
+        H3D_SKEW(SKEW_COMMIT, tile);
         wgmma_wait<0>();
         fence_regs<32>(acc);
         auto pix_of = [&](int row, int64_t& pix, bool& valid) {
@@ -572,9 +580,10 @@ struct FcChainParams {
     int* err_flag;
 };
 
-__device__ __forceinline__ void fc_layer_sync() {
+__device__ __forceinline__ void fc_layer_sync(int l) {
     __threadfence();                                        // the layer's outputs: visible at device scope ...
     asm volatile("fence.proxy.async;" ::: "memory");        // ... and to the async proxy (the next layer's TMA loads)
+    H3D_SKEW(SKEW_CLUSTER, l);
     cluster_sync_all();
 }
 
@@ -607,6 +616,7 @@ fc_chain_kernel(const __grid_constant__ FcChainParams P) {
     }
     __syncthreads();
     pdl_launch_dependents();
+    H3D_SKEW(SKEW_PDL_TAIL, 0);
     pdl_wait();
 
     // Every warp of every CTA of the cluster runs the SAME layer loop and reaches fc_layer_sync() exactly once per layer.
@@ -632,11 +642,12 @@ fc_chain_kernel(const __grid_constant__ FcChainParams P) {
                 }, L.p.w_scale);
             }
         }
-        fc_layer_sync();
+        fc_layer_sync(l);
     }
 
     // ---- last cluster to finish: Rodrigues + right-hand flip + rotation of the canonical coordinates (both chains' outputs)
     if (P.num_chains == 2 && rank == 0) {
+        H3D_SKEW(SKEW_TICKET, 0);
         if (threadIdx.x == 0) {
             __threadfence();
             s_last = atomicAdd(P.counter, 1u) == 1u;
@@ -663,6 +674,7 @@ fc_chain_kernel(const __grid_constant__ FcChainParams P) {
             }
         }
     }
+    H3D_SKEW(SKEW_CLUSTER, ch.num_layers);
     cluster_sync_all();          // no CTA of the cluster exits while a peer may still be inside a cluster barrier
 }
 
@@ -797,6 +809,31 @@ TcTuning& tc_tuning() {
     }();
     return t;
 }
+#ifdef H3D_SKEW_BUILD
+// Schedule-skew config (skew.cuh): the host copy and the uploaders of every translation unit with hooks.
+static std::vector<int (*)(const SkewCfg&)>& skew_uploaders() { static std::vector<int (*)(const SkewCfg&)> v; return v; }
+static SkewCfg g_skew_host = {};
+int skew_register(int (*upload)(const SkewCfg&)) { skew_uploaders().push_back(upload); return 0; }
+int skew_set(const char* key, int value) {
+    static const char* const sites[SKEW_SITES] = {"producer", "consumer", "commit", "epilogue", "cluster", "pdl_tail", "ticket"};
+    const std::string k(key);
+    if (k == "skew_reset") g_skew_host = SkewCfg{};
+    else {
+        int s = 0;
+        while (s < SKEW_SITES && k.compare(0, 5 + strlen(sites[s]) + 1, std::string("skew_") + sites[s] + "_") != 0) ++s;
+        const std::string f = s < SKEW_SITES ? k.substr(5 + strlen(sites[s]) + 1) : "";
+        SkewSiteCfg* c = s < SKEW_SITES ? &g_skew_host.site[s] : nullptr;
+        if (c && f == "ns" && value >= 0) c->ns = std::min((unsigned)value, kSkewMaxNs);
+        else if (c && f == "role" && value >= 0 && value <= SKEW_RANK0 + 15) c->role = (unsigned)value;
+        else if (c && f == "period" && value >= 0) c->period = (unsigned)value;
+        else if (c && f == "seed") c->seed = (unsigned)value;
+        else { set_error("h3d_set_tuning: bad skew key '%s' or value %d", key, value); return H3D_EINVAL; }
+    }
+    for (auto up : skew_uploaders()) H3D_CUDA((cudaError_t)up(g_skew_host));
+    return H3D_OK;
+}
+#endif
+
 int tc_set_tuning(const char* key, int value) {
     TcTuning& t = tc_tuning();
     const std::string k(key ? key : "");
@@ -809,6 +846,9 @@ int tc_set_tuning(const char* key, int value) {
     else if (k == "pdl") t.pdl = value;
     else if (k == "fc_chain") t.fc_chain = value;
     else if (k == "no_seg_fusion") t.no_seg_fusion = value;
+#ifdef H3D_SKEW_BUILD
+    else if (k.compare(0, 5, "skew_") == 0) return skew_set(key, value);
+#endif
     else { set_error("h3d_set_tuning: unknown key '%s'", k.c_str()); return H3D_EINVAL; }
     return H3D_OK;
 }

@@ -122,6 +122,7 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid
                 const int pb = pb0 + kb;
                 const int w0 = (pb % p.tiles_w) * p.TW, h0 = (pb / p.tiles_w % p.tiles_h) * p.TH, b0 = pb / (p.tiles_w * p.tiles_h) * p.TB;
                 mbar_wait(&ring.empty[ring.stage], ring.phase ^ 1, p.err_flag, 1);
+                H3D_SKEW(SKEW_PRODUCER, kb);
                 if (elect_one()) {
                     uint8_t* st = ring.base + ring.stage * STAGE_BYTES;
                     uint64_t* fb = &ring.full[ring.stage];
@@ -152,6 +153,7 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid
             for (int kb = kc; kb < kc_end; kb += 2) {
                 const int stage = kb % STAGES;
                 mbar_wait(&ring.full[stage], (uint32_t)(kb / STAGES) & 1u, p.err_flag, 3);
+                H3D_SKEW(SKEW_CONSUMER, kb);
                 const uint32_t sa = smem_u32(ring.base + stage * STAGE_BYTES);
                 const uint64_t a_hi = desc_mn_sw128(sa, WG_BOX_BYTES), a_lo = desc_mn_sw128(sa + WG_BOX_BYTES, WG_BOX_BYTES);
                 const uint64_t b_hi = desc_mn_sw128(sa + X_OFF, WG_BOX_BYTES), b_lo = desc_mn_sw128(sa + X_OFF + X_PLANE, WG_BOX_BYTES);
@@ -168,6 +170,7 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid
                 }
                 wgmma_commit();
                 fence_regs<NR>(acc);
+                H3D_SKEW(SKEW_COMMIT, kb);
                 wgmma_wait<1>();
                 if (pend >= 0 && lane == 0) mbar_arrive(&ring.empty[pend]);
                 pend = stage;
@@ -182,12 +185,15 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid
         // warpgroup 1's in a fixed order; thread t of both warpgroups holds the same fragment elements
         const int t = threadIdx.x & 127;
         float* red = reinterpret_cast<float*>(smem);
+        H3D_SKEW(SKEW_EPILOGUE, 0);
         named_bar_sync(1, 256);
         if (cw == 1) {
 #pragma unroll
             for (int i = 0; i < NR; ++i) red[i * 128 + t] = racc[i];
         }
+        H3D_SKEW(SKEW_EPILOGUE, 1);
         named_bar_sync(1, 256);
+        H3D_SKEW(SKEW_EPILOGUE, 2);
         if (cw == 0) {
             float* out = p.partial + ((int64_t)split * p.num_tiles + tile) * (64 * BN);
             const int m = 16 * (warp & 3) + (lane >> 2);

@@ -8,6 +8,7 @@
 #include <cooperative_groups.h>
 
 #include "common.cuh"
+#include "skew.cuh"
 #include "split_fmt.cuh"
 
 namespace h3d {
@@ -436,6 +437,7 @@ seg_prob_kernel(const float2* __restrict__ logits, float2* __restrict__ up, int 
             const unsigned long long other = __shfl_xor_sync(0xFFFFFFFFu, best, o);
             best = other > best ? other : best;
         }
+        H3D_SKEW(SKEW_TICKET, 0);
         if (threadIdx.x == 0) atomicMax(key + b, best);
     }
 }
@@ -666,6 +668,7 @@ mask_grow_cluster_kernel(const unsigned long long* __restrict__ key, const uint3
     const uint32_t* hor_up = rank > 0 ? cluster.map_shared_rank(hor, rank - 1) : nullptr;
     const uint32_t* hor_dn = rank + 1 < cs ? cluster.map_shared_rank(hor, rank + 1) : nullptr;
     const int halo_up = min(kGrowPadTop, n_up), halo_dn = min(kGrowPadTop, n_dn);
+    H3D_SKEW(SKEW_CLUSTER, 0);
     cluster.sync();   // every CTA's votes, box and seed are initialised before any peer touches them
 
     const int segs = (Ww + kGrowSeg - 1) / kGrowSeg;
@@ -697,8 +700,10 @@ mask_grow_cluster_kernel(const unsigned long long* __restrict__ key, const uint3
             for (int i = 0; i < kGrowSeg; ++i)
                 if (x0 + i < Ww) hor[base + i] = w[i + 1];
         }
+        H3D_SKEW(SKEW_CLUSTER, 3 * pass + 1);
         cluster.sync();   // every band's hor is complete
         if (rank == 0 && tid == 0) s_vote[(pass + 1) & 1] = 0u;
+        H3D_SKEW(SKEW_CLUSTER, 3 * pass + 1);
         // halo: the last rows of the band above go to rows -10 .. -1, the first rows of the band below to rows n .. n + 9 (rows past
         // the image stay zero)
         for (int i = tid; i < (halo_up + halo_dn) * Ww; i += kGrowThreads) {
@@ -729,8 +734,11 @@ mask_grow_cluster_kernel(const unsigned long long* __restrict__ key, const uint3
                 obj[i] = r;
             }
         }
+        H3D_SKEW(SKEW_CLUSTER, 3 * pass + 2);
         if (__syncthreads_or(changed) && tid == 0) atomicOr(vote0 + (pass & 1), 1u);
+        H3D_SKEW(SKEW_CLUSTER, 3 * pass + 2);
         cluster.sync();   // every vote is in
+        H3D_SKEW(SKEW_CLUSTER, 3 * pass + 3);
         unsigned int any = 0u;
         if ((tid & 31) == 0) any = *(volatile unsigned int*)(vote0 + (pass & 1));
         if (!__shfl_sync(0xFFFFFFFFu, any, 0)) break;   // fixed point, seen by every CTA of the cluster
@@ -759,10 +767,12 @@ mask_grow_cluster_kernel(const unsigned long long* __restrict__ key, const uint3
         }
     }
     __syncthreads();
+    H3D_SKEW(SKEW_CLUSTER, 1 << 20);
     if (tid == 0 && rank != 0 && s_box[1] >= 0) {
         atomicMin(box0 + 0, s_box[0]); atomicMax(box0 + 1, s_box[1]);
         atomicMin(box0 + 2, s_box[2]); atomicMax(box0 + 3, s_box[3]);
     }
+    H3D_SKEW(SKEW_CLUSTER, (1 << 20) + 1);
     cluster.sync();   // the last access to a peer's shared memory is above
     if (rank == 0 && tid == 0) {
         float c0, c1, sz;
@@ -959,6 +969,7 @@ __global__ void heatmap_argmax_kernel(const float* __restrict__ sm, int HW, int 
         skey[p_sub * C + c] = best;
     }
     __syncthreads();
+    H3D_SKEW(SKEW_TICKET, 0);
     if (t < C) {
         unsigned long long m = 0ull;
         for (int q = 0; q < P; ++q) { const unsigned long long k = skey[q * C + t]; m = k > m ? k : m; }
@@ -1043,6 +1054,7 @@ __global__ void resize_argmax_kernel(const float* __restrict__ x, float* __restr
         skey[p_sub * C + c] = best;
     }
     __syncthreads();
+    H3D_SKEW(SKEW_TICKET, 0);
     if (t < C) {
         unsigned long long m = 0ull;
         for (int q = 0; q < P; ++q) { const unsigned long long k = skey[q * C + t]; m = k > m ? k : m; }
@@ -1121,6 +1133,7 @@ __global__ void resize_argmax_pow2_kernel(const float* __restrict__ x, float* __
             }
     }
     __syncthreads();
+    H3D_SKEW(SKEW_TICKET, 0);
     if (t < C) {
         unsigned long long m = 0ull;
         for (int q = 0; q < slots; ++q) { const unsigned long long k = skey[t * slots + q]; m = k > m ? k : m; }

@@ -6,6 +6,7 @@
 // bit-reproducible run to run.  Arithmetic that TF evaluates as separate operations uses explicit __f*_rn so that nvcc cannot
 // contract it into FMAs.
 #include "common.cuh"
+#include "skew.cuh"
 
 namespace h3d {
 
@@ -302,6 +303,7 @@ __global__ void __launch_bounds__(kRedThreads) adam_step_kernel(const h3d_adam_t
         }
     }
     __syncthreads();
+    H3D_SKEW(SKEW_TICKET, 0);
     if (t == 0) {
         __threadfence();
         s_last = atomicAdd(&state->ticket, 1u) == gridDim.x - 1;

@@ -4,6 +4,7 @@
 #include <cuda.h>
 
 #include "common.cuh"
+#include "skew.cuh"
 
 namespace h3d {
 
