@@ -1,12 +1,13 @@
 #!/usr/bin/env python
-"""Forward demo in the shape of the reference's run.py (run.py:29-92), without TensorFlow and without plots.
+"""Forward demo in the shape of the reference's run.py (run.py:29-92), without TensorFlow or matplotlib.
 
 The net / util call lines are the reference's; only the placeholder / session lines are replaced by torch CUDA
 tensors.  With no arguments it runs on seeded synthetic 240x320 images and seeded random-init weights (the released
 weight pickles and sample images are not redistributable / not available offline); pass image files and --weights
-<pickles...> to run the real thing.
+<pickles...> to run the real thing.  --save-dir DIR writes run.py's four-panel figure of each image as a PNG (Pillow), drawn on the
+device by hand3d_b200.draw.run_figure.
 
-    python examples/run_demo.py [img.png ...] [--weights w1.pickle w2.pickle]
+    python examples/run_demo.py [img.png ...] [--weights w1.pickle w2.pickle] [--save-dir out]
 """
 import argparse
 import os
@@ -38,7 +39,12 @@ if __name__ == '__main__':
     ap = argparse.ArgumentParser()
     ap.add_argument("images", nargs="*")
     ap.add_argument("--weights", nargs="*", default=None)
+    ap.add_argument("--save-dir", default=None, help="write run.py's figure of each image there as <name>.png")
     args = ap.parse_args()
+    if args.save_dir:
+        from PIL import Image
+        from hand3d_b200.draw import run_figure
+        os.makedirs(args.save_dir, exist_ok=True)
 
     # network input (run.py:39-41): NHWC float32 on the GPU instead of tf.placeholder
     image_tf = torch.empty((1, 240, 320, 3), dtype=torch.float32, device="cuda")
@@ -55,8 +61,14 @@ if __name__ == '__main__':
 
     for name, image_v in load_images(args.images):
         image_tf.copy_(torch.from_numpy(image_v[None]))
-        hand_scoremap_v, image_crop_v, scale_v, center_v, keypoints_scoremap_v, keypoint_coord3d_v = \
-            [t.cpu().numpy() for t in net.inference(image_tf, hand_side_tf, evaluation)]
+        outs = net.inference(image_tf, hand_side_tf, evaluation)
+        hand_scoremap_v, image_crop_v, scale_v, center_v, keypoints_scoremap_v, keypoint_coord3d_v = [t.cpu().numpy() for t in outs]
+        if args.save_dir:     # run.py:76-92, the figure as one uint8 image (the 240x320 image back in bytes: run.py's image_raw)
+            image_raw = torch.from_numpy(np.clip(np.rint((image_v + 0.5) * 255.0), 0, 255).astype(np.uint8)).cuda()
+            result = dict(zip(("hand_scoremap", "image_crop", "scale_crop", "center", "keypoints_scoremap", "keypoint_coord3d"), outs))
+            result["keypoints_uv"] = detect_keypoints(outs[4])
+            fig = run_figure(image_raw, result)["grid"].cpu().numpy()
+            Image.fromarray(fig).save(os.path.join(args.save_dir, os.path.basename(name).replace("#", "_").split(".")[0] + ".png"))
 
         hand_scoremap_v = np.squeeze(hand_scoremap_v)
         keypoints_scoremap_v = np.squeeze(keypoints_scoremap_v)

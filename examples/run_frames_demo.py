@@ -4,6 +4,8 @@
     python examples/run_frames_demo.py                      # seeded synthetic 1080p frames, synthetic weights
     python examples/run_frames_demo.py --video clip.mp4     # decoded with OpenCV (BGR -> RGB)
     python examples/run_frames_demo.py --weights weights/   # the reference's pickled weights
+    python examples/run_frames_demo.py --track --draw-dir out   # also writes the frames of the first batch with the skeleton and
+                                                                # the crop square drawn on the device (PNG, Pillow)
 """
 import argparse
 import os
@@ -52,6 +54,9 @@ def main():
     ap.add_argument("--detect", default="batch", choices=["batch", "slots"],
                     help="with --track: re-detect the whole batch when a slot is lost (batch), or only the lost slots, chosen on the "
                          "device one step after the loss (slots)")
+    ap.add_argument("--draw-dir", default=None, help="draw the skeleton and the crop square into the frames on the device and write "
+                                                     "them there as PNG files")
+    ap.add_argument("--draw-batches", type=int, default=1, help="with --draw-dir: how many batches to write")
     args = ap.parse_args()
 
     from hand3d_b200 import runtime, weights as Wt
@@ -77,7 +82,10 @@ def main():
         batches = synthetic_batches(args.batches, args.batch, hw[0], hw[1], args.seed)
 
     runner = FrameRunner(ctx, args.batch, hw, track=args.track, redetect_every=args.redetect_every, min_score=args.min_score,
-                         detect=args.detect)
+                         detect=args.detect, draw=args.draw_dir is not None)
+    if args.draw_dir:
+        from PIL import Image
+        os.makedirs(args.draw_dir, exist_ok=True)
     t0 = time.perf_counter()
     n = 0
     for i, r in enumerate(runner.stream(batches)):
@@ -88,6 +96,9 @@ def main():
             detected = r["track_detected"][0] if args.detect == "slots" else r["detected"]
             track = " [%s, score %.4g%s]" % ("detect" if detected else "track", r["track_score"][0],
                                              ", lost" if r["track_lost"][0] else "")
+        if args.draw_dir and i < args.draw_batches:
+            for b, frame in enumerate(r["frame_drawn"]):
+                Image.fromarray(frame).save(os.path.join(args.draw_dir, "batch%03d_frame%02d.png" % (i, b)))
         print("batch %d: frame 0 key-points (row, col) in %dx%d pixels: wrist %s, index tip %s%s" % (i, hw[0], hw[1], np.round(kp[0], 1),
                                                                                                  np.round(kp[8], 1), track))
     dt = time.perf_counter() - t0

@@ -102,6 +102,7 @@ SIGNATURES = {
     "h3d_eval_store_bytes": (_i64, [_i, _i, _i]),
     "h3d_eval_feed": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _i, _i, _p]),
     "h3d_eval_stats": (_i, [_p, _p, _i, _i, _i, _p, _i, _p, _p]),
+    "h3d_draw_segments": (_i, [_p, _p, _i, _i, _i, _p, _i, _p, _p, _f, _p]),
 }
 ADAM_STATE_WORDS = 4   # H3D_ADAM_STATE_WORDS
 # training-mode reader augmentation (H3D_AUG_*): flags, and the per-sample parameter layout
@@ -121,6 +122,8 @@ EVAL_FLOAT32, EVAL_FLOAT64 = 0, 1
 EVAL_KEPT, EVAL_DROPPED, EVAL_TICKET, EVAL_COUNT, EVAL_HEADER_WORDS = 0, 1, 2, 8, 72
 EVAL_MAX_KP, EVAL_MAX_DIM, EVAL_MAX_SAMPLES, EVAL_MAX_THRESHOLDS = 64, 4, 1 << 24, 4096
 EVAL_STAT_N, EVAL_STAT_MEAN, EVAL_STAT_MEDIAN, EVAL_STAT_COUNTS = 0, 1, 2, 3
+# drawing (H3D_DRAW_*): the most segments per call and the widest line of h3d_draw_segments
+DRAW_MAX_SEGMENTS, DRAW_MAX_LINEWIDTH = 64, 64
 
 _lib = None
 

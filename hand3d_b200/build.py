@@ -24,14 +24,15 @@ LIB_SKEW = os.path.join(HERE, "libhand3d_b200_skew.so")
 STAMP_SKEW = os.path.join(HERE, ".libhand3d_b200_skew.stamp")
 SKEW_FLAGS = ["-DH3D_SKEW_BUILD"]
 SOURCES = ["api.cu", "elementwise.cu", "reader.cu", "reader_aug.cu", "conv_direct.cu", "conv_wgmma.cu", "conv_wgrad.cu", "train.cu", "train_lift.cu",
-           "frames.cu", "eval.cu", "track.cu"]
+           "frames.cu", "eval.cu", "track.cu", "draw.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--cudart=static", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",
     "-Xptxas", "-v",
 ]
-# per-source additions: frames.cu builds Pillow's resampling coefficients on the host in double, which must not be fused into FMAs
-SOURCE_FLAGS = {"frames.cu": ["-Xcompiler", "-ffp-contract=off"]}
+# per-source additions: frames.cu builds Pillow's resampling coefficients on the host in double, which must not be fused into FMAs;
+# draw.cu's coverage rule is restated in numpy float32, so its device arithmetic must not be contracted either
+SOURCE_FLAGS = {"frames.cu": ["-Xcompiler", "-ffp-contract=off"], "draw.cu": ["-fmad=false"]}
 
 
 def _nvcc():

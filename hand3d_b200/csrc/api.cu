@@ -1934,6 +1934,22 @@ int h3d_resize_frames(h3d_ctx* ctx, const uint8_t* frames, int B, int H, int W, 
     if (!rc) ctx->launches += 1;
     return rc;
 }
+int h3d_draw_segments(h3d_ctx* ctx, uint8_t* images, int B, int H, int W, const float* segments, int S, const float* host_colors,
+                      const int32_t* valid, float linewidth, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(images && segments && host_colors && B > 0, "h3d_draw_segments: bad argument");
+    H3D_REQUIRE(H >= 1 && H <= H3D_FRAME_MAX_SIDE && W >= 1 && W <= H3D_FRAME_MAX_SIDE,
+                "h3d_draw_segments: images must be 1..%d pixels a side, got %dx%d", H3D_FRAME_MAX_SIDE, H, W);
+    H3D_REQUIRE(S >= 1 && S <= H3D_DRAW_MAX_SEGMENTS, "h3d_draw_segments: S must be 1..%d, got %d", H3D_DRAW_MAX_SEGMENTS, S);
+    H3D_REQUIRE(std::isfinite(linewidth) && linewidth > 0.f && linewidth <= (float)H3D_DRAW_MAX_LINEWIDTH,
+                "h3d_draw_segments: linewidth must be finite in (0, %d], got %g", H3D_DRAW_MAX_LINEWIDTH, (double)linewidth);
+    for (int i = 0; i < 3 * S; ++i)
+        H3D_REQUIRE(std::isfinite(host_colors[i]) && host_colors[i] >= 0.f && host_colors[i] <= 255.f,
+                    "h3d_draw_segments: colour %d of segment %d must be finite in 0..255, got %g", i % 3, i / 3, (double)host_colors[i]);
+    int rc = launch_draw_segments(images, B, H, W, segments, S, host_colors, valid, linewidth, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
 int h3d_rhd_reader_items(h3d_ctx* ctx, const float* header, const uint8_t* hand_parts, const uint8_t* visibility, int B, int use_wrist_coord,
                          int hand_crop, int crop_size, float* keypoint_xyz21, float* keypoint_uv21, uint8_t* keypoint_vis21, float* hand_side,
                          float* keypoint_scale, float* keypoint_xyz21_normed, float* crop_center, float* crop_scale, float* cam_mat, void* stream) {

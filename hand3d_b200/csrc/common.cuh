@@ -175,6 +175,11 @@ FramePlan* frame_plan_create(int Hf, int Wf, int h, int w, cudaStream_t s);
 void frame_plan_destroy(FramePlan* p);
 int launch_resize_frames(const FramePlan* p, const uint8_t* frames, int B, int normalize, void* out, cudaStream_t s);
 
+// ---------------------------------------------------------------- kernels (draw.cu): anti-aliased segments into uint8 RGB images
+// (arguments checked by h3d_draw_segments; host_colors [S,3] is copied into the kernel's parameters)
+int launch_draw_segments(uint8_t* images, int B, int H, int W, const float* segments, int S, const float* host_colors,
+                         const int32_t* valid, float linewidth, cudaStream_t s);
+
 // ---------------------------------------------------------------- kernels (eval.cu): EvalUtil's store and measures (arguments checked)
 int launch_eval_feed(void* store, int K, int N, int dtype, const void* gt, const uint8_t* vis, const void* pred, int n, int D,
                      cudaStream_t s);

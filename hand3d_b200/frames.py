@@ -13,6 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib, runtime
+from . import draw as _draw
 from .utils.general import trafo_coords
 
 NETWORK_SIZE = (240, 320)   # run.py:58
@@ -138,14 +139,21 @@ class FrameRunner:
     slot b at the steps t with (t + b) % N == 0, so that the re-detections are spread over the N steps; the step's force mask is copied
     from a device table of the N phases before the replay.  The results gain track_detected [B] bool (the slots the step re-detected),
     track_score and track_lost; detected is not given.  detect="batch" (the default) is the policy above; detect="slots" without
-    track=True is refused."""
+    track=True is refused.
+
+    draw=True ends each captured step by drawing into the step's own input buffer, which the resize has consumed by then (no copy):
+    the crop square in white, then plot_hand's skeleton at keypoints_frame (as float32), both with draw_linewidth (None = max(1,
+    Hf / 240), so that lines look as they would on the 240-row network image; draw.py, DESIGN.md section 4.16).  In track mode a
+    slot whose state is lost after the step is not drawn (valid = state lost == 0, on the device).  The results gain frame_drawn
+    [B,Hf,Wf,3] uint8: that buffer, valid until the call after next like the other results.  stream(batches, drawn_every=N) reads
+    it back for every N-th batch only (0: never)."""
 
     RESULT_KEYS = ("keypoints_frame", "keypoints_uv", "keypoint_coord3d", "center", "scale_crop")
     TRACK_KEYS = ("track_score", "track_lost")
     SLOTS_KEYS = ("track_score", "track_lost", "track_detected")
 
     def __init__(self, ctx, batch, frame_hw, size=NETWORK_SIZE, outputs="keypoints", track=False, redetect_every=None, min_score=None,
-                 track_margin=1.5, detect="batch"):
+                 track_margin=1.5, detect="batch", draw=False, draw_linewidth=None):
         self.ctx, self.B = ctx, int(batch)
         self.frame_hw, self.size = (int(frame_hw[0]), int(frame_hw[1])), (int(size[0]), int(size[1]))
         self.track = bool(track)
@@ -160,6 +168,10 @@ class FrameRunner:
         self.min_score, self.track_margin = min_score, float(track_margin)
         dev = ctx.device
         Hf, Wf = self.frame_hw
+        self.draw = bool(draw)
+        self.draw_linewidth = max(1.0, Hf / 240.0) if draw_linewidth is None else float(draw_linewidth)
+        if self.draw:
+            self._draw_colors = np.concatenate([np.repeat(_draw.WHITE[None], 4, 0), _draw.PALETTE])
         h, w = self.size
         self._frames = [torch.empty((self.B, Hf, Wf, 3), dtype=torch.uint8, device=dev) for _ in range(2)]
         self._frames[0].zero_(); self._frames[1].zero_()
@@ -174,6 +186,7 @@ class FrameRunner:
         self._consumed = [torch.cuda.Event() for _ in range(2)]
         self._d2h_done = [torch.cuda.Event() for _ in range(2)]
         self._host = [None, None]
+        self._host_keys = [(), ()]          # the results the latest read-back of each buffer copied
         self._i = 0
         ctx.ensure_workspace(self.B, h, w)
 
@@ -202,6 +215,11 @@ class FrameRunner:
             else:
                 r = ctx.pipeline(self._image[k], self._hs[k], True, outputs=outputs)
             r["keypoints_frame"] = frame_coords(trafo_coords(r["keypoints_uv"], r["center"], r["scale_crop"], 256), self.frame_hw, self.size)
+            if self.draw:
+                seg = torch.cat([_draw.crop_box_segments(r["center"], r["scale_crop"], self.frame_hw, self.size),
+                                 _draw.hand_segments(r["keypoints_frame"].to(torch.float32))], 1).contiguous()
+                valid = (self._state.lost == 0).to(torch.int32) if self.track else None
+                r["frame_drawn"] = ctx.draw_segments(self._frames[k], seg, self._draw_colors, self.draw_linewidth, valid)
             return r
 
         kinds = (True, False) if self.track and not self.slots else (True,)
@@ -273,6 +291,8 @@ class FrameRunner:
             self._stage_hs[k].copy_(torch.as_tensor(np.asarray([[1.0, 0.0]] * self.B if hand_side is None else hand_side, np.float32)).reshape(self.B, 2))
             with torch.cuda.stream(self._copy):
                 self._copy.wait_event(self._consumed[k])      # the replay that last read this input buffer has finished
+                if self.draw:
+                    self._copy.wait_event(self._d2h_done[k])  # and stream()'s read-back of frame_drawn, which is this buffer
                 self._frames[k].copy_(self._stage[k], non_blocking=True)
                 self._hs[k].copy_(self._stage_hs[k], non_blocking=True)
                 self._uploaded[k].record(self._copy)
@@ -283,6 +303,8 @@ class FrameRunner:
         self._graphs[k][kind].replay()
         self._consumed[k].record(cur)
         res = {n: self._results[k][kind][n] for n in self.RESULT_KEYS}
+        if self.draw:
+            res["frame_drawn"] = self._results[k][kind]["frame_drawn"]
         if self.slots:
             res.update({n: self._results[k][kind][n] for n in self.SLOTS_KEYS})
         elif self.track:
@@ -293,16 +315,28 @@ class FrameRunner:
             res["detected"] = detect
         return res
 
-    def stream(self, batches):
-        """batches: iterable of frames, or of (frames, hand_side) -> yields one numpy dict per batch, in order."""
+    def stream(self, batches, drawn_every=1):
+        """batches: iterable of frames, or of (frames, hand_side) -> yields one numpy dict per batch, in order.
+
+        With draw=True, frame_drawn is read back for batches i with i % drawn_every == 0 only (drawn_every = 0: never), so that a
+        stream that wants key-points and an occasional picture does not copy every drawn frame to the host."""
+        drawn_every = int(drawn_every)
+        if drawn_every < 0:
+            raise ValueError("FrameRunner.stream: drawn_every must be >= 0, got %d" % drawn_every)
         pending = None
-        for item in batches:
+        for i, item in enumerate(batches):
             frames, hs = item if isinstance(item, tuple) else (item, None)
             res = self.submit(frames, hs)
             res.pop("detected", None)       # a host value: _collect adds it
+            if "frame_drawn" in res and (drawn_every == 0 or i % drawn_every):
+                del res["frame_drawn"]
             k = (self._i - 1) & 1
             if self._host[k] is None:
-                self._host[k] = {n: torch.empty(t.shape, dtype=t.dtype).pin_memory() for n, t in res.items()}
+                self._host[k] = {}
+            for n, t in res.items():        # pinned host copies, created on the first read-back of each result
+                if n not in self._host[k]:
+                    self._host[k][n] = torch.empty(t.shape, dtype=t.dtype).pin_memory()
+            self._host_keys[k] = tuple(res)
             with torch.cuda.stream(self._d2h):
                 self._d2h.wait_event(self._consumed[k])
                 for n, t in res.items():
@@ -316,7 +350,7 @@ class FrameRunner:
 
     def _collect(self, k):
         self._d2h_done[k].synchronize()             # the read-back the caller asked for
-        out = {n: t.numpy().copy() for n, t in self._host[k].items()}
+        out = {n: self._host[k][n].numpy().copy() for n in self._host_keys[k]}
         if self.track and not self.slots:
             out["detected"] = self._detected[k]
         return out

@@ -564,6 +564,31 @@ class Context:
                                               _stream()), "h3d_resize_frames")
         return out
 
+    def draw_segments(self, images, segments, colors, linewidth=1.0, valid=None):
+        """h3d_draw_segments: anti-aliased segments drawn into images (CUDA uint8 [B,H,W,3], contiguous) in place, which it returns.
+        segments CUDA float32 [B,S,4] (r0, c0, r1, c1) in pixels; colors [S,3] in 0..255 (host values, carried by a captured graph);
+        valid CUDA int32 [B] or None (an image with valid[b] == 0 is left alone).  Enqueues one kernel and nothing else, so it can
+        be captured into a CUDA graph."""
+        if not isinstance(images, torch.Tensor) or not images.is_cuda:
+            raise RuntimeError("images must be a CUDA tensor (hand3d_b200 has no CPU path)")
+        if images.dtype != torch.uint8 or images.dim() != 4 or images.shape[3] != 3 or not images.is_contiguous():
+            raise ValueError("images must be contiguous uint8 [B,H,W,3], got %s %s" % (images.dtype, tuple(images.shape)))
+        B, H, W, _ = images.shape
+        segments = _chk_f32(segments, "segments", 3)
+        if segments.shape[0] != B or segments.shape[2] != 4 or segments.device != images.device:
+            raise ValueError("segments must be [%d,S,4] on the images' device, got %s" % (B, tuple(segments.shape)))
+        S = segments.shape[1]
+        cols = np.ascontiguousarray(colors, dtype=np.float32)
+        if cols.shape != (S, 3):
+            raise ValueError("colors must be [%d,3], got %s" % (S, cols.shape))
+        if valid is not None:
+            if not isinstance(valid, torch.Tensor) or valid.dtype != torch.int32 or tuple(valid.shape) != (B,) or valid.device != images.device:
+                raise ValueError("valid must be an int32 tensor [%d] on the images' device" % B)
+            valid = valid.contiguous()
+        _lib.check(self.lib.h3d_draw_segments(self.h, _ptr(images), B, H, W, _ptr(segments), S, cols.ctypes.data_as(C.c_void_p),
+                                              _ptr(valid), C.c_float(linewidth), _stream()), "h3d_draw_segments")
+        return images
+
     # ---- training (h3d_resize_bilinear_tf1_backward, the two losses, Adam) ----------------------
     def variables(self, scope):
         """Ordered {reference variable name: torch.nn.Parameter} of "HandSegNet", "PoseNet2D", "PosePrior" (with fc_bottleneck when

@@ -578,6 +578,25 @@ H3D_API int h3d_mse_loss_forward(h3d_ctx* ctx, const float* pred, const float* t
 H3D_API int h3d_mse_loss_backward(h3d_ctx* ctx, const float* pred, const float* target, const float* grad_loss, int64_t n, float* dpred,
                                   void* stream);
 
+/* ---- drawing (utils/general.py:360-477, plot_hand / plot_hand_3d: the stick figures run.py shows)
+ * Draws S anti-aliased segments into each of B uint8 RGB images [B,H,W,3] (device, contiguous), in place.  segments [B,S,4] float32
+ * (device): (r0, c0, r1, c1) in pixels, pixel (y, x) centred at (y, x).  host_colors [S,3] float32 (HOST, 0..255) are copied into the
+ * kernel's parameters, so a captured graph carries them.  valid [B] int32 (device) or NULL: an image with valid[b] == 0 is left alone.
+ * The rule, in fp32 with no contraction: h = linewidth / 2 + 0.5; for each segment k in order whose four values are finite,
+ * dy = r1 - r0, dx = c1 - c0, L2 = dy*dy + dx*dx, ry = y - r0, rx = x - c0, t = clamp(L2 > 0 ? (ry*dy + rx*dx) / L2 : 0, 0, 1)
+ * (NaN -> 0), ey = ry - t*dy, ex = rx - t*dx, d = sqrt(ey*ey + ex*ex), a = clamp(h - d, 0, 1) (NaN -> 0); where a > 0 each channel
+ * v = v + a * (C[k] - v), v starting as float(byte); the byte written is rint(v) clamped to 0..255.  Segment k reaches only the
+ * pixels of its box min(r0, r1) - g <= y <= max(r0, r1) + g, min(c0, c1) - g <= x <= max(c0, c1) + g (g = h + 1, bounds in fp32);
+ * outside it a = 0.  For end points within 2^14 px of the image the box changes nothing (d > h outside it); farther out x - c0 and
+ * c1 - c0 can round alike, and the box keeps a long segment from drawing past its end.  A pixel no segment covers keeps its byte.
+ * 1 <= H, W <= H3D_FRAME_MAX_SIDE, 1 <= S <= H3D_DRAW_MAX_SEGMENTS, 0 < linewidth <= H3D_DRAW_MAX_LINEWIDTH (finite), colours finite
+ * in 0..255, no NULL but valid; anything else is H3D_EINVAL with nothing enqueued.  Enqueues one kernel whose grid
+ * depends on (B, H, W) only; allocates nothing (capturable). */
+#define H3D_DRAW_MAX_SEGMENTS 64
+#define H3D_DRAW_MAX_LINEWIDTH 64
+H3D_API int h3d_draw_segments(h3d_ctx* ctx, uint8_t* images, int B, int H, int W, const float* segments, int S, const float* host_colors,
+                              const int32_t* valid, float linewidth, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
