@@ -5,13 +5,14 @@ PosePriorNetwork(variant).inference(train=True) -> the variant's MSE loss -> Ada
 show_loss_freq and pickled snapshots every snapshot_freq iterations.
 
     python examples/train_lifting_demo.py --variant {direct,bottleneck,local,local_w_xyz_loss,proposed} [--db rhd_training.bin]
-                                          [--iters 30] [--augment] [--seed S] [--device-resident [--graph]]
+                                          [--iters 30] [--augment] [--seed S] [--device-resident [--graph]] [--dropout SEED]
 
 Like the reference, it starts from the initialisers (weights.xavier_weights: Xavier-uniform weights, biases 1e-4; the same
 distributions as tf.global_variables_initializer(), not TF's random values), not from a pickle.  Without --db it trains on a few
 synthetic records (examples/_synthetic_db.py).  The reference never feeds its `evaluation` placeholder, whose default is True, so
-dropout is the identity in its training too.  Snapshots are in the reference's weight-pickle layout
-(PosePriorNetwork(variant).init(weight_files=[...]) loads them), not TF checkpoints.  --device-resident keeps the records on the GPU;
+dropout is the identity in its training too; --dropout SEED trains with evaluation=False instead, as the networks' docstrings describe
+(dropout after the hidden FC layers, drawn from the context's generator seeded with SEED).  Snapshots are in the reference's
+weight-pickle layout (PosePriorNetwork(variant).init(weight_files=[...]) loads them), not TF checkpoints.  --device-resident keeps the records on the GPU;
 --graph then captures reading, the step and Adam once after two eager iterations and replays that CUDA graph for every later
 iteration.  Both print the losses of the plain run.
 """
@@ -54,6 +55,8 @@ if __name__ == '__main__':
     ap.add_argument("--device-resident", action="store_true", help="upload the records to the GPU once; get() then runs on the device")
     ap.add_argument("--graph", action="store_true", help="replay each iteration (reading, step, Adam) from one CUDA graph; "
                                                          "needs --device-resident")
+    ap.add_argument("--dropout", type=int, default=None, metavar="SEED",
+                    help="train with evaluation=False: the lifting stage's dropout, seeded with SEED")
     args = ap.parse_args()
     if args.graph and not args.device_resident:
         ap.error("--graph captures the reader too, which needs --device-resident")
@@ -76,6 +79,9 @@ if __name__ == '__main__':
         net = PosePriorNetwork(VARIANT)
         ctx = runtime.default_context()
         ctx.set_precision('bf16x3')
+        evaluation = args.dropout is None
+        if not evaluation:
+            ctx.set_dropout(args.dropout)
         # tf.global_variables_initializer() (:85)
         ctx.load_weights(Wt.xavier_weights(args.seed, bottleneck=VARIANT == 'bottleneck'))
         scopes = ['PosePrior', 'ViewpointNet'] if VARIANT == 'proposed' else ['PosePrior']
@@ -95,7 +101,7 @@ if __name__ == '__main__':
 
         def iteration():
             data = dataset.get()
-            _, coord3d_pred, R = net.inference(data['scoremap'], data['hand_side'], True, train=True)       # :53-54
+            _, coord3d_pred, R = net.inference(data['scoremap'], data['hand_side'], evaluation, train=True)  # :53-54
             if VARIANT in ('direct', 'bottleneck'):                                                          # :62-76
                 loss = A.mse_loss(coord3d_pred, data['keypoint_xyz21_normed'])
             elif VARIANT == 'local':

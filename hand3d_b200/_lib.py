@@ -103,6 +103,12 @@ SIGNATURES = {
     "h3d_eval_feed": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _i, _i, _p]),
     "h3d_eval_stats": (_i, [_p, _p, _i, _i, _i, _p, _i, _p, _p]),
     "h3d_draw_segments": (_i, [_p, _p, _i, _i, _i, _p, _i, _p, _p, _f, _p]),
+    "h3d_set_dropout": (_i, [_p, _i, C.c_uint64]),
+    "h3d_dropout_draw": (_i, [_p, C.POINTER(_p)]),
+    "h3d_dropout_forward": (_i, [_p, _p, _i, _i, _f, _i, _p, _p, _p]),
+    "h3d_dropout_forward_planes": (_i, [_p, _p, _i, _i, _f, _i, _p, _p, _i, _i, _p, _p, _p]),
+    "h3d_dropout_backward": (_i, [_p, _p, _p, _i, _i, _f, _p, _p]),
+    "h3d_dropout_advance": (_i, [_p, _p]),
 }
 ADAM_STATE_WORDS = 4   # H3D_ADAM_STATE_WORDS
 # training-mode reader augmentation (H3D_AUG_*): flags, and the per-sample parameter layout
@@ -124,6 +130,10 @@ EVAL_MAX_KP, EVAL_MAX_DIM, EVAL_MAX_SAMPLES, EVAL_MAX_THRESHOLDS = 64, 4, 1 << 2
 EVAL_STAT_N, EVAL_STAT_MEAN, EVAL_STAT_MEDIAN, EVAL_STAT_COUNTS = 0, 1, 2, 3
 # drawing (H3D_DRAW_*): the most segments per call and the widest line of h3d_draw_segments
 DRAW_MAX_SEGMENTS, DRAW_MAX_LINEWIDTH = 64, 64
+# dropout of the lifting stage (H3D_DROPOUT_*): the generator's stream id, the layer ids and their keep probabilities
+DROPOUT_STREAM = 2
+DROPOUT_LAYER_FC_REL0, DROPOUT_LAYER_FC_REL1, DROPOUT_LAYER_FC_VP0, DROPOUT_LAYER_FC_VP1, DROPOUT_LAYER_OP = 0, 1, 2, 3, 4
+DROPOUT_KEEP_POSEPRIOR, DROPOUT_KEEP_VIEWPOINT = 0.8, 0.75
 
 _lib = None
 

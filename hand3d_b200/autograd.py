@@ -14,6 +14,7 @@ input's device; there is no CPU path.
     R, out = rotate_canonical(can, uxyz, hs)     # PosePriorNetwork 'proposed': Rodrigues, flip, rotate
     xyz = bone_rel_trafo_inv(rel)                # the 'local*' variants' forward kinematics
     L = mse_loss(pred, target)                   # training_lifting.py:63-76
+    y = dropout(x, 0.8, layer)                   # ops.dropout with evaluation=False, on a seeded context (Context.set_dropout)
 
 The backward of every function reads the incoming gradient on the device: no .item(), no host synchronisation, so a whole training
 step can be captured into a CUDA graph.
@@ -139,6 +140,27 @@ class _MseLoss(torch.autograd.Function):
     def backward(ctx, g):
         pred, target = ctx.saved_tensors
         return _ctx(g).mse_loss_backward(pred, target, g), None
+
+
+class _Dropout(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, keep_prob, layer):
+        y, keep = _ctx(x).dropout_forward(x, keep_prob, layer)
+        ctx.save_for_backward(keep)
+        ctx.keep_prob = keep_prob
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (keep,) = ctx.saved_tensors
+        return _ctx(dy).dropout_backward(dy.contiguous(), keep, ctx.keep_prob), None, None
+
+
+def dropout(x, keep_prob, layer):
+    """TF 1.3 dropout (utils/general.py:139-148) of x [rows, ...] at the context's current draw, with `layer` as the generator's layer id
+    (H3D_DROPOUT_LAYER_*): y = (x / keep_prob) * k.  The keep bits are saved for the backward, dx = (dy * k) / keep_prob.  Does not
+    advance the draw: Context.dropout_advance() does, once per network forward."""
+    return _Dropout.apply(x.contiguous(), float(keep_prob), int(layer))
 
 
 def fully_connected(x, w, b, leaky=True, precision="bf16x3"):

@@ -24,7 +24,7 @@ LIB_SKEW = os.path.join(HERE, "libhand3d_b200_skew.so")
 STAMP_SKEW = os.path.join(HERE, ".libhand3d_b200_skew.stamp")
 SKEW_FLAGS = ["-DH3D_SKEW_BUILD"]
 SOURCES = ["api.cu", "elementwise.cu", "reader.cu", "reader_aug.cu", "conv_direct.cu", "conv_wgmma.cu", "conv_wgrad.cu", "train.cu", "train_lift.cu",
-           "frames.cu", "eval.cu", "track.cu", "draw.cu"]
+           "frames.cu", "eval.cu", "track.cu", "draw.cu", "dropout.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--cudart=static", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",

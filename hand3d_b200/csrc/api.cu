@@ -153,6 +153,7 @@ struct h3d_ctx {
     float* vp_head_w = nullptr; float* vp_head_b = nullptr;   // fused fc_vp_ux/uy/uz [128,3]
     char* ws = nullptr; int64_t ws_bytes = 0;
     std::unique_ptr<StagePlan> seg, pose, lift;
+    std::unique_ptr<StagePlan> lift_drop;     // the lifting plan while dropout is on (h3d_set_dropout), kept beside `lift`
     std::unique_ptr<StagePlan> seg_counted;   // HandSegNet's counted plan (h3d_track_step_slots), built on first use beside `seg`
     // persistent buffers inside the workspace (laid out by layout())
     struct Layout {
@@ -163,7 +164,7 @@ struct h3d_ctx {
         float *seg_low, *s[3];
         int64_t seg_off, pose_off, lift_off, total;
     } lay;
-    void drop_plans() { seg.reset(); pose.reset(); lift.reset(); seg_counted.reset(); }
+    void drop_plans() { seg.reset(); pose.reset(); lift.reset(); lift_drop.reset(); seg_counted.reset(); }
     // independent branches (PosePrior || ViewpointNet, x8 up-sampling || lifting) run on two private streams that fork from
     // and join back into the caller's stream with events (capturable into a CUDA graph)
     cudaStream_t side = nullptr, side2 = nullptr;
@@ -173,6 +174,10 @@ struct h3d_ctx {
     // after the trap has poisoned the CUDA context (h3d_check_errors).
     int* err_flag = nullptr;
     unsigned int* fc_counter = nullptr;      // ticket of the FC-chain kernel ("last cluster applies the rotation epilogue"), zero between launches
+    // dropout generator (h3d_set_dropout): the draw counter lives on the device so that captured graphs advance it on every replay
+    int64_t* drop_draw = nullptr;
+    uint64_t drop_seed = 0;
+    bool drop_on = false, drop_seeded = false;
     // Slot selection of h3d_track_step_slots for up to track_cap slots, outside the workspace: track_sel = [count | slots[B] | pos[B]]
     // (launch_track_select), track_crop = [center [B,2] | scale [B]] of the selected slots in compact order.  Grown (old blocks retired)
     // when the counted plan is built, so a step itself never allocates.
@@ -685,6 +690,7 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
     const int passes = 3;
     const Half16 half = half_of(ctx->precision);
     const bool tc_lift = is_tc(ctx->precision) && passes_of(ctx->precision) != 4 && !tc_tuning().lift_direct;
+    const bool drop = ctx->drop_on;
     const int64_t slot_bytes = align_up((int64_t)B * 32 * 32 * 64 * 4, 1024);
     char* slot_in = a.alloc<char>(slot_bytes);
     const int64_t fcs_floats = lift_fc_scratch_floats(B);
@@ -760,9 +766,30 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
         return add_tc(ctx, pl.get(), scope, l, B, 1, 1, x.s, x.stride, (int)align_up(in_f, 64), {}, y ? y->s : Split(), y ? y->stride : 0, 0, yf,
                       out_f, 0, 0, passes);
     };
+    // dropout after a hidden FC layer: fp32 x [B, cols] in place, or (y != nullptr) into the next tensor-core layer's planes.  The seed is
+    // read when the step is enqueued, the draw on the device.
+    auto add_dropout = [&](float* x, int cols, float keep_prob, int layer, const Planes* y) {
+        const h3d_ctx* cx = ctx;
+        const int64_t* draw = ctx->drop_draw;
+        const Split ys = y ? y->s : Split();
+        const int stride = y ? y->stride : 0;
+        float* yf = y ? nullptr : x;
+        pl->steps.push_back([=](const Ext&, cudaStream_t s) {
+            return launch_dropout(x, B, cols, keep_prob, layer, cx->drop_seed, draw, yf, nullptr, ys, stride, half, s);
+        });
+        pl->launches.push_back(1);
+    };
+    // the tensor-core hidden layer: straight into the next layer's planes, or with dropout through fp32 t
+    auto fc_tc_hidden = [&](const std::string& scope, const char* name, int in_f, int out_f, const Planes& x, const Planes& y, float* t,
+                            float keep_prob, int layer) -> int {
+        if (!drop) return fc_tc(scope, name, in_f, out_f, 1, x, &y, nullptr);
+        int rc2 = fc_tc(scope, name, in_f, out_f, 1, x, nullptr, t);
+        if (!rc2) add_dropout(t, out_f, keep_prob, layer, &y);
+        return rc2;
+    };
     // ---- FC stacks + Rodrigues / flip / rotate as ONE kernel (fc_chain_kernel): both pyramids first (ViewpointNet on the side
     //      stream), their concat kernels, one join, one launch.  tune.fc_chain = 0 keeps the layer-by-layer path below.
-    const bool use_chain = tc_lift && tc_tuning().fc_chain != 0;
+    const bool use_chain = tc_lift && tc_tuning().fc_chain != 0 && !drop;
     if (use_chain) {
         if (bott) H3D_REQUIRE(xyz_in == 30, "bottleneck variant needs PosePrior/fc_xyz/weights of shape [30,63]");
         else H3D_REQUIRE(xyz_in == 512, "PosePrior/fc_xyz/weights must have shape [512,63] for this variant");
@@ -850,8 +877,8 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
             const Planes xp = carve_planes(cur, 2050), p1 = carve_planes(cur, 512), p2 = carve_planes(cur, 512), p3 = carve_planes(cur, 64);
             pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 2048, xp.stride, half, s); });
             pl->launches.push_back(1);
-            if ((rc2 = fc_tc("PosePrior", "fc_rel0", 2050, 512, 1, xp, &p1, nullptr))) return rc2;
-            if ((rc2 = fc_tc("PosePrior", "fc_rel1", 512, 512, 1, p1, &p2, nullptr))) return rc2;
+            if ((rc2 = fc_tc_hidden("PosePrior", "fc_rel0", 2050, 512, xp, p1, b.t1, 0.8f, H3D_DROPOUT_LAYER_FC_REL0))) return rc2;
+            if ((rc2 = fc_tc_hidden("PosePrior", "fc_rel1", 512, 512, p1, p2, b.t2, 0.8f, H3D_DROPOUT_LAYER_FC_REL1))) return rc2;
             if (bott) {
                 if ((rc2 = fc_tc("PosePrior", "fc_bottleneck", 512, 30, 0, p2, &p3, nullptr))) return rc2;
                 return fc_tc("PosePrior", "fc_xyz", 30, 63, 0, p3, nullptr, can);
@@ -862,7 +889,9 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
         pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_concat_handside(feat, e.hand_side, xcat, B, 2048, s); });
         pl->launches.push_back(1);
         if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_rel0", b.xcat, b.t1, b.fcs, fcs_floats, B, 2050, 512, 1))) return rc2;
+        if (drop) add_dropout(b.t1, 512, 0.8f, H3D_DROPOUT_LAYER_FC_REL0, nullptr);
         if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_rel1", b.t1, b.t2, b.fcs, fcs_floats, B, 512, 512, 1))) return rc2;
+        if (drop) add_dropout(b.t2, 512, 0.8f, H3D_DROPOUT_LAYER_FC_REL1, nullptr);
         if (bott) {
             if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_bottleneck", b.t2, b.t3, b.fcs, fcs_floats, B, 512, 30, 0))) return rc2;
             if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_xyz", b.t3, can, b.fcs, fcs_floats, B, 30, 63, 0))) return rc2;
@@ -884,15 +913,17 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
             const Planes xp = carve_planes(cur, 4098), p1 = carve_planes(cur, 256);
             pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 4096, xp.stride, half, s); });
             pl->launches.push_back(1);
-            if ((rc = fc_tc("ViewpointNet", "fc_vp0", 4098, 256, 1, xp, &p1, nullptr))) return rc;
+            if ((rc = fc_tc_hidden("ViewpointNet", "fc_vp0", 4098, 256, xp, p1, b.t1, 0.75f, H3D_DROPOUT_LAYER_FC_VP0))) return rc;
             if ((rc = fc_tc("ViewpointNet", "fc_vp1", 256, 128, 1, p1, nullptr, b.t2))) return rc;   // fp32 [B,128] for the three 128 -> 1 heads
         } else {
             float* xcat = b.xcat;
             pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_concat_handside(feat, e.hand_side, xcat, B, 4096, s); });
             pl->launches.push_back(1);
             if ((rc = add_fc(ctx, pl.get(), "ViewpointNet/fc_vp0", b.xcat, b.t1, b.fcs, fcs_floats, B, 4098, 256, 1))) return rc;
+            if (drop) add_dropout(b.t1, 256, 0.75f, H3D_DROPOUT_LAYER_FC_VP0, nullptr);
             if ((rc = add_fc(ctx, pl.get(), "ViewpointNet/fc_vp1", b.t1, b.t2, b.fcs, fcs_floats, B, 256, 128, 1))) return rc;
         }
+        if (drop) add_dropout(b.t2, 128, 0.75f, H3D_DROPOUT_LAYER_FC_VP1, nullptr);
         const float* hw = ctx->vp_head_w; const float* hb = ctx->vp_head_b;
         float* t2 = b.t2; float* fcs = b.fcs;
         pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_fc(t2, hw, hb, uxyz, fcs, fcs_floats, B, 128, 3, 0, 128, s); });
@@ -927,6 +958,14 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
         });
         pl->launches.push_back(0);
         pl->seal();
+    }
+    if (drop) {   // after the join: every dropout layer of this forward has read the draw
+        int64_t* draw = ctx->drop_draw;
+        pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_dropout_advance(draw, s); });
+        pl->launches.push_back(1);
+        pl->seal();
+        ctx->lift_drop = std::move(pl);
+        return H3D_OK;
     }
     ctx->lift = std::move(pl);
     return H3D_OK;
@@ -985,7 +1024,7 @@ static int check_device() {
 extern "C" {
 
 const char* h3d_last_error(void) { return g_err; }
-int h3d_version(void) { return 109; }
+int h3d_version(void) { return 110; }
 
 int h3d_device_available(void) {
     int n = 0;
@@ -1030,6 +1069,11 @@ int h3d_create(h3d_ctx** out, int device) {
         h3d_destroy(c);
         return H3D_ECUDA;
     }
+    if (cudaMalloc(&c->drop_draw, sizeof(int64_t)) != cudaSuccess || cudaMemset(c->drop_draw, 0, sizeof(int64_t)) != cudaSuccess) {
+        set_error("h3d_create: cannot allocate the dropout draw counter (%s)", cudaGetErrorString(cudaGetLastError()));
+        h3d_destroy(c);
+        return H3D_ECUDA;
+    }
     tc_tuning();   // read the H3D_* environment switches now, never on a launch path
     *out = c;
     return H3D_OK;
@@ -1063,6 +1107,7 @@ int h3d_destroy(h3d_ctx* ctx) {
     for (void* p : ctx->retired) cudaFree(p);
     if (ctx->err_flag) cudaFreeHost(ctx->err_flag);
     if (ctx->fc_counter) cudaFree(ctx->fc_counter);
+    if (ctx->drop_draw) cudaFree(ctx->drop_draw);
     if (ctx->track_sel) cudaFree(ctx->track_sel);
     if (ctx->track_crop) cudaFree(ctx->track_crop);
     for (auto& kv : ctx->frame_plans) frame_plan_destroy(kv.second);
@@ -1249,10 +1294,11 @@ int h3d_lifting_forward(h3d_ctx* ctx, const float* scoremap32, const float* hand
     H3D_REQUIRE(variant >= H3D_VARIANT_DIRECT && variant <= H3D_VARIANT_LOCAL, "h3d_lifting_forward: unknown variant");
     int rc;
     if ((rc = ensure_layout_covers(ctx, B, 0, 0, 0, 0))) return rc;
-    if (!ctx->lift || ctx->lift->B != B || ctx->lift->variant != variant)
+    std::unique_ptr<StagePlan>& plan = ctx->drop_on ? ctx->lift_drop : ctx->lift;   // build_lifting fills the slot of the current setting
+    if (!plan || plan->B != B || plan->variant != variant)
         if ((rc = build_lifting(ctx, B, variant))) return rc;
     Ext e; e.in = scoremap32; e.hand_side = hand_side; e.out = coord_xyz_rel_normed; e.out2 = coord_can; e.out3 = rot_mat;
-    return run_plan(ctx, ctx->lift.get(), e, (cudaStream_t)stream);
+    return run_plan(ctx, plan.get(), e, (cudaStream_t)stream);
 }
 
 // The pipeline after the crop parameters (cen, scl) are known: crop, PoseNet2D, up-sampling + key-points, lifting.  Shared by
@@ -1947,6 +1993,56 @@ int h3d_draw_segments(h3d_ctx* ctx, uint8_t* images, int B, int H, int W, const 
         H3D_REQUIRE(std::isfinite(host_colors[i]) && host_colors[i] >= 0.f && host_colors[i] <= 255.f,
                     "h3d_draw_segments: colour %d of segment %d must be finite in 0..255, got %g", i % 3, i / 3, (double)host_colors[i]);
     int rc = launch_draw_segments(images, B, H, W, segments, S, host_colors, valid, linewidth, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_set_dropout(h3d_ctx* ctx, int enabled, uint64_t seed) {
+    H3D_REQUIRE(ctx != nullptr, "h3d_set_dropout: ctx is NULL");
+    DeviceGuard guard_(ctx->device);
+    if (enabled && (!ctx->drop_seeded || seed != ctx->drop_seed)) {
+        H3D_CUDA(cudaMemset(ctx->drop_draw, 0, sizeof(int64_t)));
+        ctx->drop_seed = seed; ctx->drop_seeded = true;
+    }
+    ctx->drop_on = enabled != 0;
+    return H3D_OK;
+}
+int h3d_dropout_draw(h3d_ctx* ctx, int64_t** draw) {
+    H3D_REQUIRE(ctx && draw, "h3d_dropout_draw: bad argument");
+    *draw = ctx->drop_draw;
+    return H3D_OK;
+}
+#define H3D_DROPOUT_CHECKS(fn)                                                                                                         \
+    H3D_REQUIRE(rows >= 1 && cols >= 1, fn ": rows and cols must be >= 1, got %d x %d", rows, cols);                                  \
+    H3D_REQUIRE(keep_prob > 0.f && keep_prob <= 1.f, fn ": keep_prob must lie in (0, 1], got %g", (double)keep_prob);                 \
+    H3D_REQUIRE(ctx->drop_on, fn ": dropout is not enabled on this context (h3d_set_dropout)")
+int h3d_dropout_forward_planes(h3d_ctx* ctx, const float* x, int rows, int cols, float keep_prob, int layer, float* y, uint8_t* keep,
+                               int half, int stride, uint16_t* hi, uint16_t* lo, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(x && (y || keep || hi) && layer >= 0, "h3d_dropout_forward: bad argument");
+    H3D_DROPOUT_CHECKS("h3d_dropout_forward");
+    H3D_REQUIRE(!hi || ((half == 0 || half == 1) && stride >= cols), "h3d_dropout_forward_planes: half must be 0 or 1 and stride >= cols");
+    H3D_REQUIRE(hi || !lo, "h3d_dropout_forward_planes: lo without hi");
+    Split sp; sp.hi = hi; sp.lo = lo;
+    int rc = launch_dropout(x, rows, cols, keep_prob, layer, ctx->drop_seed, ctx->drop_draw, y, keep, sp, stride,
+                            half == 1 ? Half16::FP16 : Half16::BF16, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_dropout_forward(h3d_ctx* ctx, const float* x, int rows, int cols, float keep_prob, int layer, float* y, uint8_t* keep, void* stream) {
+    return h3d_dropout_forward_planes(ctx, x, rows, cols, keep_prob, layer, y, keep, 0, cols, nullptr, nullptr, stream);
+}
+int h3d_dropout_backward(h3d_ctx* ctx, const float* dy, const uint8_t* keep, int rows, int cols, float keep_prob, float* dx, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(dy && keep && dx, "h3d_dropout_backward: bad argument");
+    H3D_DROPOUT_CHECKS("h3d_dropout_backward");
+    int rc = launch_dropout_backward(dy, keep, (int64_t)rows * cols, keep_prob, dx, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+int h3d_dropout_advance(h3d_ctx* ctx, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(ctx->drop_on, "h3d_dropout_advance: dropout is not enabled on this context (h3d_set_dropout)");
+    int rc = launch_dropout_advance(ctx->drop_draw, s);
     if (!rc) ctx->launches += 1;
     return rc;
 }

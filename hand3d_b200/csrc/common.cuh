@@ -350,4 +350,13 @@ int64_t mse_scratch_floats(int64_t n);                        // two kernels
 int launch_mse(const float* p, const float* q, float* scratch, int64_t n, float* loss, cudaStream_t s);
 int launch_mse_grad(const float* p, const float* q, const float* grad, float* dp, int64_t n, cudaStream_t s);
 
+// ---------------------------------------------------------------- kernels (dropout.cu): TF 1.3 dropout of the lifting FC stacks
+// Keep bits from Philox4x64-10 keyed (seed, H3D_DROPOUT_STREAM) at counter (*draw, layer, row, col / 4); y and keep may be NULL, x == y is
+// allowed.  planes.hi != NULL also writes the 16-bit hi / lo planes [rows, stride] of y (zero in columns >= cols) that feed a tensor-core
+// FC layer.
+int launch_dropout(const float* x, int rows, int cols, float keep_prob, int layer, uint64_t seed, const int64_t* draw, float* y, uint8_t* keep,
+                   Split planes, int stride, Half16 t, cudaStream_t s);
+int launch_dropout_backward(const float* dy, const uint8_t* keep, int64_t n, float keep_prob, float* dx, cudaStream_t s);
+int launch_dropout_advance(int64_t* draw, cudaStream_t s);
+
 }  // namespace h3d

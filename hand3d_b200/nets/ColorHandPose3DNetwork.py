@@ -61,27 +61,44 @@ def _train_pose2d(image_crop, num_kp):
     return scoremap_list
 
 
-def _train_evaluation(evaluation):
-    if not _truthy(evaluation):
-        raise NotImplementedError("train=True needs evaluation=True: dropout is not implemented (training_lifting.py never feeds "
-                                  "`evaluation`, so its dropout is the identity too)")
+def _dropout_wanted(evaluation):
+    """True for evaluation=False: the lifting stage applies its dropout layers, which needs a seeded context (Context.set_dropout);
+    without a seed evaluation=False raises NotImplementedError."""
+    if _truthy(evaluation):
+        return False
+    runtime.default_context()._dropout_mode(True)
+    return True
+
+
+# the dropout layers of the lifting stage's FC stacks (nets/PosePriorNetwork.py:113-114, 151-154): (keep_prob, layer id) per hidden layer
+_DROPOUT = {"fc_rel0": (_lib.DROPOUT_KEEP_POSEPRIOR, _lib.DROPOUT_LAYER_FC_REL0), "fc_rel1": (_lib.DROPOUT_KEEP_POSEPRIOR, _lib.DROPOUT_LAYER_FC_REL1),
+            "fc_vp0": (_lib.DROPOUT_KEEP_VIEWPOINT, _lib.DROPOUT_LAYER_FC_VP0), "fc_vp1": (_lib.DROPOUT_KEEP_VIEWPOINT, _lib.DROPOUT_LAYER_FC_VP1)}
+
+
+def _train_advance(dropout):
+    """Ends one network forward: the next one draws new masks."""
+    if dropout:
+        runtime.default_context().dropout_advance()
 
 
 def _train_lift_input(pooled, hand_side):
     return pooled.to(torch.float32).contiguous(), hand_side.to(torch.float32).contiguous()
 
 
-def _train_fc_stack(x, hand_side, v, scope, names, prec):
-    """Flatten (NHWC order, as tf.reshape), concat hand_side, then the leaky FC layers `names` (nets/PosePriorNetwork.py:110-114)."""
+def _train_fc_stack(x, hand_side, v, scope, names, prec, dropout=False):
+    """Flatten (NHWC order, as tf.reshape), concat hand_side, then the leaky FC layers `names` (nets/PosePriorNetwork.py:110-114),
+    each followed by its dropout layer when `dropout` (at the current draw; the caller advances it)."""
     x = torch.cat([x.reshape(x.shape[0], -1), hand_side], 1)
     for name in names:
         x = A.fully_connected(x, v["%s/%s/weights" % (scope, name)], v["%s/%s/biases" % (scope, name)], True, prec)
+        if dropout:
+            x = A.dropout(x, *_DROPOUT[name])
     return x
 
 
-def _train_pose3d_can(pooled, hand_side, bottleneck=False):
-    """PosePrior (nets/PosePriorNetwork.py:97-122) over ctx.variables('PosePrior'): [B,32,32,21], [B,2] -> [B,21,3].  Dropout is the
-    identity: training_lifting.py never feeds `evaluation`, whose default is True."""
+def _train_pose3d_can(pooled, hand_side, bottleneck=False, dropout=False):
+    """PosePrior (nets/PosePriorNetwork.py:97-122) over ctx.variables('PosePrior'): [B,32,32,21], [B,2] -> [B,21,3].  dropout=True
+    (evaluation=False) applies the dropout after fc_rel0 and fc_rel1 at the current draw."""
     _, v, prec = _train_scope("PosePrior")
     has_bn = "PosePrior/fc_bottleneck/weights" in v
     if bottleneck != has_bn:
@@ -89,20 +106,21 @@ def _train_pose3d_can(pooled, hand_side, bottleneck=False):
             "'bottleneck'" if bottleneck else "non-bottleneck", "an" if bottleneck else "no"))
     pooled, hand_side = _train_lift_input(pooled, hand_side)
     x = _train_layers(pooled, v, "PosePrior", arch.POSEPRIOR[:6], (), prec)
-    x = _train_fc_stack(x, hand_side, v, "PosePrior", ("fc_rel0", "fc_rel1"), prec)
+    x = _train_fc_stack(x, hand_side, v, "PosePrior", ("fc_rel0", "fc_rel1"), prec, dropout)
     if bottleneck:
         x = A.fully_connected(x, v["PosePrior/fc_bottleneck/weights"], v["PosePrior/fc_bottleneck/biases"], False, prec)
     x = A.fully_connected(x, v["PosePrior/fc_xyz/weights"], v["PosePrior/fc_xyz/biases"], False, prec)
     return x.view(x.shape[0], 21, 3)
 
 
-def _train_viewpoint_u(pooled, hand_side):
+def _train_viewpoint_u(pooled, hand_side, dropout=False):
     """ViewpointNet (nets/PosePriorNetwork.py:136-159) over ctx.variables('ViewpointNet') -> uxyz [B,3].  The three 128 -> 1 heads
-    run as one 128 -> 3 layer whose weights are the concatenation of the three variables."""
+    run as one 128 -> 3 layer whose weights are the concatenation of the three variables.  dropout=True applies the dropout after fc_vp0
+    and fc_vp1 at the current draw."""
     _, v, prec = _train_scope("ViewpointNet")
     pooled, hand_side = _train_lift_input(pooled, hand_side)
     x = _train_layers(pooled, v, "ViewpointNet", arch.VIEWPOINT[:6], (), prec)
-    x = _train_fc_stack(x, hand_side, v, "ViewpointNet", ("fc_vp0", "fc_vp1"), prec)
+    x = _train_fc_stack(x, hand_side, v, "ViewpointNet", ("fc_vp0", "fc_vp1"), prec, dropout)
     heads = ["ViewpointNet/fc_vp_u%s" % a for a in "xyz"]
     w = torch.cat([v[h + "/weights"] for h in heads], 1)
     b = torch.cat([v[h + "/biases"] for h in heads], 0)
@@ -151,10 +169,10 @@ class ColorHandPose3DNetwork(object):
 
             Returns (hand_scoremap [B,H,W,2], image_crop [B,256,256,3], scale_crop [B,1], center [B,2],
                      keypoints_scoremap [B,256,256,21], keypoint_coord3d [B,21,3]).
+
+            evaluation=False applies the lifting stage's dropout (a seeded context: runtime.default_context().set_dropout(seed)).
         """
-        if not _truthy(evaluation):
-            raise NotImplementedError("forward pass only: evaluation must be True (dropout is the identity)")
-        r = runtime.default_context().pipeline(image, hand_side, with_pose3d=True)
+        r = runtime.default_context().pipeline(image, hand_side, with_pose3d=True, dropout=_dropout_wanted(evaluation))
         self.last_keypoints_uv = r["keypoints_uv"]
         return (r["hand_scoremap"], r["image_crop"], r["scale_crop"], r["center"], r["keypoints_scoremap"],
                 r["keypoint_coord3d"])
@@ -193,30 +211,40 @@ class ColorHandPose3DNetwork(object):
         """ PosePrior + Viewpoint (reference :221-247): [B,32,32,21], [B,2] -> [B,21,3].
 
             train=True builds the graph from hand3d_b200.autograd over ctx.variables('PosePrior') and ctx.variables('ViewpointNet').
-            evaluation=False (dropout) is not supported.
+            evaluation=False applies the dropout layers (a seeded context: runtime.default_context().set_dropout(seed)); one call is one
+            draw.
         """
-        if not _truthy(evaluation):
-            raise NotImplementedError("forward pass only: evaluation must be True (dropout is the identity)")
+        drop = _dropout_wanted(evaluation)
         if train:
-            can = _train_pose3d_can(keypoints_scoremap, hand_side)
-            return _train_rotate(can, _train_viewpoint_u(keypoints_scoremap, hand_side), hand_side)[1]
-        return runtime.default_context().lifting(keypoints_scoremap, hand_side, "proposed")[0]
+            can = _train_pose3d_can(keypoints_scoremap, hand_side, dropout=drop)
+            out = _train_rotate(can, _train_viewpoint_u(keypoints_scoremap, hand_side, dropout=drop), hand_side)[1]
+            _train_advance(drop)
+            return out
+        return runtime.default_context().lifting(keypoints_scoremap, hand_side, "proposed", dropout=drop)[0]
+
+    @staticmethod
+    def _optional_dropout(evaluation):
+        # these two entries ignored `evaluation` before dropout existed: without a seed it stays the identity
+        return not _truthy(evaluation) and runtime.default_context().dropout_seed is not None
 
     def _inference_pose3d_can(self, keypoints_scoremap, hand_side, evaluation=True, train=False):
-        """ Canonical coordinates (reference :249-272). """
+        """ Canonical coordinates (reference :249-272).  evaluation=False on a seeded context applies PosePrior's dropout. """
         if train:
-            _train_evaluation(evaluation)
-            return _train_pose3d_can(keypoints_scoremap, hand_side)
-        return runtime.default_context().lifting(keypoints_scoremap, hand_side, "proposed")[1]
+            drop = _dropout_wanted(evaluation)
+            can = _train_pose3d_can(keypoints_scoremap, hand_side, dropout=drop)
+            _train_advance(drop)
+            return can
+        return runtime.default_context().lifting(keypoints_scoremap, hand_side, "proposed", dropout=self._optional_dropout(evaluation))[1]
 
     def _inference_viewpoint(self, keypoints_scoremap, hand_side, evaluation=True, train=False):
-        """ Viewpoint rotation matrix (reference :274-283). """
+        """ Viewpoint rotation matrix (reference :274-283).  evaluation=False on a seeded context applies ViewpointNet's dropout. """
         if train:
-            _train_evaluation(evaluation)
-            u = _train_viewpoint_u(keypoints_scoremap, hand_side)
+            drop = _dropout_wanted(evaluation)
+            u = _train_viewpoint_u(keypoints_scoremap, hand_side, dropout=drop)
+            _train_advance(drop)
             zeros = torch.zeros((u.shape[0], 21, 3), dtype=torch.float32, device=u.device)
             return _train_rotate(zeros, u, hand_side)[0]
-        return runtime.default_context().lifting(keypoints_scoremap, hand_side, "proposed")[2]
+        return runtime.default_context().lifting(keypoints_scoremap, hand_side, "proposed", dropout=self._optional_dropout(evaluation))[2]
 
     def _get_rot_mat(self, ux_b, uy_b, uz_b):
         """ Rodrigues rotation matrix from axis * angle (reference :311-334): three [B,1] -> [B,3,3]. """

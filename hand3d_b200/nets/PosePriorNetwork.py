@@ -43,38 +43,42 @@ class PosePriorNetwork(object):
             train=True builds the graph from hand3d_b200.autograd over ctx.variables('PosePrior') (and ctx.variables('ViewpointNet')
             for 'proposed'), as the reference's own inference() does with trainable variables (training_lifting.py:54): a loss of
             coord3d, R or coord_xyz_rel_normed back-propagates into those Parameters.  The 8x8 average pool takes no gradient.
+
+            evaluation=False applies the dropout layers after fc_rel0 / fc_rel1 (keep 0.8) and fc_vp0 / fc_vp1 (keep 0.75, 'proposed'),
+            drawn from the context's seeded generator (runtime.default_context().set_dropout(seed)); one call is one draw.
         """
-        ev = bool(evaluation.item()) if torch.is_tensor(evaluation) else bool(evaluation)
-        if not ev:
-            raise NotImplementedError("forward pass only: evaluation must be True")
+        from .ColorHandPose3DNetwork import _dropout_wanted
+        drop = _dropout_wanted(evaluation)
         ctx = runtime.default_context()
         scoremap_pooled = ctx.avg_pool8(scoremap)                       # :61
         if train:
-            return self._train_inference(scoremap_pooled, hand_side)
+            return self._train_inference(scoremap_pooled, hand_side, drop)
         if self.variant in ('direct', 'bottleneck'):
-            c, _, _ = ctx.lifting(scoremap_pooled, hand_side, self.variant)
+            c, _, _ = ctx.lifting(scoremap_pooled, hand_side, self.variant, dropout=drop)
             return c, c, None
         elif self.variant in ('local', 'local_w_xyz_loss'):
             # :70-75 -- the net predicts bone-relative coords; bone_rel_trafo_inv (utils/relative_trafo.py:243) assembles xyz
-            normed, rel, _ = ctx.lifting(scoremap_pooled, hand_side, 'local')
+            normed, rel, _ = ctx.lifting(scoremap_pooled, hand_side, 'local', dropout=drop)
             return normed, rel, None
         elif self.variant == 'proposed':
-            out, can, R = ctx.lifting(scoremap_pooled, hand_side, 'proposed')
+            out, can, R = ctx.lifting(scoremap_pooled, hand_side, 'proposed', dropout=drop)
             return out, can, R
         else:
             assert 0, "Unknown variant."
 
-    def _train_inference(self, scoremap_pooled, hand_side):
-        from .ColorHandPose3DNetwork import _train_pose3d_can, _train_rotate, _train_viewpoint_u
+    def _train_inference(self, scoremap_pooled, hand_side, drop=False):
+        from .ColorHandPose3DNetwork import _train_advance, _train_pose3d_can, _train_rotate, _train_viewpoint_u
         if self.variant in ('direct', 'bottleneck'):
-            c = _train_pose3d_can(scoremap_pooled, hand_side, bottleneck=self.variant == 'bottleneck')
-            return c, c, None
+            c = _train_pose3d_can(scoremap_pooled, hand_side, bottleneck=self.variant == 'bottleneck', dropout=drop)
+            r = c, c, None
         elif self.variant in ('local', 'local_w_xyz_loss'):
-            rel = _train_pose3d_can(scoremap_pooled, hand_side)
-            return A.bone_rel_trafo_inv(rel), rel, None
+            rel = _train_pose3d_can(scoremap_pooled, hand_side, dropout=drop)
+            r = A.bone_rel_trafo_inv(rel), rel, None
         elif self.variant == 'proposed':
-            can = _train_pose3d_can(scoremap_pooled, hand_side)
-            R, out = _train_rotate(can, _train_viewpoint_u(scoremap_pooled, hand_side), hand_side)
-            return out, can, R
+            can = _train_pose3d_can(scoremap_pooled, hand_side, dropout=drop)
+            R, out = _train_rotate(can, _train_viewpoint_u(scoremap_pooled, hand_side, dropout=drop), hand_side)
+            r = out, can, R
         else:
             assert 0, "Unknown variant."
+        _train_advance(drop)
+        return r

@@ -56,6 +56,9 @@ class Context:
         self._ws = None
         self._ws_key = (0, 0, 0)
         self.weights = {}
+        self.dropout_seed = None     # set_dropout()
+        self._dropout_on = False     # the C-level switch, turned per call by _dropout_mode()
+        self._draw = None
         self.set_precision(precision)
 
     def __del__(self):
@@ -85,6 +88,80 @@ class Context:
         """Kernel-selection switch (process-wide, see include/hand3d_b200.h: h3d_set_tuning); drops this context's plans."""
         self._no_live_graphs("set_tuning()")
         _lib.check(self.lib.h3d_set_tuning(self.h, key.encode(), int(value)), "h3d_set_tuning(%s)" % key)
+
+    # ---- dropout (evaluation=False in the lifting stage; include/hand3d_b200.h: H3D_DROPOUT_*) ---------------------------
+    def set_dropout(self, seed):
+        """Seeds the context's dropout generator and sets its draw counter to 0; None turns dropout off again.  Only calls that ask for
+        dropout apply it (evaluation=False, or dropout=True here); every other call computes what it computes without a seed."""
+        if seed is None:
+            self._dropout_mode(False)
+            self.dropout_seed = None
+            return
+        seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        _lib.check(self.lib.h3d_set_dropout(self.h, 1, C.c_uint64(seed)), "h3d_set_dropout")
+        self._dropout_on = True
+        self.dropout_seed = seed
+        self._draw_counter().zero_()          # the same seed again restarts its stream as well
+
+    def _dropout_mode(self, on):
+        if on and self.dropout_seed is None:
+            raise NotImplementedError("evaluation=False applies dropout, which needs a seeded generator: call set_dropout(seed) on the "
+                                      "context (runtime.default_context()) first")
+        if bool(on) != self._dropout_on:
+            _lib.check(self.lib.h3d_set_dropout(self.h, int(bool(on)), C.c_uint64(self.dropout_seed or 0)), "h3d_set_dropout")
+            self._dropout_on = bool(on)
+
+    def _draw_counter(self):
+        """The int64 [1] draw counter in the context's device memory (an alias, not a copy)."""
+        if self._draw is None:
+            p = C.c_void_p()
+            _lib.check(self.lib.h3d_dropout_draw(self.h, C.byref(p)), "h3d_dropout_draw")
+
+            class _Counter:
+                __cuda_array_interface__ = {"shape": (1,), "typestr": "<i8", "data": (p.value, False), "version": 2}
+            self._draw = torch.as_tensor(_Counter(), device=self.device)
+        return self._draw
+
+    def dropout_state(self):
+        """A device copy (int64 [1]) of the draw counter, enqueued on the current stream: pass it to load_dropout_state() to replay
+        the same masks."""
+        return self._draw_counter().clone()
+
+    def load_dropout_state(self, state):
+        """Sets the draw counter from dropout_state()'s tensor or an int."""
+        d = self._draw_counter()
+        if torch.is_tensor(state):
+            d.copy_(state.reshape(1))
+        else:
+            d.fill_(int(state))
+
+    def dropout_forward(self, x, keep_prob, layer):
+        """TF 1.3 dropout of x [rows, ...] fp32 at the current draw (row = index along dim 0) -> (y, keep uint8), without advancing."""
+        x = _chk_f32(x, "x")
+        if x.dim() < 1 or x.numel() == 0:
+            raise ValueError("dropout needs a non-empty tensor")
+        self._dropout_mode(True)
+        y = torch.empty_like(x)
+        keep = torch.empty(x.shape, dtype=torch.uint8, device=x.device)
+        _lib.check(self.lib.h3d_dropout_forward(self.h, _ptr(x), x.shape[0], x.numel() // x.shape[0], float(keep_prob), int(layer), _ptr(y),
+                                                _ptr(keep), _stream()), "h3d_dropout_forward")
+        return y, keep
+
+    def dropout_backward(self, dy, keep, keep_prob):
+        """dx = (dy * keep) / keep_prob."""
+        dy = _chk_f32(dy, "dy")
+        if keep.dtype != torch.uint8 or keep.shape != dy.shape or keep.device != dy.device:
+            raise ValueError("keep must be a uint8 tensor shaped like dy on its device")
+        self._dropout_mode(True)
+        dx = torch.empty_like(dy)
+        _lib.check(self.lib.h3d_dropout_backward(self.h, _ptr(dy), _ptr(keep.contiguous()), dy.shape[0], dy.numel() // dy.shape[0],
+                                                 float(keep_prob), _ptr(dx), _stream()), "h3d_dropout_backward")
+        return dx
+
+    def dropout_advance(self):
+        """Adds 1 to the draw counter on the device."""
+        self._dropout_mode(True)
+        _lib.check(self.lib.h3d_dropout_advance(self.h, _stream()), "h3d_dropout_advance")
 
     @property
     def launch_count(self):
@@ -187,7 +264,9 @@ class Context:
         _lib.check(self.lib.h3d_pose2d_forward(self.h, _ptr(image_crop), B, H, W, _ptr(sm), _ptr(uv), _stream()), "h3d_pose2d_forward")
         return {"keypoints_scoremap": sm, "keypoints_uv": uv}
 
-    def lifting(self, scoremap32, hand_side, variant="proposed"):
+    def lifting(self, scoremap32, hand_side, variant="proposed", dropout=False):
+        """PosePrior (+ ViewpointNet): [B,32,32,21], [B,2] -> (out, can, R).  dropout=True (evaluation=False) applies the four dropout
+        layers at the current draw and advances it; it needs set_dropout()."""
         scoremap32 = _chk_f32(scoremap32, "scoremap", 4)
         hand_side = _chk_f32(hand_side, "hand_side", 2)
         B = scoremap32.shape[0]
@@ -199,14 +278,16 @@ class Context:
         can = torch.empty((B, 21, 3), dtype=torch.float32, device=dev)
         v = VARIANTS[variant]
         rot = torch.empty((B, 3, 3), dtype=torch.float32, device=dev) if variant == "proposed" else None
+        self._dropout_mode(dropout)
         _lib.check(self.lib.h3d_lifting_forward(self.h, _ptr(scoremap32), _ptr(hand_side), B, v, _ptr(out), _ptr(can), _ptr(rot),
                                                 _stream()), "h3d_lifting_forward")
         return out, can, rot
 
     def pipeline(self, image, hand_side=None, with_pose3d=True, force_center=None, force_scale=None, want_mask=False,
-                 outputs="all"):
+                 outputs="all", dropout=False):
         """ColorHandPose3DNetwork.inference / inference2d + detect_keypoints.  outputs="all" materialises the
-        reference's large tensors; outputs="keypoints" keeps them in the workspace (serving mode)."""
+        reference's large tensors; outputs="keypoints" keeps them in the workspace (serving mode).  dropout=True: the lifting as in
+        lifting(dropout=True)."""
         image = _chk_f32(image, "image", 4)
         B, H, W, _ = image.shape
         dev = image.device
@@ -227,6 +308,7 @@ class Context:
         }
         fc = _chk_f32(force_center, "force_center") if force_center is not None else None
         fs = _chk_f32(force_scale, "force_scale") if force_scale is not None else None
+        self._dropout_mode(dropout)
         _lib.check(self.lib.h3d_pipeline_forward(
             self.h, _ptr(image), _ptr(hand_side if with_pose3d else None), B, H, W, int(bool(with_pose3d)), _ptr(fc), _ptr(fs),
             _ptr(r["hand_scoremap"]), _ptr(r["image_crop"]), _ptr(r["scale_crop"]), _ptr(r["center"]),
@@ -256,13 +338,14 @@ class Context:
         """Declares every graph returned by capture_pipeline() dead (the caller must drop them); the workspace may grow again."""
         self._graphs_captured = 0
 
-    def track_step(self, image, hand_side, state, detect, margin=1.5, min_score=None, outputs="all", with_pose3d=True):
+    def track_step(self, image, hand_side, state, detect, margin=1.5, min_score=None, outputs="all", with_pose3d=True, dropout=False):
         """One step of a tracked stream per batch slot (h3d_track_step, DESIGN.md section 4.14).  detect=True runs pipeline() (no
         forced crop); detect=False crops at state.center / state.scale and skips HandSegNet and the mask post-processing.  Either way
         the step then updates `state` (a TrackState of the same batch) from its key-points: the next crop, the score and the lost
         flag.  min_score None turns the score test off.  Returns image_crop, scale_crop, center (the crop this step used),
         keypoints_scoremap, keypoint_coord3d and keypoints_uv as pipeline() does; outputs="keypoints" leaves the large ones in the
-        workspace.  Enqueue-only: a call on fixed tensors can be captured into a CUDA graph."""
+        workspace.  dropout=True: the lifting as in lifting(dropout=True).  Enqueue-only: a call on fixed tensors can be captured into a
+        CUDA graph."""
         image = _chk_f32(image, "image", 4)
         B, H, W, _ = image.shape
         dev = image.device
@@ -281,6 +364,7 @@ class Context:
             "keypoint_coord3d": torch.empty((B, 21, 3), **f32) if with_pose3d else None,
             "keypoints_uv": torch.empty((B, 21, 2), dtype=torch.int32, device=dev),
         }
+        self._dropout_mode(dropout)
         _lib.check(self.lib.h3d_track_step(
             self.h, _ptr(image), _ptr(hand_side if with_pose3d else None), B, H, W, int(bool(with_pose3d)), int(bool(detect)),
             float(margin), float("nan") if min_score is None else float(min_score), _ptr(state.buffer),
@@ -288,7 +372,8 @@ class Context:
             _ptr(r["keypoint_coord3d"]), _ptr(r["keypoints_uv"]), _stream()), "h3d_track_step")
         return r
 
-    def track_step_slots(self, image, hand_side, state, force=None, margin=1.5, min_score=None, outputs="all", with_pose3d=True):
+    def track_step_slots(self, image, hand_side, state, force=None, margin=1.5, min_score=None, outputs="all", with_pose3d=True,
+                         dropout=False):
         """A track step that re-detects only the slots that need it (h3d_track_step_slots, DESIGN.md section 4.15): slot b runs
         HandSegNet and the mask post-processing when state.lost[b] (from the previous step) or force[b] (optional CUDA int32 or bool [B])
         is set, and is cropped from the state otherwise.  The choice is made on the device: nothing is read back.  Returns track_step's
@@ -319,6 +404,7 @@ class Context:
             "keypoints_uv": torch.empty((B, 21, 2), dtype=torch.int32, device=dev),
         }
         detected = torch.empty(B, dtype=torch.int32, device=dev)
+        self._dropout_mode(dropout)
         _lib.check(self.lib.h3d_track_step_slots(
             self.h, _ptr(image), _ptr(hand_side if with_pose3d else None), B, H, W, int(bool(with_pose3d)),
             float(margin), float("nan") if min_score is None else float(min_score), _ptr(state.buffer), _ptr(force), _ptr(detected),

@@ -16,7 +16,7 @@ import contextlib
 import numpy as np
 import torch
 
-from .. import _lib, runtime
+from .. import _lib, autograd as A, runtime
 
 _scope_stack = []
 
@@ -77,10 +77,20 @@ class NetworkOps(object):
 
     @staticmethod
     def dropout(in_tensor, keep_prob, evaluation):
-        """Identity at evaluation time (utils/general.py:139-148); training is out of scope."""
-        if not bool(evaluation):
-            raise NotImplementedError("hand3d_b200 implements the forward pass only (evaluation must be True)")
-        return in_tensor
+        """utils/general.py:139-148: the identity at evaluation time; evaluation=False applies TF 1.3 dropout (y = (x / keep_prob) * k,
+        differentiable) at the default context's current draw with layer id H3D_DROPOUT_LAYER_OP, then advances the draw.  That needs a
+        seeded context (runtime.default_context().set_dropout(seed)).  keep_prob == 1 returns the input, as TF does."""
+        ev = bool(evaluation.item()) if torch.is_tensor(evaluation) else bool(evaluation)
+        if ev:
+            return in_tensor
+        kp = float(keep_prob.item()) if torch.is_tensor(keep_prob) else float(keep_prob)
+        ctx = runtime.default_context()
+        ctx._dropout_mode(True)
+        if kp == 1.0:
+            return in_tensor
+        y = A.dropout(in_tensor, kp, _lib.DROPOUT_LAYER_OP)
+        ctx.dropout_advance()
+        return y
 
 
 def crop_image_from_xy(image, crop_location, crop_size, scale=1.0):

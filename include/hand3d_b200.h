@@ -578,6 +578,47 @@ H3D_API int h3d_mse_loss_forward(h3d_ctx* ctx, const float* pred, const float* t
 H3D_API int h3d_mse_loss_backward(h3d_ctx* ctx, const float* pred, const float* target, const float* grad_loss, int64_t n, float* dpred,
                                   void* stream);
 
+/* ---- Dropout of the lifting stage (ops.dropout, utils/general.py:139-148: evaluation = False) ----
+ * TF 1.3's tf.nn.dropout in fp32: keep bit k = floor(keep_prob + u), y = (x / keep_prob) * k (a rounded division, then a rounded
+ * multiply), and the gradient dx = (dy * k) / keep_prob (TF's Mul gradient, then its RealDiv gradient).  keep_prob == 1 keeps every
+ * element and returns x bit for bit.
+ * Draws are the project's own, not TF's streams: Philox4x64-10 (as for the reader) keyed (seed, H3D_DROPOUT_STREAM), counter
+ * (draw, layer, row, col / 4); element (row, col) takes word col mod 4 and u = (w >> 40) 2^-24 (exact in fp32).
+ * Layers: H3D_DROPOUT_LAYER_FC_REL0 / _FC_REL1 (PosePrior, keep 0.8, nets/PosePriorNetwork.py:113-114), _FC_VP0 / _FC_VP1 (ViewpointNet,
+ * keep 0.75, :151-154); NetworkOps.dropout uses H3D_DROPOUT_LAYER_OP.  row is the sample's index in the batch.
+ * One generator per context: a seed and the int64 `draw` counter in context-owned device memory.  Every dropout kernel reads draw on
+ * the device, and the advance kernel adds 1 to it there, so a captured graph draws fresh masks on every replay and the host never reads
+ * the counter. */
+#define H3D_DROPOUT_STREAM 2
+#define H3D_DROPOUT_LAYER_FC_REL0 0
+#define H3D_DROPOUT_LAYER_FC_REL1 1
+#define H3D_DROPOUT_LAYER_FC_VP0 2
+#define H3D_DROPOUT_LAYER_FC_VP1 3
+#define H3D_DROPOUT_LAYER_OP 4
+/* enabled != 0: dropout on with `seed`; draw is set to 0 on the first enabling and whenever the seed changes (a synchronous write: not
+ * while a stream is being captured).  enabled == 0: off (the default); seed and draw are kept, so enabling again with the same seed
+ * continues the stream.  While it is on, every lifting computation of the context (h3d_lifting_forward, h3d_pipeline_forward with
+ * with_pose3d, h3d_track_step, h3d_track_step_slots) applies the four layers above after the hidden FC layers, layer by layer, and then
+ * adds 1 to draw: one forward is one draw.  Off, they compute exactly what they compute without this entry.  The context keeps one plan
+ * for each setting, so switching between calls rebuilds nothing. */
+H3D_API int h3d_set_dropout(h3d_ctx* ctx, int enabled, uint64_t seed);
+/* *draw = the device address of the counter (int64), so that a caller can save and restore the stream. */
+H3D_API int h3d_dropout_draw(h3d_ctx* ctx, int64_t** draw);
+/* x [rows, cols] fp32 (device) -> y [rows, cols] fp32 (may be x) and keep [rows, cols] uint8 (0 / 1; may be NULL) at the current draw.
+ * Does not advance the draw.  0 < keep_prob <= 1, rows, cols >= 1, layer >= 0 and dropout enabled, else H3D_EINVAL with nothing
+ * enqueued.  These entries only enqueue: no allocation, no synchronisation (capturable). */
+H3D_API int h3d_dropout_forward(h3d_ctx* ctx, const float* x, int rows, int cols, float keep_prob, int layer, float* y, uint8_t* keep,
+                                void* stream);
+/* The same, also writing the 16-bit planes a tensor-core FC layer reads: hi = h16(y), lo = h16(y - hi) (lo may be NULL), [rows, stride]
+ * with stride >= cols and zeros in the columns [cols, stride); h16 is bf16 (half = 0) or fp16 (half = 1), round to nearest even. */
+H3D_API int h3d_dropout_forward_planes(h3d_ctx* ctx, const float* x, int rows, int cols, float keep_prob, int layer, float* y, uint8_t* keep,
+                                       int half, int stride, uint16_t* hi, uint16_t* lo, void* stream);
+/* dy, keep [rows, cols] -> dx = (dy * keep) / keep_prob (may be dy); the same argument rules. */
+H3D_API int h3d_dropout_backward(h3d_ctx* ctx, const float* dy, const uint8_t* keep, int rows, int cols, float keep_prob, float* dx,
+                                 void* stream);
+/* Adds 1 to draw on the device (one kernel). */
+H3D_API int h3d_dropout_advance(h3d_ctx* ctx, void* stream);
+
 /* ---- drawing (utils/general.py:360-477, plot_hand / plot_hand_3d: the stick figures run.py shows)
  * Draws S anti-aliased segments into each of B uint8 RGB images [B,H,W,3] (device, contiguous), in place.  segments [B,S,4] float32
  * (device): (r0, c0, r1, c1) in pixels, pixel (y, x) centred at (y, x).  host_colors [S,3] float32 (HOST, 0..255) are copied into the
