@@ -14,6 +14,9 @@ LIB_PATH = os.path.join(HERE, "libhand3d_b200.so")
 OK, EINVAL, ENODEVICE, ECUDA, EWEIGHTS, EWORKSPACE = 0, -1, -2, -3, -4, -5
 PREC_FP32_FFMA, PREC_BF16X3, PREC_FP16X3, PREC_FP16, PREC_BF16 = 0, 1, 2, 3, 4
 PRECISIONS = {"fp32_ffma": 0, "bf16x3": 1, "fp16x3": 2, "fp16": 3, "bf16": 4, "fp16_f8c": 5}
+# kernels of the CUDA-core convolution (H3D_DIRECT_*) and the split-K scratch the entries give it (H3D_CONV_SPLITK_SCRATCH_FLOATS)
+DIRECT_KERNELS = {0: "c3_tc", 1: "c3_ffma", 2: "vec", 3: "scalar"}
+CONV_SPLITK_SCRATCH_FLOATS = 600 * 64 * 64
 VARIANTS = {"direct": 0, "bottleneck": 1, "proposed": 2, "local": 3, "local_w_xyz_loss": 3}
 
 _p, _i, _i64, _f = C.c_void_p, C.c_int, C.c_int64, C.c_float
@@ -57,10 +60,12 @@ SIGNATURES = {
     "h3d_conv2d_layer_planes": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _i, _i, _i, _p, _i, _i, _i, _i, _p, _p, _p, _p, _i, _i, _p, _i, _i, _p]),
     "h3d_conv2d_tc_geometry": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(_i)]),
     "h3d_conv2d_wgrad_geometry": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(_i)]),
+    "h3d_conv2d_f32_geometry": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i64, C.POINTER(_i)]),
     "h3d_leaky_relu_f32": (_i, [_p, _p, _p, _i64, _p]),
     "h3d_maxpool2x2_f32": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),
     "h3d_maxpool2x2_backward_f32": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _p]),
     "h3d_fully_connected_f32": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _p]),
+    "h3d_fully_connected_f32_geometry": (_i, [_i, _i, _i, C.POINTER(_i)]),
     "h3d_resize_bilinear_tf1": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _i, _p]),
     "h3d_avgpool8": (_i, [_p, _p, _p, _i, _i, _i, _i, _p]),
     "h3d_seg_postprocess": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _p, _p, _p]),

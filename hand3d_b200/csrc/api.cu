@@ -1709,6 +1709,42 @@ int h3d_conv2d_wgrad_geometry(int B, int H, int W, int ksize, int Cin, int Cout,
     return H3D_OK;
 }
 
+int h3d_conv2d_f32_geometry(int B, int H, int W, int Cin, int Cin_total, int cin_off, int Cout, int Cout_total, int cout_off, int yf,
+                            int planes, int Cs_total, int cs_off, int ksize, int stride, int x_aligned, int64_t splitk_scratch_floats,
+                            int* out) {
+    H3D_REQUIRE(out && B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && ksize > 0 && stride > 0 && splitk_scratch_floats >= 0,
+                "h3d_conv2d_f32_geometry: bad argument");
+    H3D_REQUIRE(cin_off >= 0 && Cin_total >= cin_off + Cin, "h3d_conv2d_f32_geometry: input channels outside x");
+    H3D_REQUIRE(planes >= H3D_PREC_FP32_FFMA && planes <= H3D_PREC_FP16_F8C, "h3d_conv2d_f32_geometry: planes must be a precision mode");
+    H3D_REQUIRE(yf || planes != H3D_PREC_FP32_FFMA, "h3d_conv2d_f32_geometry: no output requested");
+    H3D_REQUIRE(!yf || (cout_off >= 0 && Cout_total >= cout_off + Cout), "h3d_conv2d_f32_geometry: output channels outside y");
+    H3D_REQUIRE(planes == H3D_PREC_FP32_FFMA || (cs_off >= 0 && Cs_total >= cs_off + Cout),
+                "h3d_conv2d_f32_geometry: output channels outside the planes");
+    // the choosers test these pointers for NULL (and x for its alignment) and never dereference them
+    alignas(16) static float probe[4];
+    const int passes = planes == H3D_PREC_FP32_FFMA ? 0 : passes_of(planes);
+    DirectConvArgs a;
+    a.x = x_aligned ? probe : probe + 1; a.Cin_total = Cin_total; a.cin_off = cin_off; a.w = probe; a.bias = probe;
+    a.y = yf ? probe : nullptr; a.Cout_total = Cout_total; a.cout_off = cout_off;
+    a.ys = Split();
+    if (passes) {
+        a.ys.hi = (uint16_t*)probe;
+        if (passes == 3) a.ys.lo = (uint16_t*)probe;
+        if (passes == 4) { a.ys.l8 = (uint8_t*)probe; a.ys.h8 = (uint8_t*)probe; }
+    }
+    a.Cs_total = Cs_total; a.cs_off = cs_off; a.half = passes ? half_of(planes) : Half16::BF16;
+    a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.k = ksize; a.stride = stride; a.leaky = 0;
+    a.splitk_scratch = splitk_scratch_floats ? probe : nullptr; a.splitk_scratch_floats = splitk_scratch_floats;
+    conv_direct_geometry(a, out);
+    return H3D_OK;
+}
+
+int h3d_fully_connected_f32_geometry(int B, int in_features, int out_features, int* out) {
+    H3D_REQUIRE(out && B > 0 && in_features > 0 && out_features > 0, "h3d_fully_connected_f32_geometry: bad argument");
+    fc_geometry(B, in_features, out_features, out);
+    return H3D_OK;
+}
+
 int h3d_conv2d_tc(h3d_ctx* ctx, const float* x, const float* host_w_hwio, const float* host_bias, float* y, int B, int H, int W,
                   int Cin, int Cout, int ksize, int leaky, int precision, void* stream) {
     return h3d_conv2d_tc_strided(ctx, x, host_w_hwio, host_bias, y, B, H, W, Cin, Cout, ksize, 1, leaky, precision, stream);

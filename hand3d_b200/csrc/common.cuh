@@ -218,12 +218,15 @@ struct DirectConvArgs {
     const int* count = nullptr;
     const int* slots = nullptr;
 };
-constexpr int64_t kConvSplitKScratchFloats = 600ll * 64 * 64;   // upper bound used by launch_conv_direct's split-K policy
+constexpr int64_t kConvSplitKScratchFloats = H3D_CONV_SPLITK_SCRATCH_FLOATS;   // upper bound used by launch_conv_direct's split-K policy
 int launch_conv_direct(const DirectConvArgs& a, cudaStream_t s);
 int conv_direct_num_launches(const DirectConvArgs& a);   // 1, or 2 when the split-K policy applies
+// out[6] of h3d_conv2d_f32_geometry for a (host only: the pointers of a are only tested for NULL and x for its alignment)
+void conv_direct_geometry(const DirectConvArgs& a, int* out);
 // scratch: fc_scratch_floats(B, in_f, out_f) floats (split-K partial sums); two kernels per call.  scratch_floats is the capacity
 // of the scratch buffer: a call that would need more returns H3D_EINVAL and launches nothing.
 int64_t fc_scratch_floats(int B, int in_f, int out_f);
+void fc_geometry(int B, int in_f, int out_f, int* out);   // out[5] of h3d_fully_connected_f32_geometry
 int launch_fc(const float* x, const float* w, const float* bias, float* y, float* scratch, int64_t scratch_floats, int B, int in_f,
               int out_f, int leaky, int x_stride, cudaStream_t s);
 // gathers [conv_feat(b, :feat) , hand_side(b, :2)] -> xcat [B, feat+2]

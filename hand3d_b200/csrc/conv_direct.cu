@@ -346,6 +346,16 @@ static void plan_direct(const DirectConvArgs& a, ConvGeom* gp, dim3* gridp, int*
     *gridp = grid; *ksplitp = ksplit;
 }
 
+// The kernel launch_conv_direct runs (H3D_DIRECT_*).
+static int direct_kernel(const DirectConvArgs& a) {
+    if (is_c3_case(a))   // split planes only (not fp16_f8c): the tensor-core version
+        return !a.y && a.ys.hi && !a.ys.l8 && !tc_tuning().c3_ffma ? H3D_DIRECT_C3_TC : H3D_DIRECT_C3_FFMA;
+    const bool vec = (a.Cin % KC == 0) && (a.Cin_total % 4 == 0) && (a.cin_off % 4 == 0) && (((uintptr_t)a.x & 15) == 0);
+    return vec ? H3D_DIRECT_VEC : H3D_DIRECT_SCALAR;
+}
+
+static int c3_ctas(const DirectConvArgs& a) { return ceil_div(ceil_div(a.W, C3_TW) * ceil_div(a.H, C3_TH) * a.B, C3_TILES_PER_CTA); }
+
 int conv_direct_num_launches(const DirectConvArgs& a) {
     if (is_c3_case(a)) return 1;
     ConvGeom g; dim3 grid; int ksplit;
@@ -353,12 +363,26 @@ int conv_direct_num_launches(const DirectConvArgs& a) {
     return ksplit > 1 ? 2 : 1;
 }
 
+void conv_direct_geometry(const DirectConvArgs& a, int* out) {
+    const int kernel = direct_kernel(a);
+    out[0] = kernel;
+    if (kernel == H3D_DIRECT_C3_TC || kernel == H3D_DIRECT_C3_FFMA) {
+        const int ctas = kernel == H3D_DIRECT_C3_FFMA ? c3_ctas(a) : 0;
+        out[1] = ctas; out[2] = out[3] = ctas ? 1 : 0; out[4] = 1; out[5] = 27;
+        return;
+    }
+    ConvGeom g; dim3 grid; int ksplit;
+    plan_direct(a, &g, &grid, &ksplit);
+    out[1] = (int)grid.x; out[2] = (int)grid.y; out[3] = (int)grid.z; out[4] = ksplit; out[5] = g.k_per_split;
+}
+
 int launch_conv_direct(const DirectConvArgs& a, cudaStream_t s) {
     H3D_REQUIRE(a.k >= 1 && a.stride >= 1 && a.Cin >= 1 && a.Cout >= 1, "conv_direct: bad geometry");
-    if (is_c3_case(a) && !a.y && a.ys.hi && !a.ys.l8 && !tc_tuning().c3_ffma)   // split planes only: tensor-core version
+    const int kernel = direct_kernel(a);
+    if (kernel == H3D_DIRECT_C3_TC)
         return launch_conv_c3_tc(a.x, a.w, a.bias, a.ys, a.Cs_total, a.cs_off, a.B, a.H, a.W, a.leaky, a.half, s, a.err_flag, a.count, a.slots);
-    if (is_c3_case(a)) {
-        const int tiles = ceil_div(ceil_div(a.W, C3_TW) * ceil_div(a.H, C3_TH) * a.B, C3_TILES_PER_CTA);
+    if (kernel == H3D_DIRECT_C3_FFMA) {
+        const int tiles = c3_ctas(a);
         if (a.half == Half16::FP16)
             conv3x3_c3_kernel<true><<<tiles, 256, 0, s>>>(a.x, a.w, a.bias, a.y, a.ys.hi, a.ys.lo, a.ys.l8, a.ys.h8, a.B, a.H, a.W, a.Cout_total, a.cout_off, a.Cs_total, a.cs_off, a.leaky, a.count, a.slots);
         else
@@ -369,7 +393,7 @@ int launch_conv_direct(const DirectConvArgs& a, cudaStream_t s) {
     ConvGeom g; dim3 grid; int ksplit;
     plan_direct(a, &g, &grid, &ksplit);
     const int64_t M = (int64_t)g.B * g.Ho * g.Wo;
-    const bool vec = (a.Cin % KC == 0) && (a.Cin_total % 4 == 0) && (a.cin_off % 4 == 0) && (((uintptr_t)a.x & 15) == 0);
+    const bool vec = kernel == H3D_DIRECT_VEC;
     const bool fp16 = a.half == Half16::FP16;
 #define LAUNCH(V, F) conv_direct_kernel<V, F><<<grid, 256, 0, s>>>(a.x, a.w, a.bias, a.y, a.ys.hi, a.ys.lo, g)
     if (vec) { if (fp16) LAUNCH(true, true); else LAUNCH(true, false); }
@@ -448,13 +472,18 @@ int fc_ksplit(int B, int in_f, int out_f) {
     return ks;
 }
 int64_t fc_scratch_floats(int B, int in_f, int out_f) { return (int64_t)fc_ksplit(B, in_f, out_f) * B * out_f; }
+static int fc_k_per_split(int in_f, int ksplit) { return (int)align_up(ceil_div(in_f, ksplit), FCK); }
+void fc_geometry(int B, int in_f, int out_f, int* out) {
+    const int ksplit = fc_ksplit(B, in_f, out_f);
+    out[0] = ksplit; out[1] = fc_k_per_split(in_f, ksplit); out[2] = ceil_div(out_f, FCN); out[3] = ksplit; out[4] = ceil_div(B, FCB);
+}
 
 int launch_fc(const float* x, const float* w, const float* bias, float* y, float* scratch, int64_t scratch_floats, int B, int in_f,
               int out_f, int leaky, int x_stride, cudaStream_t s) {
     const int ksplit = fc_ksplit(B, in_f, out_f);
     H3D_REQUIRE((int64_t)ksplit * B * out_f <= scratch_floats, "fully_connected %d -> %d at B=%d: split-K needs %lld scratch floats, have %lld",
                 in_f, out_f, B, (long long)ksplit * B * out_f, (long long)scratch_floats);
-    const int k_per_split = (int)align_up(ceil_div(in_f, ksplit), FCK);
+    const int k_per_split = fc_k_per_split(in_f, ksplit);
     dim3 grid(ceil_div(out_f, FCN), ksplit, ceil_div(B, FCB));
     fc_splitk_kernel<<<grid, 256, 0, s>>>(x, w, scratch, B, in_f, out_f, x_stride, k_per_split);
     H3D_CHECK_LAUNCH();

@@ -1160,6 +1160,25 @@ def conv2d_wgrad_geometry(B, H, W, ksize, Cin, Cout):
     return tuple(out)
 
 
+def conv2d_f32_geometry(B, H, W, Cin, Cout, ksize, stride=1, Cin_total=None, cin_off=0, Cout_total=None, cout_off=0, yf=True,
+                        planes=None, Cs_total=None, cs_off=0, x_aligned=True, splitk_scratch_floats=_lib.CONV_SPLITK_SCRATCH_FLOATS):
+    """(kernel, (grid x, y, z), ksplit, k_per_split) of the CUDA-core convolution (h3d_conv2d_f32_geometry): kernel is one of
+    "c3_tc", "c3_ffma", "vec", "scalar"; planes a tensor-core precision or None.  Needs no device."""
+    out = (C.c_int * 6)()
+    _lib.check(_lib.load().h3d_conv2d_f32_geometry(
+        B, H, W, Cin, Cin if Cin_total is None else Cin_total, cin_off, Cout, Cout if Cout_total is None else Cout_total, cout_off,
+        int(bool(yf)), PRECISIONS[planes or "fp32_ffma"], Cout if Cs_total is None else Cs_total, cs_off, ksize, stride, int(bool(x_aligned)),
+        int(splitk_scratch_floats), out), "h3d_conv2d_f32_geometry")
+    return _lib.DIRECT_KERNELS[out[0]], tuple(out[1:4]), out[4], out[5]
+
+
+def fully_connected_f32_geometry(B, in_features, out_features):
+    """(ksplit, k_per_split, (grid x, y, z)) of the fp32 fully connected layer (h3d_fully_connected_f32_geometry).  Needs no device."""
+    out = (C.c_int * 5)()
+    _lib.check(_lib.load().h3d_fully_connected_f32_geometry(B, in_features, out_features, out), "h3d_fully_connected_f32_geometry")
+    return out[0], out[1], tuple(out[2:5])
+
+
 _default = {}
 
 

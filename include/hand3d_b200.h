@@ -275,6 +275,24 @@ H3D_API int h3d_conv2d_tc_geometry(int B, int H, int W, int Cout, int pool, int 
  * out[6] = TW, TH, TB (a 64-pixel box), BN (64 or 128 input channels per tile), num_tiles (ksize^2 x Cout tiles x Cin tiles) and
  * splits (CTAs that share one tile's pixel blocks). */
 H3D_API int h3d_conv2d_wgrad_geometry(int B, int H, int W, int ksize, int Cin, int Cout, int* out);
+/* The kernels of the fp32 CUDA-core convolution (h3d_conv2d_f32, and route 1 of h3d_conv2d_layer_planes): */
+#define H3D_DIRECT_C3_TC 0      /* first layer (3x3, 3 -> 64, stride 1) on the tensor cores, planes only */
+#define H3D_DIRECT_C3_FFMA 1    /* first layer on the register-tiled FFMA kernel */
+#define H3D_DIRECT_VEC 2        /* generic kernel, float4 gathers (Cin % 16 == 0, 16-byte aligned input channels) */
+#define H3D_DIRECT_SCALAR 3     /* generic kernel, scalar gathers */
+/* Split-K scratch (floats) the library's entries give the generic kernel. */
+#define H3D_CONV_SPLITK_SCRATCH_FLOATS (600LL * 64 * 64)
+/* Which kernel, grid and split of K the CUDA-core convolution runs a layer on, from the launcher's own choosers (host only, like
+ * h3d_conv2d_tc_geometry).  The layer reads channels [cin_off, cin_off + Cin) of x [B,H,W,Cin_total]; x_aligned says whether those
+ * channels start 16 bytes aligned.  It writes fp32 output when yf != 0 (Cout channels at cout_off of Cout_total) and/or the planes of
+ * precision `planes` (a tensor-core mode, H3D_PREC_FP32_FFMA = none; Cout channels at cs_off of Cs_total).  splitk_scratch_floats is
+ * the split-K scratch offered (0 = none; h3d_conv2d_f32 offers H3D_CONV_SPLITK_SCRATCH_FLOATS when B ceil(H/s) ceil(W/s) <= 64 x 295,
+ * the stage entries always), under the current "c3_ffma" tuning.  out[6] = kernel (H3D_DIRECT_*), grid x, y, z, ksplit (2 launches when
+ * > 1: the partial sums, then their fixed-order reduction) and k_per_split (reduction rows per blockIdx.z).  The first-layer kernels
+ * do not split K (k_per_split = 27); the grid of H3D_DIRECT_C3_TC depends on the device's SM count and is reported as 0 x 0 x 0. */
+H3D_API int h3d_conv2d_f32_geometry(int B, int H, int W, int Cin, int Cin_total, int cin_off, int Cout, int Cout_total, int cout_off,
+                                    int yf, int planes, int Cs_total, int cs_off, int ksize, int stride, int x_aligned,
+                                    int64_t splitk_scratch_floats, int* out);
 /* NetworkOps.leaky_relu (utils/general.py:31-33): y = max(x, 0.01 x), n elements, 16-byte aligned pointers. */
 H3D_API int h3d_leaky_relu_f32(h3d_ctx* ctx, const float* x, float* y, int64_t n, void* stream);
 /* NetworkOps.max_pool (utils/general.py:62-65): 2x2 / 2 VALID. */
@@ -285,6 +303,9 @@ H3D_API int h3d_maxpool2x2_backward_f32(h3d_ctx* ctx, const float* x, const floa
 /* NetworkOps.fully_connected(_relu) (utils/general.py:113-136): y = x[B,in] @ w[in,out] + b. */
 H3D_API int h3d_fully_connected_f32(h3d_ctx* ctx, const float* x, const float* w, const float* bias, float* y,
                             int B, int in_features, int out_features, int leaky, void* stream);
+/* Its split of K, from the launcher's own chooser (host only): out[5] = ksplit, k_per_split, grid x (64-output tiles), y (= ksplit),
+ * z (32-row batch tiles).  Every call is two launches: the partial sums, then their fixed-order reduction. */
+H3D_API int h3d_fully_connected_f32_geometry(int B, int in_features, int out_features, int* out);
 /* tf.image.resize_images bilinear, align_corners=False, TF1 legacy (nets/...:97,128,166). */
 H3D_API int h3d_resize_bilinear_tf1(h3d_ctx* ctx, const float* x, float* y, int B, int H, int W, int C,
                             int out_h, int out_w, void* stream);
