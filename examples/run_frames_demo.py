@@ -2,7 +2,10 @@
 (run.py:57-59), then goes through ColorHandPose3DNetwork.inference; key-points come back in frame pixels.
 
     python examples/run_frames_demo.py                      # seeded synthetic 1080p frames, synthetic weights
-    python examples/run_frames_demo.py --video clip.mp4     # decoded with OpenCV (BGR -> RGB)
+    python examples/run_frames_demo.py --video clip.mp4     # decoded with OpenCV; its BGR frames go in as they are
+    python examples/run_frames_demo.py --raw-video clip.nv12 --pixel-format nv12 --height 1080 --width 1920
+                                                            # concatenated raw frames, as ffmpeg -f rawvideo -pix_fmt nv12 (or
+                                                            # yuv420p -> i420, yuyv422 -> yuyv) writes them
     python examples/run_frames_demo.py --weights weights/   # the reference's pickled weights
     python examples/run_frames_demo.py --track --draw-dir out   # also writes the frames of the first batch with the skeleton and
                                                                 # the crop square drawn on the device (PNG, Pillow)
@@ -32,16 +35,32 @@ def video_batches(path, B, max_batches):
         ok, bgr = cap.read()
         if not ok:
             break
-        batch.append(cv2.cvtColor(bgr, cv2.COLOR_BGR2RGB))
+        batch.append(bgr)                   # FrameRunner(pixel_format="bgr") converts on the device
         if len(batch) == B:
             yield np.stack(batch)
             batch, n = [], n + 1
     cap.release()
 
 
+def raw_video_batches(path, pixel_format, B, H, W, max_batches):
+    """Concatenated raw frames of frame_shape(pixel_format, H, W), read through a memory map (a trailing partial batch is dropped)."""
+    from hand3d_b200.frames import frame_shape
+    shape = frame_shape(pixel_format, H, W)
+    frame_bytes = int(np.prod(shape))
+    n = os.path.getsize(path) // frame_bytes
+    if n == 0:
+        return
+    frames = np.memmap(path, dtype=np.uint8, mode="r", shape=(n,) + shape)
+    for i in range(min(max_batches, n // B)):
+        yield np.ascontiguousarray(frames[i * B:(i + 1) * B])
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--video", default=None, help="video file (cv2 decodes it); default: synthetic frames")
+    ap.add_argument("--raw-video", default=None, help="file of concatenated raw frames (ffmpeg -f rawvideo); needs --pixel-format, "
+                                                     "--height and --width")
+    ap.add_argument("--pixel-format", default=None, choices=["nv12", "i420", "yuyv"], help="with --raw-video: the frames' layout")
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--batches", type=int, default=10)
     ap.add_argument("--height", type=int, default=1080)
@@ -71,18 +90,26 @@ def main():
         net.init(None, weights=Wt.synthetic_weights(0))
     ctx = runtime.default_context()
 
-    if args.video:
+    pixel_format = "rgb"
+    if args.raw_video:
+        if args.pixel_format is None:
+            ap.error("--raw-video needs --pixel-format")
+        hw = (args.height, args.width)
+        pixel_format = args.pixel_format
+        batches = raw_video_batches(args.raw_video, pixel_format, args.batch, hw[0], hw[1], args.batches)
+    elif args.video:
         import cv2
         cap = cv2.VideoCapture(args.video)
         hw = (int(cap.get(cv2.CAP_PROP_FRAME_HEIGHT)), int(cap.get(cv2.CAP_PROP_FRAME_WIDTH)))
         cap.release()
+        pixel_format = "bgr"
         batches = video_batches(args.video, args.batch, args.batches)
     else:
         hw = (args.height, args.width)
         batches = synthetic_batches(args.batches, args.batch, hw[0], hw[1], args.seed)
 
     runner = FrameRunner(ctx, args.batch, hw, track=args.track, redetect_every=args.redetect_every, min_score=args.min_score,
-                         detect=args.detect, draw=args.draw_dir is not None)
+                         detect=args.detect, draw=args.draw_dir is not None, pixel_format=pixel_format)
     if args.draw_dir:
         from PIL import Image
         os.makedirs(args.draw_dir, exist_ok=True)

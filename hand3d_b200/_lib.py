@@ -83,6 +83,8 @@ SIGNATURES = {
     "h3d_reader_next_serials": (_i, [_p, _p, _i, C.c_uint64, _i, _p, _p]),
     "h3d_decode_records_gather": (_i, [_p, _i, _p, _i64, _p, _i, _i, _p, _p, _p, _p, _p]),
     "h3d_resize_frames": (_i, [_p, _p, _i, _i, _i, _i, _i, _i, _p, _p]),
+    "h3d_resize_frames_fmt": (_i, [_p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p]),
+    "h3d_convert_frames": (_i, [_p, _p, _i, _i, _i, _i, _p, _p]),
     "h3d_augment_image":(_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
     "h3d_rhd_reader_items_aug": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "h3d_gaussian_scoremap_dropout": (_i, [_p, _p, _p, _p, _i, _f, _i, _i, _i, _i, _f, _p, _p]),
@@ -124,6 +126,8 @@ AUG_UV_NOISE, AUG_CENTER_NOISE, AUG_SCALE, AUG_OFFSET_NOISE, AUG_HUE_DELTA, AUG_
 READER_QUEUE_CAPACITY, READER_STATE_COUNT, READER_STATE_NEXT, READER_STATE_SLOTS, READER_STATE_WORDS, READER_MAX_GATHER = 100, 0, 1, 2, 102, 4096
 # camera frames (H3D_FRAME_*): the largest frame side and output side of h3d_resize_frames
 FRAME_MAX_SIDE, FRAME_MAX_OUT = 4096, 512
+# pixel formats of camera frames (H3D_PIXEL_*), by the names hand3d_b200.frames takes
+PIXEL_FORMATS = {"rgb": 0, "bgr": 1, "nv12": 2, "i420": 3, "yuyv": 4}
 # the largest image side of h3d_pipeline_forward and h3d_seg_postprocess (H3D_PIPELINE_MAX_SIDE)
 PIPELINE_MAX_SIDE = 2048
 # tracking state (H3D_TRACK_*): the word offset of each array, in units of B words

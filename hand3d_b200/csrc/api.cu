@@ -190,9 +190,9 @@ struct h3d_ctx {
     bool profiling = false;
     struct ProfRec { cudaEvent_t a, b; int kind; int64_t flops; };
     std::vector<ProfRec> prof;
-    // h3d_resize_frames plans by (Hf, Wf, h, w): created outside graph capture, freed only by h3d_destroy (captured graphs point into
-    // their coefficients, so adding a plan never frees or moves another)
-    std::map<std::array<int, 4>, FramePlan*> frame_plans;
+    // h3d_resize_frames(_fmt) plans by (format, Hf, Wf, h, w): created outside graph capture, freed only by h3d_destroy (captured graphs
+    // point into their coefficients, so adding a plan never frees or moves another)
+    std::map<std::array<int, 5>, FramePlan*> frame_plans;
 };
 
 namespace h3d {
@@ -1024,7 +1024,7 @@ static int check_device() {
 extern "C" {
 
 const char* h3d_last_error(void) { return g_err; }
-int h3d_version(void) { return 110; }
+int h3d_version(void) { return 111; }
 
 int h3d_device_available(void) {
     int n = 0;
@@ -1992,27 +1992,63 @@ int h3d_reader_next_serials(h3d_ctx* ctx, int64_t* state, int B, uint64_t seed, 
     if (!rc) ctx->launches += 1;
     return rc;
 }
-int h3d_resize_frames(h3d_ctx* ctx, const uint8_t* frames, int B, int H, int W, int out_h, int out_w, int normalize, void* out, void* stream) {
-    H3D_OP_PROLOGUE(ctx);
-    H3D_REQUIRE(frames && out && B > 0 && (normalize == 0 || normalize == 1), "h3d_resize_frames: bad argument");
+namespace {
+
+// The frame sizes a pixel format accepts (include/hand3d_b200.h's table); the caller's name goes into the message.
+int check_frame_format(const char* fn, int format, int H, int W) {
+    H3D_REQUIRE(format >= H3D_PIXEL_RGB && format <= H3D_PIXEL_YUYV, "%s: unknown pixel format %d", fn, format);
+    H3D_REQUIRE(H >= 1 && H <= H3D_FRAME_MAX_SIDE && W >= 1 && W <= H3D_FRAME_MAX_SIDE, "%s: frames must be 1..%d pixels a side, got %dx%d",
+                fn, H3D_FRAME_MAX_SIDE, H, W);
+    if (format == H3D_PIXEL_NV12 || format == H3D_PIXEL_I420)
+        H3D_REQUIRE(H % 2 == 0 && W % 2 == 0, "%s: 4:2:0 frames must have an even height and width, got %dx%d", fn, H, W);
+    if (format == H3D_PIXEL_YUYV) H3D_REQUIRE(W % 2 == 0, "%s: YUYV frames must have an even width, got %d", fn, W);
+    return H3D_OK;
+}
+
+int resize_frames(h3d_ctx* ctx, const char* fn, const uint8_t* frames, int format, int B, int H, int W, int out_h, int out_w, int normalize,
+                  void* out, cudaStream_t s) {
+    H3D_REQUIRE(frames && out && B > 0 && (normalize == 0 || normalize == 1), "%s: bad argument", fn);
     H3D_REQUIRE(H >= 1 && H <= H3D_FRAME_MAX_SIDE && W >= 1 && W <= H3D_FRAME_MAX_SIDE && out_h >= 1 && out_h <= H3D_FRAME_MAX_OUT &&
                     out_w >= 1 && out_w <= H3D_FRAME_MAX_OUT,
-                "h3d_resize_frames: frames must be 1..%d pixels a side and the output 1..%d, got %dx%d -> %dx%d", H3D_FRAME_MAX_SIDE,
+                "%s: frames must be 1..%d pixels a side and the output 1..%d, got %dx%d -> %dx%d", fn, H3D_FRAME_MAX_SIDE,
                 H3D_FRAME_MAX_OUT, H, W, out_h, out_w);
-    const std::array<int, 4> key{H, W, out_h, out_w};
+    int rc = check_frame_format(fn, format, H, W);
+    if (rc) return rc;
+    const std::array<int, 5> key{format, H, W, out_h, out_w};
     auto it = ctx->frame_plans.find(key);
     if (it == ctx->frame_plans.end()) {
         cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
         H3D_CUDA(cudaStreamIsCapturing(s, &cs));
         H3D_REQUIRE(cs == cudaStreamCaptureStatusNone,
-                    "h3d_resize_frames: %dx%d -> %dx%d was not resized before this stream capture began, and its plan cannot be built "
+                    "%s: %dx%d -> %dx%d was not resized before this stream capture began, and its plan cannot be built "
                     "under capture (the coefficients are uploaded with a host-to-device copy): resize one batch of this size first",
-                    H, W, out_h, out_w);
-        FramePlan* p = frame_plan_create(H, W, out_h, out_w, s);
+                    fn, H, W, out_h, out_w);
+        FramePlan* p = frame_plan_create(format, H, W, out_h, out_w, s);
         if (!p) return H3D_ECUDA;
         it = ctx->frame_plans.emplace(key, p).first;
     }
-    int rc = launch_resize_frames(it->second, frames, B, normalize, out, s);
+    rc = launch_resize_frames(it->second, frames, B, normalize, out, s);
+    if (!rc) ctx->launches += 1;
+    return rc;
+}
+
+}  // namespace
+
+int h3d_resize_frames(h3d_ctx* ctx, const uint8_t* frames, int B, int H, int W, int out_h, int out_w, int normalize, void* out, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    return resize_frames(ctx, "h3d_resize_frames", frames, H3D_PIXEL_RGB, B, H, W, out_h, out_w, normalize, out, s);
+}
+int h3d_resize_frames_fmt(h3d_ctx* ctx, const uint8_t* frames, int format, int B, int H, int W, int out_h, int out_w, int normalize,
+                          void* out, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    return resize_frames(ctx, "h3d_resize_frames_fmt", frames, format, B, H, W, out_h, out_w, normalize, out, s);
+}
+int h3d_convert_frames(h3d_ctx* ctx, const uint8_t* frames, int format, int B, int H, int W, uint8_t* out_rgb, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(frames && out_rgb && B > 0, "h3d_convert_frames: bad argument");
+    int rc = check_frame_format("h3d_convert_frames", format, H, W);
+    if (rc) return rc;
+    rc = launch_convert_frames(frames, format, B, H, W, out_rgb, s);
     if (!rc) ctx->launches += 1;
     return rc;
 }

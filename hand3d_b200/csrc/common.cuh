@@ -168,12 +168,14 @@ int launch_augment_image(const float* image, const uint8_t* parts, const float* 
                          float* out_image, int32_t* out_parts, int32_t* out_mask, cudaStream_t s);
 int launch_canonical_trafo(const float* xyz, const uint8_t* cond_right, int B, float* can, float* rot, float* rot_inv, cudaStream_t s);
 
-// ---------------------------------------------------------------- kernels (frames.cu): Pillow's bilinear resize of uint8 RGB frames
-struct FramePlan;   // opaque: the coefficients of one (Hf, Wf, h, w) on the device and the launch geometry
+// ---------------------------------------------------------------- kernels (frames.cu): Pillow's bilinear resize of uint8 frames
+struct FramePlan;   // opaque: the coefficients of one (format, Hf, Wf, h, w) on the device and the launch geometry
 // builds the plan and enqueues its upload on s (never under capture); nullptr on failure (h3d_last_error set)
-FramePlan* frame_plan_create(int Hf, int Wf, int h, int w, cudaStream_t s);
+FramePlan* frame_plan_create(int fmt, int Hf, int Wf, int h, int w, cudaStream_t s);
 void frame_plan_destroy(FramePlan* p);
 int launch_resize_frames(const FramePlan* p, const uint8_t* frames, int B, int normalize, void* out, cudaStream_t s);
+// frames of format fmt (H3D_PIXEL_*, arguments checked) -> uint8 RGB [B,H,W,3]
+int launch_convert_frames(const uint8_t* frames, int fmt, int B, int H, int W, uint8_t* out, cudaStream_t s);
 
 // ---------------------------------------------------------------- kernels (draw.cu): anti-aliased segments into uint8 RGB images
 // (arguments checked by h3d_draw_segments; host_colors [S,3] is copied into the kernel's parameters)

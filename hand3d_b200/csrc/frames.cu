@@ -11,6 +11,12 @@
 // vertical filter's halo) from HBM through a double-buffered shared-memory stage (cp.async for the 16-byte words inside the row, byte
 // loads at its unaligned ends), filters them horizontally into a uint8 chunk and adds each chunk's vertical contributions to int32
 // accumulators of the band's output rows.  No intermediate leaves the SM.
+//
+// The kernel is instantiated per input pixel format (H3D_PIXEL_*; DESIGN.md section 4.18).  RGB and BGR stage the packed row; BGR only
+// swaps the channels the horizontal pass writes.  The YUV formats stage each row's segments (NV12: the Y row and its interleaved UV row;
+// I420: the Y row, its U row and its V row; YUYV: the packed row), each 16-byte aligned in its own slot, and convert them once per
+// source pixel into an RGB chunk in shared memory (OpenCV's cvtColor BT.601 rule below), which the horizontal pass reads as the RGB
+// instance reads its stage.  The plan pays for that chunk with fewer rows per stage.
 #include <cstring>
 #include <vector>
 
@@ -34,6 +40,12 @@ struct FrameArgs {
     int acc_bytes, inter_bytes;
     const int32_t *xb, *kx, *yb, *ky;   // bounds (first tap, taps) and fixed-point coefficients per output column / row
     const float* lut;                   // [256] run.py's normalisation of each code
+};
+// The YUV formats' geometry: one frame's bytes, each segment's slot within a staged row, the converted RGB row's stride.  A kernel
+// parameter of its own: growing FrameArgs changes the RGB instance's code (and made it 2-4 % slower on an H100).
+struct YuvArgs {
+    int64_t frame_bytes;
+    int seg_off[3], rgb_stride;
 };
 
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
@@ -67,7 +79,76 @@ __device__ __forceinline__ void stage_rows(const FrameArgs& a, const uint8_t* im
 
 __device__ __forceinline__ int clip8(int v) { return min(255, max(0, v >> kPrecisionBits)); }
 
-__global__ void __launch_bounds__(kFrameThreads, 2) resize_frames_kernel(FrameArgs a) {
+constexpr bool is_yuv(int fmt) { return fmt == H3D_PIXEL_NV12 || fmt == H3D_PIXEL_I420 || fmt == H3D_PIXEL_YUYV; }
+constexpr int n_segments(int fmt) { return fmt == H3D_PIXEL_I420 ? 3 : fmt == H3D_PIXEL_NV12 ? 2 : 1; }
+constexpr int64_t frame_bytes_of(int fmt, int64_t H, int64_t W) {
+    return fmt == H3D_PIXEL_NV12 || fmt == H3D_PIXEL_I420 ? H * W * 3 / 2 : fmt == H3D_PIXEL_YUYV ? H * W * 2 : H * W * 3;
+}
+
+// Segment s of input row r of a YUV frame (the planes and their layouts are in include/hand3d_b200.h) -> its first byte and length.
+template <int FMT>
+__device__ __forceinline__ const uint8_t* yuv_segment(const uint8_t* img, int Hf, int Wf, int s, int r, int& len) {
+    const int64_t Y = (int64_t)Hf * Wf;
+    if (FMT == H3D_PIXEL_YUYV) { len = 2 * Wf; return img + (int64_t)r * 2 * Wf; }
+    if (s == 0) { len = Wf; return img + (int64_t)r * Wf; }
+    if (FMT == H3D_PIXEL_NV12) { len = Wf; return img + Y + (int64_t)(r >> 1) * Wf; }
+    len = Wf >> 1;                                                           // I420: U (s = 1) then V (s = 2)
+    return img + Y + (s == 2 ? Y >> 2 : 0) + (int64_t)(r >> 1) * (Wf >> 1);
+}
+
+// stage_rows for the YUV formats: each segment of a row into its own slot, with the same alignment rule.
+template <int FMT>
+__device__ __forceinline__ void stage_yuv_rows(const FrameArgs& a, const YuvArgs& y, const uint8_t* img, int c0, int n, uint8_t* buf) {
+#pragma unroll
+    for (int sg = 0; sg < n_segments(FMT); ++sg) {
+        const int words = (sg + 1 < n_segments(FMT) ? y.seg_off[sg + 1] - y.seg_off[sg] : a.row_stride - y.seg_off[sg]) >> 4;
+        for (int k = threadIdx.x; k < n * words; k += kFrameThreads) {
+            const int i = k / words, wd = k - i * words;
+            int len;
+            const uintptr_t lo = (uintptr_t)yuv_segment<FMT>(img, a.Hf, a.Wf, sg, c0 + i, len), hi = lo + (uintptr_t)len;
+            const uintptr_t g = (lo & ~(uintptr_t)15) + 16 * (uintptr_t)wd;
+            uint8_t* d = buf + (int64_t)i * a.row_stride + y.seg_off[sg] + 16 * wd;
+            if (g >= lo && g + 16 <= hi) {
+                cp_async16(d, (const void*)g);
+            } else {
+#pragma unroll
+                for (int j = 0; j < 16; ++j)
+                    if (g + j >= lo && g + j < hi) d[j] = __ldg((const uint8_t*)(g + j));
+            }
+        }
+    }
+}
+
+// OpenCV's cvtColor COLOR_YUV2RGB_* (BT.601 limited range, 20-bit fixed point): one pixel from its luma and its block's chroma.
+__device__ __forceinline__ void yuv_to_rgb(int Y, int U, int V, uint8_t* q) {
+    const int c = max(Y - 16, 0) * 1220542 + (1 << 19), u = U - 128, v = V - 128;
+    q[0] = (uint8_t)min(255, max(0, (c + 1673527 * v) >> 20));
+    q[1] = (uint8_t)min(255, max(0, (c - 852492 * v - 409993 * u) >> 20));
+    q[2] = (uint8_t)min(255, max(0, (c + 2116026 * u) >> 20));
+}
+
+// The luma of pixels 2p, 2p + 1 of a row and their shared chroma, read from the row's staged segments (st = the staged row).
+template <int FMT>
+__device__ __forceinline__ void yuv_pair(const FrameArgs& a, const YuvArgs& ya, const uint8_t* img, const uint8_t* st, int r, int p, int& y0,
+                                         int& y1, int& u, int& v) {
+    int len;
+    const uint8_t* s0 = st + ya.seg_off[0] + ((uintptr_t)yuv_segment<FMT>(img, a.Hf, a.Wf, 0, r, len) & 15);
+    if (FMT == H3D_PIXEL_YUYV) {
+        y0 = s0[4 * p]; u = s0[4 * p + 1]; y1 = s0[4 * p + 2]; v = s0[4 * p + 3];
+        return;
+    }
+    y0 = s0[2 * p]; y1 = s0[2 * p + 1];
+    const uint8_t* s1 = st + ya.seg_off[1] + ((uintptr_t)yuv_segment<FMT>(img, a.Hf, a.Wf, 1, r, len) & 15);
+    if (FMT == H3D_PIXEL_NV12) {
+        u = s1[2 * p]; v = s1[2 * p + 1];
+    } else {
+        const uint8_t* s2 = st + ya.seg_off[2] + ((uintptr_t)yuv_segment<FMT>(img, a.Hf, a.Wf, 2, r, len) & 15);
+        u = s1[p]; v = s2[p];
+    }
+}
+
+template <int FMT>
+__global__ void __launch_bounds__(kFrameThreads, 2) resize_frames_kernel(FrameArgs a, YuvArgs ya) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int band = blockIdx.x % a.nbands;
     const int64_t b = blockIdx.x / a.nbands;
@@ -77,32 +158,47 @@ __global__ void __launch_bounds__(kFrameThreads, 2) resize_frames_kernel(FrameAr
     uint8_t* inter = smem + a.acc_bytes;                                 // [chunk][w3]: the horizontal pass of the current chunk
     uint8_t* stage = inter + a.inter_bytes;                              // 2 x [chunk][row_stride]
     const int64_t stage_bytes = (int64_t)a.chunk * a.row_stride;
+    uint8_t* rgb = stage + 2 * stage_bytes;                              // YUV formats: [chunk][rgb_stride], the converted chunk
     const int64_t rb = (int64_t)a.Wf * 3;
-    const uint8_t* img = a.in + b * a.Hf * rb;
+    const uint8_t* img = is_yuv(FMT) ? a.in + b * ya.frame_bytes : a.in + b * a.Hf * rb;
     const int r0 = a.yb[2 * y0], r1 = a.yb[2 * (y1 - 1)] + a.yb[2 * (y1 - 1) + 1];   // the band's input rows (bounds are monotone)
     const int nchunks = (r1 - r0 + a.chunk - 1) / a.chunk;
 
     for (int i = threadIdx.x; i < ny * w3; i += kFrameThreads) acc[i] = 1 << (kPrecisionBits - 1);
-    stage_rows(a, img, r0, min(a.chunk, r1 - r0), stage);
+    if (is_yuv(FMT)) stage_yuv_rows<FMT>(a, ya, img, r0, min(a.chunk, r1 - r0), stage);
+    else stage_rows(a, img, r0, min(a.chunk, r1 - r0), stage);
     cp_async_commit();
     for (int c = 0; c < nchunks; ++c) {
         const int c0 = r0 + c * a.chunk, n = min(a.chunk, r1 - c0);
         const uint8_t* cur = stage + (c & 1) * stage_bytes;
         if (c + 1 < nchunks) {        // the other buffer was last read before the barrier that ended the previous iteration
-            stage_rows(a, img, c0 + a.chunk, min(a.chunk, r1 - c0 - a.chunk), stage + ((c + 1) & 1) * stage_bytes);
+            if (is_yuv(FMT)) stage_yuv_rows<FMT>(a, ya, img, c0 + a.chunk, min(a.chunk, r1 - c0 - a.chunk), stage + ((c + 1) & 1) * stage_bytes);
+            else stage_rows(a, img, c0 + a.chunk, min(a.chunk, r1 - c0 - a.chunk), stage + ((c + 1) & 1) * stage_bytes);
             cp_async_commit();
             cp_async_wait_all_but_one();
         } else {
             cp_async_wait_all();
         }
         __syncthreads();
+        if (is_yuv(FMT)) {            // convert the chunk once per source pixel (two pixels, one chroma sample per thread)
+            const int np = a.Wf >> 1;
+            for (int i = threadIdx.x; i < n * np; i += kFrameThreads) {
+                const int r = i / np, p = i - r * np;
+                int y0p, y1p, u, v;
+                yuv_pair<FMT>(a, ya, img, cur + (int64_t)r * a.row_stride, c0 + r, p, y0p, y1p, u, v);
+                uint8_t* q = rgb + (int64_t)r * ya.rgb_stride + 6 * p;
+                yuv_to_rgb(y0p, u, v, q);
+                yuv_to_rgb(y1p, u, v, q + 3);
+            }
+            __syncthreads();
+        }
         // horizontal pass: n input rows x w output columns, three channels per thread (one coefficient load per tap)
         for (int i = threadIdx.x; i < n * a.w; i += kFrameThreads) {
             const int r = i / a.w, x = i - r * a.w;
-            const int off = (int)((uintptr_t)(img + (int64_t)(c0 + r) * rb) & 15);
+            const int off = is_yuv(FMT) ? 0 : (int)((uintptr_t)(img + (int64_t)(c0 + r) * rb) & 15);
             const int xmin = __ldg(a.xb + 2 * x), nx = __ldg(a.xb + 2 * x + 1);
             const int32_t* k = a.kx + (int64_t)x * a.kxs;
-            const uint8_t* p = cur + (int64_t)r * a.row_stride + off + xmin * 3;
+            const uint8_t* p = is_yuv(FMT) ? rgb + (int64_t)r * ya.rgb_stride + xmin * 3 : cur + (int64_t)r * a.row_stride + off + xmin * 3;
             int s0 = 1 << (kPrecisionBits - 1), s1 = s0, s2 = s0;
             for (int t = 0; t < nx; ++t) {
                 const int kt = __ldg(k + t);
@@ -110,6 +206,7 @@ __global__ void __launch_bounds__(kFrameThreads, 2) resize_frames_kernel(FrameAr
                 s1 += p[3 * t + 1] * kt;
                 s2 += p[3 * t + 2] * kt;
             }
+            if (FMT == H3D_PIXEL_BGR) { const int t = s0; s0 = s2; s2 = t; }
             uint8_t* q = inter + r * w3 + 3 * x;
             q[0] = (uint8_t)clip8(s0); q[1] = (uint8_t)clip8(s1); q[2] = (uint8_t)clip8(s2);
         }
@@ -135,6 +232,48 @@ __global__ void __launch_bounds__(kFrameThreads, 2) resize_frames_kernel(FrameAr
     } else {
         uint8_t* out = static_cast<uint8_t*>(a.out) + o;
         for (int i = threadIdx.x; i < ny * w3; i += kFrameThreads) out[i] = (uint8_t)clip8(acc[i]);
+    }
+}
+
+// Full-size conversion of any format into packed RGB: one thread per chroma block (2x2 for NV12 and I420, 2x1 for YUYV; one pixel for
+// RGB and BGR), consecutive threads on consecutive blocks of a row pair.
+template <int FMT>
+__global__ void __launch_bounds__(256) convert_frames_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, int H, int W,
+                                                             int64_t blocks) {
+    constexpr int BH = FMT == H3D_PIXEL_NV12 || FMT == H3D_PIXEL_I420 ? 2 : 1, BW = is_yuv(FMT) ? 2 : 1;
+    const int bw = W / BW, bh = H / BH;
+    const int64_t per_image = (int64_t)bw * bh;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < blocks; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t b = i / per_image;
+        const int64_t j = i - b * per_image;
+        const int by = (int)(j / bw), bx = (int)(j - (int64_t)by * bw);
+        const uint8_t* img = in + b * frame_bytes_of(FMT, H, W);
+        uint8_t* q = out + ((b * H + (int64_t)by * BH) * W + (int64_t)bx * BW) * 3;
+        if (FMT == H3D_PIXEL_RGB || FMT == H3D_PIXEL_BGR) {
+            const uint8_t* p = img + ((int64_t)by * W + bx) * 3;
+            const uint8_t c0 = p[0], c1 = p[1], c2 = p[2];
+            q[0] = FMT == H3D_PIXEL_BGR ? c2 : c0; q[1] = c1; q[2] = FMT == H3D_PIXEL_BGR ? c0 : c2;
+        } else if (FMT == H3D_PIXEL_YUYV) {
+            const uint8_t* p = img + ((int64_t)by * W + 2 * bx) * 2;
+            const int y0 = p[0], u = p[1], y1 = p[2], v = p[3];
+            yuv_to_rgb(y0, u, v, q);
+            yuv_to_rgb(y1, u, v, q + 3);
+        } else {
+            const int64_t Y = (int64_t)H * W;
+            const uint8_t* yp = img + (int64_t)2 * by * W + 2 * bx;
+            int u, v;
+            if (FMT == H3D_PIXEL_NV12) {
+                const uint8_t* c = img + Y + (int64_t)by * W + 2 * bx;
+                u = c[0]; v = c[1];
+            } else {
+                const int64_t ci = (int64_t)by * (W / 2) + bx;
+                u = img[Y + ci]; v = img[Y + Y / 4 + ci];
+            }
+            yuv_to_rgb(yp[0], u, v, q);
+            yuv_to_rgb(yp[1], u, v, q + 3);
+            yuv_to_rgb(yp[W], u, v, q + (int64_t)W * 3);
+            yuv_to_rgb(yp[W + 1], u, v, q + (int64_t)W * 3 + 3);
+        }
     }
 }
 
@@ -182,28 +321,55 @@ int pil_bilinear_coeffs(int in, int out, std::vector<int32_t>& bounds, std::vect
 }  // namespace
 
 struct FramePlan {
-    int Hf = 0, Wf = 0, h = 0, w = 0;
+    int fmt = H3D_PIXEL_RGB, Hf = 0, Wf = 0, h = 0, w = 0;
     int kxs = 0, kys = 0, band = 0, chunk = 0, row_stride = 0, nbands = 0, acc_bytes = 0, inter_bytes = 0, smem = 0;
+    int seg_off[3] = {0, 0, 0}, rgb_stride = 0;
     std::vector<int32_t> host;      // the source of the asynchronous upload, kept for the plan's lifetime
     int32_t* dev = nullptr;         // [xb | kx | yb | ky | lut]
     const int32_t *xb = nullptr, *kx = nullptr, *yb = nullptr, *ky = nullptr;
     const float* lut = nullptr;
 };
 
-FramePlan* frame_plan_create(int Hf, int Wf, int h, int w, cudaStream_t s) {
+namespace {
+
+const void* resize_kernel_of(int fmt) {
+    switch (fmt) {
+        case H3D_PIXEL_BGR: return (const void*)resize_frames_kernel<H3D_PIXEL_BGR>;
+        case H3D_PIXEL_NV12: return (const void*)resize_frames_kernel<H3D_PIXEL_NV12>;
+        case H3D_PIXEL_I420: return (const void*)resize_frames_kernel<H3D_PIXEL_I420>;
+        case H3D_PIXEL_YUYV: return (const void*)resize_frames_kernel<H3D_PIXEL_YUYV>;
+        default: return (const void*)resize_frames_kernel<H3D_PIXEL_RGB>;
+    }
+}
+
+}  // namespace
+
+FramePlan* frame_plan_create(int fmt, int Hf, int Wf, int h, int w, cudaStream_t s) {
     auto* p = new FramePlan();
-    p->Hf = Hf; p->Wf = Wf; p->h = h; p->w = w;
+    p->fmt = fmt; p->Hf = Hf; p->Wf = Wf; p->h = h; p->w = w;
     std::vector<int32_t> xb, kx, yb, ky;
     p->kxs = pil_bilinear_coeffs(Wf, w, xb, kx);
     p->kys = pil_bilinear_coeffs(Hf, h, yb, ky);
     const int w3 = 3 * w;
-    p->row_stride = (int)align_up((int64_t)Wf * 3 + 15, 16);
-    p->chunk = std::max(1, std::min(kMaxChunk, kStageBudget / p->row_stride));
+    if (is_yuv(fmt)) {
+        // a staged row is one 16-byte aligned slot per segment; the converted chunk takes its share of both stage buffers' budget
+        const int n = fmt == H3D_PIXEL_I420 ? 3 : fmt == H3D_PIXEL_NV12 ? 2 : 1;
+        const int len[3] = {fmt == H3D_PIXEL_YUYV ? 2 * Wf : Wf, fmt == H3D_PIXEL_NV12 ? Wf : Wf / 2, Wf / 2};
+        for (int i = 0; i < n; ++i) {
+            p->seg_off[i] = p->row_stride;
+            p->row_stride += (int)align_up((int64_t)len[i] + 15, 16);
+        }
+        p->rgb_stride = (int)align_up((int64_t)Wf * 3, 16);
+        p->chunk = std::max(1, std::min(kMaxChunk, 2 * kStageBudget / (2 * p->row_stride + p->rgb_stride)));
+    } else {
+        p->row_stride = (int)align_up((int64_t)Wf * 3 + 15, 16);
+        p->chunk = std::max(1, std::min(kMaxChunk, kStageBudget / p->row_stride));
+    }
     p->band = std::max(1, std::min({kMaxBand, h, kAccBudget / (w3 * 4)}));
     p->nbands = ceil_div(h, p->band);
     p->acc_bytes = (int)align_up((int64_t)p->band * w3 * 4, 16);
     p->inter_bytes = (int)align_up((int64_t)p->chunk * w3, 16);
-    p->smem = p->acc_bytes + p->inter_bytes + 2 * p->chunk * p->row_stride;
+    p->smem = p->acc_bytes + p->inter_bytes + 2 * p->chunk * p->row_stride + p->chunk * p->rgb_stride;
     auto& v = p->host;
     const size_t oxb = 0, okx = oxb + xb.size(), oyb = okx + kx.size(), oky = oyb + yb.size(), olut = oky + ky.size();
     v.resize(olut + 256);
@@ -217,9 +383,10 @@ FramePlan* frame_plan_create(int Hf, int Wf, int h, int w, cudaStream_t s) {
     }
     // the attribute is per kernel, not per plan: only ever raise it, or a plan with less shared memory would break the earlier ones
     cudaFuncAttributes fa;
-    cudaError_t e = cudaFuncGetAttributes(&fa, resize_frames_kernel);
+    const void* kern = resize_kernel_of(fmt);
+    cudaError_t e = cudaFuncGetAttributes(&fa, kern);
     if (e == cudaSuccess && fa.maxDynamicSharedSizeBytes < p->smem)
-        e = cudaFuncSetAttribute(resize_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, p->smem);
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, p->smem);
     if (e == cudaSuccess) e = cudaMalloc(&p->dev, v.size() * 4);
     if (e == cudaSuccess) e = cudaMemcpyAsync(p->dev, v.data(), v.size() * 4, cudaMemcpyHostToDevice, s);
     if (e != cudaSuccess) {
@@ -248,8 +415,33 @@ int launch_resize_frames(const FramePlan* p, const uint8_t* frames, int B, int n
     a.in = frames; a.out = out; a.Hf = p->Hf; a.Wf = p->Wf; a.h = p->h; a.w = p->w; a.normalize = normalize;
     a.kxs = p->kxs; a.kys = p->kys; a.band = p->band; a.chunk = p->chunk; a.row_stride = p->row_stride; a.nbands = p->nbands;
     a.acc_bytes = p->acc_bytes; a.inter_bytes = p->inter_bytes;
+    YuvArgs y;
+    for (int i = 0; i < 3; ++i) y.seg_off[i] = p->seg_off[i];
+    y.rgb_stride = p->rgb_stride;
+    y.frame_bytes = frame_bytes_of(p->fmt, p->Hf, p->Wf);
     a.xb = p->xb; a.kx = p->kx; a.yb = p->yb; a.ky = p->ky; a.lut = p->lut;
-    resize_frames_kernel<<<(unsigned)grid, kFrameThreads, p->smem, s>>>(a);
+    switch (p->fmt) {
+        case H3D_PIXEL_BGR: resize_frames_kernel<H3D_PIXEL_BGR><<<(unsigned)grid, kFrameThreads, p->smem, s>>>(a, y); break;
+        case H3D_PIXEL_NV12: resize_frames_kernel<H3D_PIXEL_NV12><<<(unsigned)grid, kFrameThreads, p->smem, s>>>(a, y); break;
+        case H3D_PIXEL_I420: resize_frames_kernel<H3D_PIXEL_I420><<<(unsigned)grid, kFrameThreads, p->smem, s>>>(a, y); break;
+        case H3D_PIXEL_YUYV: resize_frames_kernel<H3D_PIXEL_YUYV><<<(unsigned)grid, kFrameThreads, p->smem, s>>>(a, y); break;
+        default: resize_frames_kernel<H3D_PIXEL_RGB><<<(unsigned)grid, kFrameThreads, p->smem, s>>>(a, y); break;
+    }
+    H3D_CHECK_LAUNCH();
+    return H3D_OK;
+}
+
+int launch_convert_frames(const uint8_t* frames, int fmt, int B, int H, int W, uint8_t* out, cudaStream_t s) {
+    const int per_block = fmt == H3D_PIXEL_NV12 || fmt == H3D_PIXEL_I420 ? 4 : fmt == H3D_PIXEL_YUYV ? 2 : 1;
+    const int64_t blocks = (int64_t)B * H * W / per_block;
+    const int64_t grid = std::min<int64_t>(ceil_div64(blocks, 256), 1 << 20);   // grid-stride beyond
+    switch (fmt) {
+        case H3D_PIXEL_BGR: convert_frames_kernel<H3D_PIXEL_BGR><<<(unsigned)grid, 256, 0, s>>>(frames, out, H, W, blocks); break;
+        case H3D_PIXEL_NV12: convert_frames_kernel<H3D_PIXEL_NV12><<<(unsigned)grid, 256, 0, s>>>(frames, out, H, W, blocks); break;
+        case H3D_PIXEL_I420: convert_frames_kernel<H3D_PIXEL_I420><<<(unsigned)grid, 256, 0, s>>>(frames, out, H, W, blocks); break;
+        case H3D_PIXEL_YUYV: convert_frames_kernel<H3D_PIXEL_YUYV><<<(unsigned)grid, 256, 0, s>>>(frames, out, H, W, blocks); break;
+        default: convert_frames_kernel<H3D_PIXEL_RGB><<<(unsigned)grid, 256, 0, s>>>(frames, out, H, W, blocks); break;
+    }
     H3D_CHECK_LAUNCH();
     return H3D_OK;
 }

@@ -6,6 +6,10 @@
 imresize() is that first line, bit for bit, for uint8 RGB frames of 1..4096 pixels a side (scipy.misc.imresize is gone from current
 scipy); to_network_input() fuses both lines into one kernel; frame_coords() maps coordinates of the 240x320 image back to frame
 pixels; FrameRunner serves a stream of equal-size frames through the resize and the whole pipeline as one CUDA graph per buffer.
+
+to_network_input, to_rgb and FrameRunner also take camera frames as they come from decoders and capture devices (pixel_format "bgr",
+"nv12", "i420" or "yuyv"; frame_shape gives each one's tensor layout): the conversion to RGB is OpenCV's cvtColor rule, on the device,
+fused into the resize (DESIGN.md section 4.18).
 """
 from __future__ import annotations
 
@@ -14,6 +18,7 @@ import torch
 
 from . import _lib, runtime
 from . import draw as _draw
+from .runtime import frame_shape
 from .utils.general import trafo_coords
 
 NETWORK_SIZE = (240, 320)   # run.py:58
@@ -23,13 +28,13 @@ def _ctx_for(t):
     return runtime.default_context(t.device if isinstance(t, torch.Tensor) and t.is_cuda else None)
 
 
-def _batched(frames):
-    """CUDA uint8 [H,W,3] or [B,H,W,3] -> ([B,H,W,3], squeezed)."""
+def _batched(frames, pixel_format="rgb"):
+    """CUDA uint8 one frame or a batch of frames in pixel_format ([H,W,3] or [B,H,W,3] for RGB) -> (the batch, squeezed)."""
     if not isinstance(frames, torch.Tensor):
         raise TypeError("frames must be a torch.Tensor or a numpy array")
     if not frames.is_cuda:
         raise RuntimeError("frames must be a CUDA tensor here (numpy arrays are accepted by imresize)")
-    if frames.dim() == 3:
+    if frames.dim() == (2 if pixel_format in ("nv12", "i420") else 3):
         return frames.unsqueeze(0), True
     return frames, False
 
@@ -71,12 +76,22 @@ def imresize(arr, size, interp="bilinear", mode=None):
     return out[0] if squeeze else out
 
 
-def to_network_input(frames, size=NETWORK_SIZE, out=None):
+def to_network_input(frames, size=NETWORK_SIZE, out=None, pixel_format="rgb"):
     """run.py:58-59 in one kernel: CUDA uint8 frames [B,H,W,3] (or [H,W,3]) -> float32 [B,h,w,3] = float64(imresize(frame, size))
     / 255.0 - 0.5 rounded to float32, the pipeline's input.  With `out` (float32 [B,h,w,3]) it writes there and allocates nothing, so a
-    call of an already seen size can be captured into a CUDA graph."""
-    frames, squeeze = _batched(frames)
-    r = _ctx_for(frames).resize_frames(frames, size[0], size[1], normalize=True, out=None if out is None else (out.unsqueeze(0) if squeeze else out))
+    call of an already seen size can be captured into a CUDA graph.  frames in another pixel_format ("bgr", "nv12", "i420", "yuyv";
+    one frame or a batch of frame_shape(pixel_format, H, W)) are converted to RGB inside the same kernel."""
+    frames, squeeze = _batched(frames, pixel_format)
+    r = _ctx_for(frames).resize_frames(frames, size[0], size[1], normalize=True, out=None if out is None else (out.unsqueeze(0) if squeeze else out),
+                                       pixel_format=pixel_format)
+    return r[0] if squeeze else r
+
+
+def to_rgb(frames, pixel_format, out=None):
+    """CUDA uint8 frames in pixel_format (one frame or a batch of frame_shape(pixel_format, H, W)) -> uint8 RGB [B,H,W,3] (or [H,W,3])
+    at full size, by OpenCV's cvtColor rule (include/hand3d_b200.h); with `out` it writes there and allocates nothing."""
+    frames, squeeze = _batched(frames, pixel_format)
+    r = _ctx_for(frames).convert_frames(frames, pixel_format, out=None if out is None else (out.unsqueeze(0) if squeeze else out))
     return r[0] if squeeze else r
 
 
@@ -115,7 +130,7 @@ class FrameRunner:
       keypoint_coord3d [B,21,3], center [B,2] and scale_crop [B,1] (float32).
     Those tensors belong to buffer (call index mod 2): the replay of the call after next overwrites them, in stream order on the
     current stream; read them (or copy them) before that call.
-      - Host frames (numpy or CPU torch, [B,H,W,3] uint8) are copied into a pinned staging buffer and uploaded on a copy stream, so
+      - Host frames (numpy or CPU torch, [B,H,W,3] uint8, or pixel_format's shape) are copied into a pinned staging buffer and uploaded on a copy stream, so
         the upload of one batch overlaps the replay of the previous one.  A staging buffer is refilled only after its previous upload
         has finished (an event wait for the upload two calls back).
       - CUDA frames are copied into the graph's input buffer on the current stream; nothing synchronises the host.
@@ -146,16 +161,24 @@ class FrameRunner:
     Hf / 240), so that lines look as they would on the 240-row network image; draw.py, DESIGN.md section 4.16).  In track mode a
     slot whose state is lost after the step is not drawn (valid = state lost == 0, on the device).  The results gain frame_drawn
     [B,Hf,Wf,3] uint8: that buffer, valid until the call after next like the other results.  stream(batches, drawn_every=N) reads
-    it back for every N-th batch only (0: never)."""
+    it back for every N-th batch only (0: never).
+
+    pixel_format ("rgb", "bgr", "nv12", "i420" or "yuyv") is the layout of the submitted frames: the input buffers and the pinned
+    staging take frame_shape(pixel_format, *frame_hw), so a host upload carries the format's bytes (half of RGB's for 4:2:0), and the
+    captured resize converts to RGB as it reads.  frame_hw stays the picture's (H, W).  With draw=True and a format other than "rgb",
+    the captured step first converts the frames into an RGB frame buffer (h3d_convert_frames) and draws there; frame_drawn is that
+    buffer, [B,Hf,Wf,3] RGB as for "rgb"."""
 
     RESULT_KEYS = ("keypoints_frame", "keypoints_uv", "keypoint_coord3d", "center", "scale_crop")
     TRACK_KEYS = ("track_score", "track_lost")
     SLOTS_KEYS = ("track_score", "track_lost", "track_detected")
 
     def __init__(self, ctx, batch, frame_hw, size=NETWORK_SIZE, outputs="keypoints", track=False, redetect_every=None, min_score=None,
-                 track_margin=1.5, detect="batch", draw=False, draw_linewidth=None):
+                 track_margin=1.5, detect="batch", draw=False, draw_linewidth=None, pixel_format="rgb"):
         self.ctx, self.B = ctx, int(batch)
         self.frame_hw, self.size = (int(frame_hw[0]), int(frame_hw[1])), (int(size[0]), int(size[1]))
+        self.pixel_format = pixel_format
+        self._frame_shape = frame_shape(pixel_format, *self.frame_hw)
         self.track = bool(track)
         if detect not in ("batch", "slots"):
             raise ValueError("FrameRunner: detect must be 'batch' or 'slots', got %r" % (detect,))
@@ -173,8 +196,10 @@ class FrameRunner:
         if self.draw:
             self._draw_colors = np.concatenate([np.repeat(_draw.WHITE[None], 4, 0), _draw.PALETTE])
         h, w = self.size
-        self._frames = [torch.empty((self.B, Hf, Wf, 3), dtype=torch.uint8, device=dev) for _ in range(2)]
-        self._frames[0].zero_(); self._frames[1].zero_()
+        self._frames = [torch.zeros((self.B,) + self._frame_shape, dtype=torch.uint8, device=dev) for _ in range(2)]
+        # the frames drawn into: the input buffers themselves for RGB, else an RGB conversion of them made by the step
+        self._drawn = self._frames if pixel_format == "rgb" or not self.draw else \
+            [torch.zeros((self.B, Hf, Wf, 3), dtype=torch.uint8, device=dev) for _ in range(2)]
         self._default_hs = torch.tensor([[1.0, 0.0]], dtype=torch.float32).expand(self.B, 2).contiguous().to(dev)
         self._hs = [self._default_hs.clone() for _ in range(2)]
         self._image = [torch.empty((self.B, h, w, 3), dtype=torch.float32, device=dev) for _ in range(2)]
@@ -201,7 +226,7 @@ class FrameRunner:
             self._detected = [True, True]
 
         def body(k, detect=True):
-            ctx.resize_frames(self._frames[k], h, w, normalize=True, out=self._image[k])
+            ctx.resize_frames(self._frames[k], h, w, normalize=True, out=self._image[k], pixel_format=pixel_format)
             if self.slots:
                 r = ctx.track_step_slots(self._image[k], self._hs[k], self._state, None if self._force is None else self._force[k],
                                          margin=self.track_margin, min_score=self.min_score, outputs=outputs)
@@ -219,7 +244,9 @@ class FrameRunner:
                 seg = torch.cat([_draw.crop_box_segments(r["center"], r["scale_crop"], self.frame_hw, self.size),
                                  _draw.hand_segments(r["keypoints_frame"].to(torch.float32))], 1).contiguous()
                 valid = (self._state.lost == 0).to(torch.int32) if self.track else None
-                r["frame_drawn"] = ctx.draw_segments(self._frames[k], seg, self._draw_colors, self.draw_linewidth, valid)
+                if self._drawn is not self._frames:
+                    ctx.convert_frames(self._frames[k], pixel_format, out=self._drawn[k])
+                r["frame_drawn"] = ctx.draw_segments(self._drawn[k], seg, self._draw_colors, self.draw_linewidth, valid)
             return r
 
         kinds = (True, False) if self.track and not self.slots else (True,)
@@ -258,7 +285,7 @@ class FrameRunner:
         return bool(self._lost_host[k].any())
 
     def _check_frames(self, frames):
-        shape = (self.B,) + self.frame_hw + (3,)
+        shape = (self.B,) + self._frame_shape
         if tuple(frames.shape) != shape:
             raise ValueError("FrameRunner: frames must be %s, got %s" % (shape, tuple(frames.shape)))
 

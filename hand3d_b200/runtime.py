@@ -35,6 +35,51 @@ def _chk_f32(t, name, ndim=None):
     return t.contiguous()
 
 
+def frame_shape(pixel_format, H, W):
+    """The tensor shape of one H x W frame in pixel_format (include/hand3d_b200.h's table): rgb / bgr (H, W, 3), nv12 / i420
+    (H * 3 / 2, W) with H and W even, yuyv (H, W, 2) with W even."""
+    if pixel_format not in _lib.PIXEL_FORMATS:
+        raise ValueError("pixel_format must be one of %s, got %r" % (sorted(_lib.PIXEL_FORMATS), pixel_format))
+    H, W = int(H), int(W)
+    if pixel_format in ("nv12", "i420"):
+        if H % 2 or W % 2:
+            raise ValueError("%s frames must have an even height and width, got %dx%d" % (pixel_format, H, W))
+        return (H * 3 // 2, W)
+    if pixel_format == "yuyv":
+        if W % 2:
+            raise ValueError("yuyv frames must have an even width, got %d" % W)
+        return (H, W, 2)
+    return (H, W, 3)
+
+
+def _frames_bhw(frames, pixel_format):
+    """A CUDA uint8 batch of frames in pixel_format -> (B, H, W) of its pictures; the sizes themselves are checked by the C entry."""
+    if pixel_format not in _lib.PIXEL_FORMATS:
+        raise ValueError("pixel_format must be one of %s, got %r" % (sorted(_lib.PIXEL_FORMATS), pixel_format))
+    if not isinstance(frames, torch.Tensor):
+        raise TypeError("frames must be a torch.Tensor")
+    if not frames.is_cuda:
+        raise RuntimeError("frames must live on a CUDA device (hand3d_b200 has no CPU path)")
+    if frames.dtype != torch.uint8:
+        raise TypeError("frames must be uint8, got %s" % frames.dtype)
+    shp = tuple(frames.shape)
+    if pixel_format in ("nv12", "i420"):
+        if len(shp) != 3 or shp[1] % 3:
+            raise ValueError("%s frames must be [B,H*3/2,W], got %s" % (pixel_format, shp))
+        B, H, W = shp[0], shp[1] * 2 // 3, shp[2]
+    elif pixel_format == "yuyv":
+        if len(shp) != 4 or shp[3] != 2:
+            raise ValueError("yuyv frames must be [B,H,W,2], got %s" % (shp,))
+        B, H, W = shp[:3]
+    else:
+        if len(shp) != 4 or shp[3] != 3:
+            raise ValueError("frames must be [B,H,W,3] %s, got %s" % (pixel_format.upper(), shp))
+        B, H, W = shp[:3]
+    if not frames.is_contiguous():
+        raise ValueError("frames must be contiguous")
+    return B, H, W
+
+
 def _chk_params(params, B):
     if params is None:
         return None
@@ -626,28 +671,32 @@ class Context:
                    "h3d_resize_bilinear_tf1")
         return y
 
-    def resize_frames(self, frames, out_h, out_w, normalize, out=None):
-        """run.py:57-59 on the device: frames uint8 CUDA [B,H,W,3] (contiguous RGB) -> [B,out_h,out_w,3], uint8 scipy.misc.imresize
-        bytes (Pillow BILINEAR) or, with normalize, float32 u / 255.0 - 0.5 computed in double.  The first call with a new size builds
-        its plan (not under graph capture); later calls only enqueue one kernel."""
-        if not isinstance(frames, torch.Tensor):
-            raise TypeError("frames must be a torch.Tensor")
-        if not frames.is_cuda:
-            raise RuntimeError("frames must live on a CUDA device (hand3d_b200 has no CPU path)")
-        if frames.dtype != torch.uint8:
-            raise TypeError("frames must be uint8, got %s" % frames.dtype)
-        if frames.dim() != 4 or frames.shape[3] != 3:
-            raise ValueError("frames must be [B,H,W,3] RGB, got %s" % (tuple(frames.shape),))
-        if not frames.is_contiguous():
-            raise ValueError("frames must be contiguous")
-        B, H, W, _ = frames.shape
+    def resize_frames(self, frames, out_h, out_w, normalize, out=None, pixel_format="rgb"):
+        """run.py:57-59 on the device: frames uint8 CUDA (contiguous; [B,H,W,3] RGB, or pixel_format's layout, see frame_shape) ->
+        [B,out_h,out_w,3], uint8 scipy.misc.imresize bytes (Pillow BILINEAR) of the RGB frames or, with normalize, float32 u / 255.0 - 0.5
+        computed in double.  Other formats are converted to RGB inside the kernel first (OpenCV's cvtColor rule,
+        include/hand3d_b200.h).  The first call with a new format and size builds its plan (not under graph capture); later calls only
+        enqueue one kernel."""
+        B, H, W = _frames_bhw(frames, pixel_format)
         dt = torch.float32 if normalize else torch.uint8
         if out is None:
             out = torch.empty((B, int(out_h), int(out_w), 3), dtype=dt, device=frames.device)
         elif out.dtype != dt or tuple(out.shape) != (B, int(out_h), int(out_w), 3) or not out.is_contiguous() or out.device != frames.device:
             raise ValueError("out must be a contiguous %s tensor [%d,%d,%d,3] on the frames' device" % (dt, B, out_h, out_w))
-        _lib.check(self.lib.h3d_resize_frames(self.h, _ptr(frames), B, H, W, int(out_h), int(out_w), int(bool(normalize)), _ptr(out),
-                                              _stream()), "h3d_resize_frames")
+        _lib.check(self.lib.h3d_resize_frames_fmt(self.h, _ptr(frames), _lib.PIXEL_FORMATS[pixel_format], B, H, W, int(out_h), int(out_w),
+                                                  int(bool(normalize)), _ptr(out), _stream()), "h3d_resize_frames_fmt")
+        return out
+
+    def convert_frames(self, frames, pixel_format, out=None):
+        """h3d_convert_frames: frames uint8 CUDA in pixel_format's layout -> uint8 RGB [B,H,W,3] at full size (OpenCV's cvtColor
+        rule).  With `out` (contiguous uint8 [B,H,W,3]) it writes there and allocates nothing, so it can be captured."""
+        B, H, W = _frames_bhw(frames, pixel_format)
+        if out is None:
+            out = torch.empty((B, H, W, 3), dtype=torch.uint8, device=frames.device)
+        elif out.dtype != torch.uint8 or tuple(out.shape) != (B, H, W, 3) or not out.is_contiguous() or out.device != frames.device:
+            raise ValueError("out must be a contiguous uint8 tensor [%d,%d,%d,3] on the frames' device" % (B, H, W))
+        _lib.check(self.lib.h3d_convert_frames(self.h, _ptr(frames), _lib.PIXEL_FORMATS[pixel_format], B, H, W, _ptr(out), _stream()),
+                   "h3d_convert_frames")
         return out
 
     def draw_segments(self, images, segments, colors, linewidth=1.0, valid=None):

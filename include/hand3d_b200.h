@@ -452,6 +452,33 @@ H3D_API int h3d_decode_records_gather(h3d_ctx* ctx, int dataset, const uint8_t* 
 #define H3D_FRAME_MAX_OUT 512
 H3D_API int h3d_resize_frames(h3d_ctx* ctx, const uint8_t* frames, int B, int H, int W, int out_h, int out_w, int normalize, void* out,
                               void* stream);
+/* Pixel formats of camera frames (B frames back to back, contiguous, uint8; H x W is the picture):
+ *   H3D_PIXEL_RGB   [B,H,W,3] packed R G B (h3d_resize_frames' input)            1 <= H, W <= H3D_FRAME_MAX_SIDE
+ *   H3D_PIXEL_BGR   [B,H,W,3] packed B G R (OpenCV's VideoCapture)               1 <= H, W <= H3D_FRAME_MAX_SIDE
+ *   H3D_PIXEL_NV12  [B,H*3/2,W]: H rows of Y, then H/2 rows of interleaved U V   H, W even, 2..H3D_FRAME_MAX_SIDE
+ *   H3D_PIXEL_I420  [B,H*3/2,W] as flat bytes: H*W of Y, then (H/2)(W/2) of U, then (H/2)(W/2) of V (ffmpeg's yuv420p)
+ *                                                                                H, W even, 2..H3D_FRAME_MAX_SIDE
+ *   H3D_PIXEL_YUYV  [B,H,W,2]: Y0 U Y1 V per pixel pair (YUY2, ffmpeg's yuyv422) 1 <= H <= H3D_FRAME_MAX_SIDE, W even, 2..H3D_FRAME_MAX_SIDE
+ * The YUV formats are converted to RGB as OpenCV's cvtColor COLOR_YUV2RGB_NV12 / _I420 / _YUYV converts them: BT.601 limited range in
+ * 20-bit fixed point, chroma replicated (not interpolated).  Pixel (y, x) takes its luma Y and the chroma (U, V) at (y/2, x/2) (4:2:0) or
+ * (y, x/2) (YUYV); c = max(Y - 16, 0) * 1220542 + (1 << 19), u = U - 128, v = V - 128, and with an arithmetic shift, clipped to 0..255:
+ *   R = (c + 1673527 v) >> 20,   G = (c - 852492 v - 409993 u) >> 20,   B = (c + 2116026 u) >> 20.
+ * This is not ffmpeg/swscale's rgb24 conversion, which rounds and interpolates chroma differently. */
+#define H3D_PIXEL_RGB 0
+#define H3D_PIXEL_BGR 1
+#define H3D_PIXEL_NV12 2
+#define H3D_PIXEL_I420 3
+#define H3D_PIXEL_YUYV 4
+/* h3d_resize_frames of frames in `format` (H3D_PIXEL_*): out is Pillow's BILINEAR resize (and with normalize = 1 run.py's
+ * normalisation) of the frames converted to RGB by the rule above, bit for bit; BGR is the resize of the channel-reversed frame.  With
+ * H3D_PIXEL_RGB it is h3d_resize_frames.  The conversion is fused into the resize kernel (one instance per format), so nothing but `out`
+ * is written.  Sizes per the table above and 1 <= out_h, out_w <= H3D_FRAME_MAX_OUT, anything else (or an unknown format) is H3D_EINVAL
+ * before anything is enqueued.  Plans are kept per (format, H, W, out_h, out_w) and built as h3d_resize_frames builds them. */
+H3D_API int h3d_resize_frames_fmt(h3d_ctx* ctx, const uint8_t* frames, int format, int B, int H, int W, int out_h, int out_w, int normalize,
+                                  void* out, void* stream);
+/* frames in `format` -> out_rgb [B,H,W,3] uint8 RGB at full size, by the rule above (RGB: a copy; BGR: the channels reversed).  Sizes
+ * per the table above, else H3D_EINVAL before anything is enqueued.  Enqueues one kernel and allocates nothing (capturable). */
+H3D_API int h3d_convert_frames(h3d_ctx* ctx, const uint8_t* frames, int format, int B, int H, int W, uint8_t* out_rgb, void* stream);
 /* tf.image.random_hue (TF 1.3 adjust_hue, non-fused: rgb_to_hsv, h = mod(h + (delta + 1), 1), hsv_to_rgb, in the functors' fp32 order)
  * and / or the random_crop window, in one pass.  image [B,H,W,3] fp32, hand_parts [B,H,W] u8, params as above (delta at
  * H3D_AUG_HUE_DELTA when flags has H3D_AUG_HUE, window at H3D_AUG_WINDOW when flags has H3D_AUG_RANDOM_CROP) -> out_image [B,h,w,3]
