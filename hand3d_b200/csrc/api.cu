@@ -14,8 +14,10 @@
 
 namespace h3d {
 
-// ------------------------------------------------------------------------------------------ errors
+// ------------------------------------------------------------------------------------------ errors, launch tally
 static thread_local char g_err[1024] = "";
+thread_local int64_t t_launches = 0;
+static thread_local int t_guard_depth = 0;   // DeviceGuards alive on this thread (entries that call entries nest them)
 void set_error(const char* fmt, ...) {
     va_list ap;
     va_start(ap, fmt);
@@ -111,16 +113,20 @@ using StepFn = std::function<int(const Ext&, cudaStream_t)>;
 
 enum StepKind { KIND_TC = 0, KIND_DIRECT = 1, KIND_FC = 2, KIND_OTHER = 3, KIND_COUNT = 4 };
 
+struct Step {
+    StepFn fn;
+    int kind = KIND_OTHER;      // StepKind (profiling)
+    int64_t flops = 0;          // algorithmic FLOPs
+    int lane = 0;               // 0 = caller's stream, 1 = the context's side stream (independent branch)
+    bool join_before = false;   // wait for the side stream before this step
+};
+
 struct StagePlan {
-    std::vector<StepFn> steps;
-    std::vector<int> launches;          // kernels per step
-    std::vector<int> kinds;             // StepKind per step (profiling)
-    std::vector<int64_t> step_flops;    // algorithmic FLOPs per step
+    std::vector<Step> steps;
     std::vector<TcConvPlan*> tc;
     std::vector<FcChainPlan*> fc;
-    std::vector<int> lane;              // per step: 0 = caller's stream, 1 = the context's side stream (independent branch)
-    std::vector<char> join_before;      // per step: wait for the side stream before this step
-    int cur_lane = 0;                   // lane given to steps as they are appended (see seal())
+    int cur_lane = 0;           // lane of the steps appended next
+    bool join_next = false;     // the next step appended waits for the side stream
     int B = 0, H = 0, W = 0, variant = -1;
     int64_t flops = 0;
     // counted plan (HandSegNet for the slots a slots step re-detects): every kernel computes only images [0, *count), and the first layer
@@ -131,11 +137,10 @@ struct StagePlan {
         for (auto* p : tc) tc_conv_plan_destroy(p);
         for (auto* p : fc) fc_chain_plan_destroy(p);
     }
-    // label every step appended since the last call with the current lane
-    void seal(bool join = false) {
-        const size_t first = lane.size();
-        while (lane.size() < steps.size()) { lane.push_back(cur_lane); join_before.push_back(0); }
-        if (join && first < steps.size()) join_before[first] = 1;
+    Step& add(StepFn fn) {
+        steps.push_back({std::move(fn), KIND_OTHER, 0, cur_lane, join_next});
+        join_next = false;
+        return steps.back();
     }
 };
 
@@ -294,14 +299,24 @@ static void free_packed(PackedW& p) {
     p = PackedW();
 }
 
-// RAII: make ctx's device current for the duration of an entry point and restore the caller's device afterwards (one process may
-// hold contexts on several GPUs; torch keeps its own notion of the current device).
+// RAII of every entry point that takes a context (ctx may be NULL): makes ctx's device current for the duration of the entry and
+// restores the caller's device afterwards (one process may hold contexts on several GPUs; torch keeps its own notion of the current
+// device).  The outermost guard on the thread adds the kernels enqueued meanwhile (t_launches) to ctx's launch count, whatever the
+// entry returns; an entry called by another entry is counted by its caller's guard.
 struct DeviceGuard {
+    h3d_ctx* ctx;
+    int64_t launches0 = t_launches;
+    bool outer = t_guard_depth++ == 0;
     int prev = -1; bool switched = false;
-    explicit DeviceGuard(int dev) {
+    explicit DeviceGuard(h3d_ctx* c) : ctx(c) {
+        const int dev = c ? c->device : 0;
         if (cudaGetDevice(&prev) == cudaSuccess && prev != dev) switched = cudaSetDevice(dev) == cudaSuccess;
     }
-    ~DeviceGuard() { if (switched) cudaSetDevice(prev); }
+    ~DeviceGuard() {
+        --t_guard_depth;
+        if (outer && ctx) ctx->launches += t_launches - launches0;
+        if (switched) cudaSetDevice(prev);
+    }
 };
 
 static int op_scratch(h3d_ctx* ctx, int64_t bytes, char** out) {
@@ -429,11 +444,6 @@ static Act slot_view(char* p, int64_t elems, int C, bool split, int passes) {
     return a;
 }
 
-static void tag(StagePlan* pl, int kind, int64_t flops) {
-    while (pl->kinds.size() + 1 < pl->launches.size()) { pl->kinds.push_back(KIND_OTHER); pl->step_flops.push_back(0); }
-    pl->kinds.push_back(kind); pl->step_flops.push_back(flops);
-}
-
 static int add_direct(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, const LayerSpec& l, int B, int H, int W,
                       const float* x /*null -> Ext.in*/, int Cin_total, int cin_off, float* y, int Cout_total, int cout_off,
                       Split ys, int Cs_total, int cs_off, float* splitk_scratch = nullptr) {
@@ -449,15 +459,14 @@ static int add_direct(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, con
     a.err_flag = ctx->err_flag;
     a.count = pl->count;
     a.slots = x ? nullptr : pl->slots;   // the plan's external input is indexed through the slot list
-    pl->steps.push_back([a](const Ext& e, cudaStream_t s) {
+    Step& st = pl->add([a](const Ext& e, cudaStream_t s) {
         DirectConvArgs aa = a;
         if (!aa.x) aa.x = e.in;
         return launch_conv_direct(aa, s);
     });
-    pl->launches.push_back(conv_direct_num_launches(a));
     const int64_t fl = 2ll * B * ceil_div(H, l.stride) * ceil_div(W, l.stride) * l.k * l.k * l.cin * l.cout;
     pl->flops += fl;
-    tag(pl, KIND_DIRECT, fl);
+    st.kind = KIND_DIRECT; st.flops = fl;
     return H3D_OK;
 }
 
@@ -480,11 +489,10 @@ static int add_tc(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, const L
     TcConvPlan* tp = tc_conv_plan_create(d, &rc);
     if (!tp) return rc;
     pl->tc.push_back(tp);
-    pl->steps.push_back([tp](const Ext&, cudaStream_t s) { return tc_conv_launch(tp, s); });
-    pl->launches.push_back(1);
+    Step& st = pl->add([tp](const Ext&, cudaStream_t s) { return tc_conv_launch(tp, s); });
     const int64_t fl = 2ll * B * H * W * l.k * l.k * l.cin * l.cout / (pool == 2 ? 4 : 1);
     pl->flops += fl;
-    tag(pl, KIND_TC, fl);
+    st.kind = KIND_TC; st.flops = fl;
     return H3D_OK;
 }
 
@@ -524,9 +532,8 @@ static int build_trunk(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, co
             const int hh = h, ww = w, cc = l.cout;
             if (tc && lo == 4) { set_error("fp16_f8c: max-pool must be fused into the convolution (even H, W required)"); return H3D_EINVAL; }
             const int* cnt = pl->count;
-            if (tc) pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_maxpool_split(src.s, pooled.s, B, hh, ww, cc, half, s, cnt); });
-            else pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_maxpool_f32(src.f, pooled.f, B, hh, ww, cc, s, cnt); });
-            pl->launches.push_back(1);
+            if (tc) pl->add([=](const Ext&, cudaStream_t s) { return launch_maxpool_split(src.s, pooled.s, B, hh, ww, cc, half, s, cnt); });
+            else pl->add([=](const Ext&, cudaStream_t s) { return launch_maxpool_f32(src.f, pooled.f, B, hh, ww, cc, s, cnt); });
             in = pooled; cur ^= 1; h /= 2; w /= 2;
         }
     }
@@ -560,8 +567,7 @@ static int build_handsegnet(h3d_ctx* ctx, int B, int H, int W, const int* count 
     }
     // e.out == nullptr (pipeline): the x8 up-sampling is fused into the mask post-processing (launch_seg_postprocess reads seg_low)
     const int* cnt = pl->count;
-    pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return e.out ? launch_resize_bilinear_tf1(low, e.out, B, h, w, 2, H, W, s, cnt) : H3D_OK; });
-    pl->launches.push_back(1);
+    pl->add([=](const Ext& e, cudaStream_t s) { return e.out ? launch_resize_bilinear_tf1(low, e.out, B, h, w, 2, H, W, s, cnt) : H3D_OK; });
     (count ? ctx->seg_counted : ctx->seg) = std::move(pl);
     return H3D_OK;
 }
@@ -591,13 +597,12 @@ static int build_posenet(h3d_ctx* ctx, int B, int Hc, int Wc) {
     else { cb.C = 149; cb.f = (float*)cbuf; }
     if (tc) {
         const Split cs = cb.s; const size_t bytes = (size_t)pix * 192 * 2;
-        pl->steps.push_back([=](const Ext&, cudaStream_t s) {   // zero the padding channels (and everything else) once per call
+        pl->add([=](const Ext&, cudaStream_t s) {   // zero the padding channels (and everything else) once per call
             H3D_CUDA(cudaMemsetAsync(cs.hi, 0, bytes, s));
             if (cs.lo) H3D_CUDA(cudaMemsetAsync(cs.lo, 0, bytes, s));
             if (cs.l8) { H3D_CUDA(cudaMemsetAsync(cs.l8, 0, bytes / 2, s)); H3D_CUDA(cudaMemsetAsync(cs.h8, 0, bytes / 2, s)); }
             return H3D_OK;
         });
-        pl->launches.push_back(0);
     }
     if ((rc = build_trunk(ctx, pl.get(), "PoseNet2D", kPoseTrunk, 15, B, Hc, Wc, slot0, slot1, se, &last, &h, &w, &cb, tc ? 0 : 21))) return rc;
     float** S = ctx->lay.s;
@@ -616,8 +621,7 @@ static int build_posenet(h3d_ctx* ctx, int B, int Hc, int Wc) {
         if (rc2) return rc2;
         if (!tc && feed_back) {
             float* dst = cb.f;
-            pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_copy_channels(sm_out, dst, pix, 21, 149, 0, s); });
-            pl->launches.push_back(1);
+            pl->add([=](const Ext&, cudaStream_t s) { return launch_copy_channels(sm_out, dst, pix, 21, 149, 0, s); });
         }
         return H3D_OK;
     };
@@ -670,10 +674,9 @@ static int add_fc(h3d_ctx* ctx, StagePlan* pl, const std::string& name, const fl
     int rc;
     if ((rc = dev_weight(ctx, name + "/weights", &w))) return rc;
     if ((rc = dev_weight(ctx, name + "/biases", &b))) return rc;
-    pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_fc(x, w, b, y, scratch, scratch_floats, B, in_f, out_f, leaky, in_f, s); });
-    pl->launches.push_back(2);
+    Step& st = pl->add([=](const Ext&, cudaStream_t s) { return launch_fc(x, w, b, y, scratch, scratch_floats, B, in_f, out_f, leaky, in_f, s); });
     pl->flops += 2ll * B * in_f * out_f;
-    tag(pl, KIND_FC, 2ll * B * in_f * out_f);
+    st.kind = KIND_FC; st.flops = 2ll * B * in_f * out_f;
     return H3D_OK;
 }
 
@@ -710,9 +713,7 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
     if (tc_lift) {
         xin = slot_view(slot_in, (int64_t)B * 32 * 32 * 64, 64, true, passes);
         const Split xs = xin.s;
-        pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_f32_to_split(e.in, xs, (int64_t)B * 32 * 32, 21, 64, half, s); });
-        pl->launches.push_back(1);
-        pl->seal();
+        pl->add([=](const Ext& e, cudaStream_t s) { return launch_f32_to_split(e.in, xs, (int64_t)B * 32 * 32, 21, 64, half, s); });
     }
     // returns the flattened NHWC fp32 feature map [B, 4*4*C] in *feat
     auto pyramid = [&](const std::string& scope, const LayerSpec* L, const Branch& b, float** feat) -> int {
@@ -774,10 +775,9 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
         const Split ys = y ? y->s : Split();
         const int stride = y ? y->stride : 0;
         float* yf = y ? nullptr : x;
-        pl->steps.push_back([=](const Ext&, cudaStream_t s) {
+        pl->add([=](const Ext&, cudaStream_t s) {
             return launch_dropout(x, B, cols, keep_prob, layer, cx->drop_seed, draw, yf, nullptr, ys, stride, half, s);
         });
-        pl->launches.push_back(1);
     };
     // the tensor-core hidden layer: straight into the next layer's planes, or with dropout through fp32 t
     auto fc_tc_hidden = [&](const std::string& scope, const char* name, int in_f, int out_f, const Planes& x, const Planes& y, float* t,
@@ -817,9 +817,7 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
             if ((rc = pyramid("ViewpointNet", kViewpoint, b, &feat))) return rc;
             char* cur = b.slot[0];
             const Planes xp = carve_planes(cur, 4098), p1 = carve_planes(cur, 256), p2 = carve_planes(cur, 128);
-            pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 4096, xp.stride, half, s); });
-            pl->launches.push_back(1);
-            pl->seal();
+            pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 4096, xp.stride, half, s); });
             pl->cur_lane = 0;
             if ((rc = fc_layer(chains[1], "ViewpointNet", "fc_vp0", 4098, 256, 1, xp, &p1, nullptr, 0))) return rc;
             if ((rc = fc_layer(chains[1], "ViewpointNet", "fc_vp1", 256, 128, 1, p1, &p2, nullptr, 0))) return rc;
@@ -831,8 +829,7 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
             if ((rc = pyramid("PosePrior", kPosePrior, b, &feat))) return rc;
             char* cur = b.slot[0];
             const Planes xp = carve_planes(cur, 2050), p1 = carve_planes(cur, 512), p2 = carve_planes(cur, 512), p3 = carve_planes(cur, 64);
-            pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 2048, xp.stride, half, s); });
-            pl->launches.push_back(1);
+            pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 2048, xp.stride, half, s); });
             if ((rc = fc_layer(chains[0], "PosePrior", "fc_rel0", 2050, 512, 1, xp, &p1, nullptr, 0))) return rc;
             if ((rc = fc_layer(chains[0], "PosePrior", "fc_rel1", 512, 512, 1, p1, &p2, nullptr, 0))) return rc;
             if (bott) {
@@ -841,13 +838,13 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
             } else {
                 if ((rc = fc_layer(chains[0], "PosePrior", "fc_xyz", 512, 63, 0, p2, nullptr, can, 63))) return rc;
             }
-            pl->seal();
         }
         FcChainPlan* fp = fc_chain_plan_create(chains, proposed ? 2 : 1, B, half, can, uxyz, ctx->fc_counter, ctx->err_flag);
         if (!fp) return H3D_ECUDA;
         pl->fc.push_back(fp);
         const int var = variant;
-        pl->steps.push_back([=](const Ext& e, cudaStream_t s) {
+        pl->join_next = true;                                 // joins the ViewpointNet branch before the launch
+        Step& st = pl->add([=](const Ext& e, cudaStream_t s) {
             int rc2 = fc_chain_launch(fp, e.hand_side, var == H3D_VARIANT_PROPOSED ? e.out3 : nullptr, var == H3D_VARIANT_PROPOSED ? e.out : nullptr, s);
             if (rc2) return rc2;
             if (var == H3D_VARIANT_LOCAL) {
@@ -858,10 +855,8 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
             if (e.out2) H3D_CUDA(cudaMemcpyAsync(e.out2, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
             return H3D_OK;
         });
-        pl->launches.push_back(variant == H3D_VARIANT_LOCAL ? 2 : 1);
         pl->flops += fl;
-        tag(pl.get(), KIND_TC, fl);
-        pl->seal(true);                                       // joins the ViewpointNet branch before the launch
+        st.kind = KIND_TC; st.flops = fl;
         ctx->lift = std::move(pl);
         return H3D_OK;
     }
@@ -875,8 +870,7 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
         if (tc_lift) {   // slot[0] (layer-4 output, dead by now) holds the FC activations
             char* cur = b.slot[0];
             const Planes xp = carve_planes(cur, 2050), p1 = carve_planes(cur, 512), p2 = carve_planes(cur, 512), p3 = carve_planes(cur, 64);
-            pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 2048, xp.stride, half, s); });
-            pl->launches.push_back(1);
+            pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 2048, xp.stride, half, s); });
             if ((rc2 = fc_tc_hidden("PosePrior", "fc_rel0", 2050, 512, xp, p1, b.t1, 0.8f, H3D_DROPOUT_LAYER_FC_REL0))) return rc2;
             if ((rc2 = fc_tc_hidden("PosePrior", "fc_rel1", 512, 512, p1, p2, b.t2, 0.8f, H3D_DROPOUT_LAYER_FC_REL1))) return rc2;
             if (bott) {
@@ -886,8 +880,7 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
             return fc_tc("PosePrior", "fc_xyz", 512, 63, 0, p2, nullptr, can);
         }
         float* xcat = b.xcat;
-        pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_concat_handside(feat, e.hand_side, xcat, B, 2048, s); });
-        pl->launches.push_back(1);
+        pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside(feat, e.hand_side, xcat, B, 2048, s); });
         if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_rel0", b.xcat, b.t1, b.fcs, fcs_floats, B, 2050, 512, 1))) return rc2;
         if (drop) add_dropout(b.t1, 512, 0.8f, H3D_DROPOUT_LAYER_FC_REL0, nullptr);
         if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_rel1", b.t1, b.t2, b.fcs, fcs_floats, B, 512, 512, 1))) return rc2;
@@ -911,14 +904,12 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
         if (tc_lift) {
             char* cur = b.slot[0];
             const Planes xp = carve_planes(cur, 4098), p1 = carve_planes(cur, 256);
-            pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 4096, xp.stride, half, s); });
-            pl->launches.push_back(1);
+            pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 4096, xp.stride, half, s); });
             if ((rc = fc_tc_hidden("ViewpointNet", "fc_vp0", 4098, 256, xp, p1, b.t1, 0.75f, H3D_DROPOUT_LAYER_FC_VP0))) return rc;
             if ((rc = fc_tc("ViewpointNet", "fc_vp1", 256, 128, 1, p1, nullptr, b.t2))) return rc;   // fp32 [B,128] for the three 128 -> 1 heads
         } else {
             float* xcat = b.xcat;
-            pl->steps.push_back([=](const Ext& e, cudaStream_t s) { return launch_concat_handside(feat, e.hand_side, xcat, B, 4096, s); });
-            pl->launches.push_back(1);
+            pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside(feat, e.hand_side, xcat, B, 4096, s); });
             if ((rc = add_fc(ctx, pl.get(), "ViewpointNet/fc_vp0", b.xcat, b.t1, b.fcs, fcs_floats, B, 4098, 256, 1))) return rc;
             if (drop) add_dropout(b.t1, 256, 0.75f, H3D_DROPOUT_LAYER_FC_VP0, nullptr);
             if ((rc = add_fc(ctx, pl.get(), "ViewpointNet/fc_vp1", b.t1, b.t2, b.fcs, fcs_floats, B, 256, 128, 1))) return rc;
@@ -926,44 +917,34 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
         if (drop) add_dropout(b.t2, 128, 0.75f, H3D_DROPOUT_LAYER_FC_VP1, nullptr);
         const float* hw = ctx->vp_head_w; const float* hb = ctx->vp_head_b;
         float* t2 = b.t2; float* fcs = b.fcs;
-        pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_fc(t2, hw, hb, uxyz, fcs, fcs_floats, B, 128, 3, 0, 128, s); });
-        pl->launches.push_back(2);
-        tag(pl.get(), KIND_FC, 2ll * B * 128 * 3);
-        pl->seal();
+        Step& st = pl->add([=](const Ext&, cudaStream_t s) { return launch_fc(t2, hw, hb, uxyz, fcs, fcs_floats, B, 128, 3, 0, 128, s); });
+        st.kind = KIND_FC; st.flops = 2ll * B * 128 * 3;
         pl->cur_lane = 0;
     }
     if ((rc = pose_prior())) return rc;
-    pl->seal();
     if (variant == H3D_VARIANT_PROPOSED) {
         // Rodrigues / flip / rotate (:239-247,311-334): needs both branches
-        pl->steps.push_back([=](const Ext& e, cudaStream_t s) {
+        pl->join_next = true;
+        pl->add([=](const Ext& e, cudaStream_t s) {
             if (e.out2) H3D_CUDA(cudaMemcpyAsync(e.out2, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
             return launch_rotate_canonical(can, uxyz, e.hand_side, B, e.out3, e.out, s);
         });
-        pl->launches.push_back(1);
-        pl->seal(true);
     } else if (variant == H3D_VARIANT_LOCAL) {
         // nets/PosePriorNetwork.py:70-75: the network predicts bone-relative coordinates; assemble xyz by forward kinematics
-        pl->steps.push_back([=](const Ext& e, cudaStream_t s) {
+        pl->add([=](const Ext& e, cudaStream_t s) {
             if (e.out2) H3D_CUDA(cudaMemcpyAsync(e.out2, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
             return launch_bone_rel_trafo_inv(can, e.out, B, s);
         });
-        pl->launches.push_back(1);
-        pl->seal();
     } else {
-        pl->steps.push_back([=](const Ext& e, cudaStream_t s) {
+        pl->add([=](const Ext& e, cudaStream_t s) {
             H3D_CUDA(cudaMemcpyAsync(e.out, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
             if (e.out2) H3D_CUDA(cudaMemcpyAsync(e.out2, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
             return H3D_OK;
         });
-        pl->launches.push_back(0);
-        pl->seal();
     }
     if (drop) {   // after the join: every dropout layer of this forward has read the draw
         int64_t* draw = ctx->drop_draw;
-        pl->steps.push_back([=](const Ext&, cudaStream_t s) { return launch_dropout_advance(draw, s); });
-        pl->launches.push_back(1);
-        pl->seal();
+        pl->add([=](const Ext&, cudaStream_t s) { return launch_dropout_advance(draw, s); });
         ctx->lift_drop = std::move(pl);
         return H3D_OK;
     }
@@ -981,28 +962,31 @@ static int run_plan(h3d_ctx* ctx, StagePlan* pl, const Ext& e, cudaStream_t s) {
         return H3D_OK;
     };
     const bool lanes = !tc_tuning().no_side_stream;
-    for (size_t i = 0; i < pl->steps.size(); ++i) {
+    for (const Step& step : pl->steps) {
         int rc;
-        const int ln = (lanes && i < pl->lane.size()) ? pl->lane[i] : 0;
-        if (i < pl->join_before.size() && pl->join_before[i] && (rc = join())) return rc;
+        const int ln = lanes ? step.lane : 0;
+        if (step.join_before && (rc = join())) return rc;
         if (ln == 1 && !forked) {   // the branch starts from everything enqueued on the caller's stream so far
             H3D_CUDA(cudaEventRecord(ctx->ev_fork, s));
             H3D_CUDA(cudaStreamWaitEvent(ctx->side, ctx->ev_fork, 0));
             forked = true;
         }
         cudaStream_t st = ln == 1 ? ctx->side : s;
-        h3d_ctx::ProfRec pr;
-        const bool prof = ctx->profiling && pl->launches[i] > 0;
-        if (prof) {
+        h3d_ctx::ProfRec pr{nullptr, nullptr, step.kind, step.flops};
+        if (ctx->profiling) {
             H3D_CUDA(cudaEventCreate(&pr.a)); H3D_CUDA(cudaEventCreate(&pr.b));
-            pr.kind = i < pl->kinds.size() ? pl->kinds[i] : KIND_OTHER;
-            pr.flops = i < pl->step_flops.size() ? pl->step_flops[i] : 0;
             H3D_CUDA(cudaEventRecord(pr.a, st));
         }
-        rc = pl->steps[i](e, st);
+        const int64_t launches0 = t_launches;
+        rc = step.fn(e, st);
         if (rc) { join(); return rc; }
-        if (prof) { H3D_CUDA(cudaEventRecord(pr.b, st)); ctx->prof.push_back(pr); }
-        ctx->launches += pl->launches[i];
+        if (!pr.a) continue;
+        if (t_launches > launches0) {   // steps that only set or copy memory are not profiled
+            H3D_CUDA(cudaEventRecord(pr.b, st));
+            ctx->prof.push_back(pr);
+        } else {
+            cudaEventDestroy(pr.a); cudaEventDestroy(pr.b);
+        }
     }
     return join();
 }
@@ -1093,7 +1077,8 @@ int h3d_check_errors(h3d_ctx* ctx, int* code) {
 
 int h3d_destroy(h3d_ctx* ctx) {
     if (!ctx) return H3D_OK;
-    DeviceGuard guard(ctx->device);
+    std::unique_ptr<h3d_ctx> owned(ctx);   // deleted after the guard has ended: the guard's end writes ctx->launches
+    DeviceGuard guard(ctx);
     ctx->drop_plans();
     for (auto& kv : ctx->dev_w) cudaFree(kv.second);
     for (auto& kv : ctx->packed) free_packed(kv.second);
@@ -1111,7 +1096,6 @@ int h3d_destroy(h3d_ctx* ctx) {
     if (ctx->track_sel) cudaFree(ctx->track_sel);
     if (ctx->track_crop) cudaFree(ctx->track_crop);
     for (auto& kv : ctx->frame_plans) frame_plan_destroy(kv.second);
-    delete ctx;
     return H3D_OK;
 }
 
@@ -1229,7 +1213,7 @@ int h3d_set_workspace(h3d_ctx* ctx, void* dev_ptr, int64_t bytes) {
 int h3d_fill_scratch(h3d_ctx* ctx, int byte, void* stream) {
     H3D_REQUIRE(ctx != nullptr, "h3d_fill_scratch: ctx is NULL");
     H3D_REQUIRE(byte >= 0 && byte <= 255, "h3d_fill_scratch: byte must be 0..255, got %d", byte);
-    DeviceGuard guard_(ctx->device);
+    DeviceGuard guard_(ctx);
     cudaStream_t s = (cudaStream_t)stream;
     if (ctx->op_scratch) H3D_CUDA(cudaMemsetAsync(ctx->op_scratch, byte, (size_t)ctx->op_scratch_bytes, s));
     if (ctx->ws && ctx->ws_bytes > 0) H3D_CUDA(cudaMemsetAsync(ctx->ws, byte, (size_t)ctx->ws_bytes, s));
@@ -1243,19 +1227,17 @@ static int run_handsegnet(h3d_ctx* ctx, const float* image, int B, int H, int W,
     if (!ctx->seg || ctx->seg->B != B || ctx->seg->H != H || ctx->seg->W != W)
         if ((rc = build_handsegnet(ctx, B, H, W))) return rc;
     Ext e; e.in = image; e.out = logits;
-    rc = run_plan(ctx, ctx->seg.get(), e, (cudaStream_t)stream);
-    if (!logits) ctx->launches -= 1;   // the skipped up-sampling step
-    return rc;
+    return run_plan(ctx, ctx->seg.get(), e, (cudaStream_t)stream);
 }
 
 int h3d_handsegnet_forward(h3d_ctx* ctx, const float* image, int B, int H, int W, float* logits, void* stream) {
-    DeviceGuard guard_(ctx ? ctx->device : 0);
+    DeviceGuard guard_(ctx);
     H3D_REQUIRE(ctx && image && logits && B > 0, "h3d_handsegnet_forward: bad argument");
     return run_handsegnet(ctx, image, B, H, W, logits, stream);
 }
 
 int h3d_posenet_forward(h3d_ctx* ctx, const float* image_crop, int B, int Hc, int Wc, float* s0, float* s1, float* s2, void* stream) {
-    DeviceGuard guard_(ctx ? ctx->device : 0);
+    DeviceGuard guard_(ctx);
     H3D_REQUIRE(ctx && image_crop && B > 0, "h3d_posenet_forward: bad argument");
     int rc;
     if ((rc = ensure_layout_covers(ctx, B, 0, 0, Hc, Wc))) return rc;
@@ -1274,22 +1256,19 @@ int h3d_pose2d_forward(h3d_ctx* ctx, const float* image_crop, int B, int Hc, int
                        void* stream) {
     H3D_REQUIRE(ctx && image_crop && B > 0, "h3d_pose2d_forward: bad argument");
     H3D_REQUIRE(keypoints_scoremap || (Hc <= 256 && Wc <= 256), "h3d_pose2d_forward: keypoints_scoremap is required for crops larger than 256x256");
-    DeviceGuard guard_(ctx->device);
+    DeviceGuard guard_(ctx);
     cudaStream_t s = (cudaStream_t)stream;
     int rc;
     if ((rc = h3d_posenet_forward(ctx, image_crop, B, Hc, Wc, nullptr, nullptr, nullptr, stream))) return rc;
     h3d_ctx::Layout& L = ctx->lay;
     float* kps = keypoints_scoremap ? keypoints_scoremap : L.kp_scoremap;
-    int nl = 0;
-    if (keypoints_uv) rc = launch_resize_argmax21(L.s[2], kps, B, Hc / 8, Wc / 8, Hc, Wc, L.argmax_scratch, keypoints_uv, s, &nl);
-    else { rc = launch_resize_bilinear_tf1(L.s[2], kps, B, Hc / 8, Wc / 8, 21, Hc, Wc, s); nl = 1; }
-    ctx->launches += nl;
-    return rc;
+    if (keypoints_uv) return launch_resize_argmax21(L.s[2], kps, B, Hc / 8, Wc / 8, Hc, Wc, L.argmax_scratch, keypoints_uv, s);
+    return launch_resize_bilinear_tf1(L.s[2], kps, B, Hc / 8, Wc / 8, 21, Hc, Wc, s);
 }
 
 int h3d_lifting_forward(h3d_ctx* ctx, const float* scoremap32, const float* hand_side, int B, int variant,
                         float* coord_xyz_rel_normed, float* coord_can, float* rot_mat, void* stream) {
-    DeviceGuard guard_(ctx ? ctx->device : 0);
+    DeviceGuard guard_(ctx);
     H3D_REQUIRE(ctx && scoremap32 && hand_side && coord_xyz_rel_normed && B > 0, "h3d_lifting_forward: bad argument");
     H3D_REQUIRE(variant >= H3D_VARIANT_DIRECT && variant <= H3D_VARIANT_LOCAL, "h3d_lifting_forward: unknown variant");
     int rc;
@@ -1307,10 +1286,9 @@ static int pipeline_tail(h3d_ctx* ctx, const float* image, const float* hand_sid
                          const float* scl, float* crop, float* kps, float* keypoint_coord3d, int32_t* keypoints_uv, void* stream) {
     cudaStream_t s = (cudaStream_t)stream;
     h3d_ctx::Layout& L = ctx->lay;
-    int rc = H3D_OK, nl = 0;
+    int rc = H3D_OK;
     // crop_image_from_xy (nets/...:86)
     if ((rc = launch_crop_image(image, cen, scl, crop, B, H, W, 3, 256, s))) return rc;
-    ctx->launches += 1;
     // PoseNet2D (nets/...:89-90)
     if ((rc = h3d_posenet_forward(ctx, crop, B, 256, 256, nullptr, nullptr, nullptr, stream))) return rc;
     // x8 up-sampling (nets/...:96-97) and detect_keypoints (utils/general.py:331-344), fused when both are requested; it only
@@ -1322,15 +1300,8 @@ static int pipeline_tail(h3d_ctx* ctx, const float* image, const float* hand_sid
         H3D_CUDA(cudaStreamWaitEvent(ctx->side2, ctx->ev_fork2, 0));
         us = ctx->side2;
     }
-    int rc_up;
-    if (keypoints_uv) {
-        nl = 0;
-        rc_up = launch_resize_argmax21(L.s[2], kps, B, 32, 32, 256, 256, L.argmax_scratch, keypoints_uv, us, &nl);
-        ctx->launches += nl;
-    } else {
-        rc_up = launch_resize_bilinear_tf1(L.s[2], kps, B, 32, 32, 21, 256, 256, us);
-        ctx->launches += 1;
-    }
+    const int rc_up = keypoints_uv ? launch_resize_argmax21(L.s[2], kps, B, 32, 32, 256, 256, L.argmax_scratch, keypoints_uv, us)
+                                   : launch_resize_bilinear_tf1(L.s[2], kps, B, 32, 32, 21, 256, 256, us);
     if (overlap) H3D_CUDA(cudaEventRecord(ctx->ev_join2, ctx->side2));
     if (rc_up) {   // never leave the side stream un-joined
         if (overlap) cudaStreamWaitEvent(s, ctx->ev_join2, 0);
@@ -1354,7 +1325,7 @@ int h3d_pipeline_forward(h3d_ctx* ctx, const float* image, const float* hand_sid
                          const float* force_center, const float* force_scale, float* hand_scoremap, float* image_crop,
                          float* scale_crop, float* center, float* keypoints_scoremap, float* keypoint_coord3d,
                          int32_t* keypoints_uv, uint8_t* hand_mask, void* stream) {
-    DeviceGuard guard_(ctx ? ctx->device : 0);
+    DeviceGuard guard_(ctx);
     H3D_PIPELINE_CHECKS("h3d_pipeline_forward");
     cudaStream_t s = (cudaStream_t)stream;
     int rc;
@@ -1368,10 +1339,8 @@ int h3d_pipeline_forward(h3d_ctx* ctx, const float* image, const float* hand_sid
     const bool fuse_up = !tc_tuning().no_seg_fusion;
     if ((rc = run_handsegnet(ctx, image, B, H, W, fuse_up ? nullptr : seg, stream))) return rc;
     // single_obj_scoremap + calc_center_bb + scale (nets/...:82-85)
-    int nl = 0;
-    if ((rc = launch_seg_postprocess(seg, B, H, W, L.seg_scratch, hand_mask, nullptr, cen, L.crop_size, scl, s, &nl,
-                                     fuse_up ? L.seg_low : nullptr, H / 8, W / 8))) return rc;
-    ctx->launches += nl;
+    if ((rc = launch_seg_postprocess(seg, B, H, W, L.seg_scratch, hand_mask, nullptr, cen, L.crop_size, scl, s, fuse_up ? L.seg_low : nullptr,
+                                     H / 8, W / 8))) return rc;
     if (force_center) H3D_CUDA(cudaMemcpyAsync(cen, force_center, (size_t)B * 8, cudaMemcpyDeviceToDevice, s));
     if (force_scale) H3D_CUDA(cudaMemcpyAsync(scl, force_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
     return pipeline_tail(ctx, image, hand_side, B, H, W, with_pose3d, cen, scl, image_crop ? image_crop : L.image_crop,
@@ -1390,18 +1359,16 @@ int64_t h3d_track_state_bytes(int B) {
 
 int h3d_track_update(h3d_ctx* ctx, const float* scoremap32, const int32_t* keypoints_uv, const float* center, const float* scale_crop,
                      int B, float margin, float min_score, void* state, void* stream) {
-    DeviceGuard guard_(ctx ? ctx->device : 0);
+    DeviceGuard guard_(ctx);
     H3D_REQUIRE(ctx && scoremap32 && keypoints_uv && center && scale_crop && B > 0, "h3d_track_update: bad argument");
     H3D_TRACK_CHECKS("h3d_track_update");
-    int rc = launch_track_update(scoremap32, keypoints_uv, center, scale_crop, B, margin, min_score, state, (cudaStream_t)stream);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_track_update(scoremap32, keypoints_uv, center, scale_crop, B, margin, min_score, state, (cudaStream_t)stream);
 }
 
 int h3d_track_step(h3d_ctx* ctx, const float* image, const float* hand_side, int B, int H, int W, int with_pose3d, int detect,
                    float margin, float min_score, void* state, float* image_crop, float* scale_crop, float* center,
                    float* keypoints_scoremap, float* keypoint_coord3d, int32_t* keypoints_uv, void* stream) {
-    DeviceGuard guard_(ctx ? ctx->device : 0);
+    DeviceGuard guard_(ctx);
     H3D_PIPELINE_CHECKS("h3d_track_step");
     H3D_TRACK_CHECKS("h3d_track_step");
     cudaStream_t s = (cudaStream_t)stream;
@@ -1422,9 +1389,7 @@ int h3d_track_step(h3d_ctx* ctx, const float* image, const float* hand_side, int
                            keypoints_scoremap ? keypoints_scoremap : L.kp_scoremap, keypoint_coord3d, uv, stream);
     }
     if (rc) return rc;
-    if ((rc = launch_track_update(L.s[2], uv, cen, scl, B, margin, min_score, state, s))) return rc;
-    ctx->launches += 1;
-    return H3D_OK;
+    return launch_track_update(L.s[2], uv, cen, scl, B, margin, min_score, state, s);
 }
 
 // HandSegNet's counted plan for (B, H, W) and the selection memory it reads: built outside any step that could be captured mid-way (a
@@ -1449,7 +1414,7 @@ static int ensure_counted_seg(h3d_ctx* ctx, int B, int H, int W) {
 int h3d_track_step_slots(h3d_ctx* ctx, const float* image, const float* hand_side, int B, int H, int W, int with_pose3d, float margin,
                          float min_score, void* state, const int32_t* force, int32_t* detected, float* image_crop, float* scale_crop,
                          float* center, float* keypoints_scoremap, float* keypoint_coord3d, int32_t* keypoints_uv, void* stream) {
-    DeviceGuard guard_(ctx ? ctx->device : 0);
+    DeviceGuard guard_(ctx);
     H3D_PIPELINE_CHECKS("h3d_track_step_slots");
     H3D_TRACK_CHECKS("h3d_track_step_slots");
     cudaStream_t s = (cudaStream_t)stream;
@@ -1465,26 +1430,19 @@ int h3d_track_step_slots(h3d_ctx* ctx, const float* image, const float* hand_sid
     float* scl_c = ctx->track_crop + 2 * B;
     // 1. the slots to re-detect, from the lost flags the previous step's update wrote (stream order) and the caller's mask
     if ((rc = launch_track_select(state, force, B, ctx->track_sel, detected, s))) return rc;
-    ctx->launches += 1;
     // 2. HandSegNet and the mask post-processing on the selected slots only, in compact order (slot slots[i] -> image i); the x8
     //    up-sampling fused into the post-processing or on its own, as in h3d_pipeline_forward
     const bool fuse_up = !tc_tuning().no_seg_fusion;
     Ext e; e.in = image; e.out = fuse_up ? nullptr : L.hand_scoremap;
     if ((rc = run_plan(ctx, ctx->seg_counted.get(), e, s))) return rc;
-    if (fuse_up) ctx->launches -= 1;   // the skipped up-sampling step
-    int nl = 0;
-    if ((rc = launch_seg_postprocess(L.hand_scoremap, B, H, W, L.seg_scratch, nullptr, nullptr, cen_c, L.crop_size, scl_c, s, &nl,
+    if ((rc = launch_seg_postprocess(L.hand_scoremap, B, H, W, L.seg_scratch, nullptr, nullptr, cen_c, L.crop_size, scl_c, s,
                                      fuse_up ? L.seg_low : nullptr, H / 8, W / 8, count))) return rc;
-    ctx->launches += nl;
     // 3. the step's crop: detected for the selected slots, the state's for the others
     if ((rc = launch_track_merge(state, ctx->track_sel, cen_c, scl_c, B, cen, scl, s))) return rc;
-    ctx->launches += 1;
     // 4. the rest of the pipeline on every slot, then the update
     if ((rc = pipeline_tail(ctx, image, hand_side, B, H, W, with_pose3d, cen, scl, image_crop ? image_crop : L.image_crop,
                             keypoints_scoremap ? keypoints_scoremap : L.kp_scoremap, keypoint_coord3d, uv, stream))) return rc;
-    if ((rc = launch_track_update(L.s[2], uv, cen, scl, B, margin, min_score, state, s))) return rc;
-    ctx->launches += 1;
-    return H3D_OK;
+    return launch_track_update(L.s[2], uv, cen, scl, B, margin, min_score, state, s);
 }
 
 // ---------------------------------------------------------------------------------------------- operators
@@ -1493,7 +1451,7 @@ int h3d_track_step_slots(h3d_ctx* ctx, const float* image, const float* hand_sid
 // frees them around the call (test / tuning entry); its enqueue-only form is h3d_pack_conv_weights + h3d_conv2d_tc_packed.
 #define H3D_OP_PROLOGUE(ctx)                              \
     H3D_REQUIRE((ctx) != nullptr, "ctx is NULL");         \
-    DeviceGuard guard_((ctx)->device);                    \
+    DeviceGuard guard_(ctx);                              \
     cudaStream_t s = (cudaStream_t)stream;
 
 struct h3d_packed_conv { PackedW pw; int k = 0, Cin = 0, Cout = 0, precision = 0; };
@@ -1514,9 +1472,7 @@ int h3d_conv2d_f32(h3d_ctx* ctx, const float* x, const float* w_hwio, const floa
         if (rc0) return rc0;
         a.splitk_scratch = (float*)scratch; a.splitk_scratch_floats = kConvSplitKScratchFloats;
     }
-    int rc = launch_conv_direct(a, s);
-    if (!rc) ctx->launches += conv_direct_num_launches(a);
-    return rc;
+    return launch_conv_direct(a, s);
 }
 
 int h3d_pack_conv_weights(h3d_ctx* ctx, const float* host_w_hwio, const float* host_bias, int ksize, int Cin, int Cout, int precision,
@@ -1524,7 +1480,7 @@ int h3d_pack_conv_weights(h3d_ctx* ctx, const float* host_w_hwio, const float* h
     H3D_REQUIRE(ctx && host_w_hwio && host_bias && out, "h3d_pack_conv_weights: NULL argument");
     H3D_REQUIRE(precision >= H3D_PREC_BF16X3 && precision <= H3D_PREC_FP16_F8C, "h3d_pack_conv_weights: precision must be a tensor-core mode");
     H3D_REQUIRE(ksize == 1 || ksize == 3 || ksize == 5 || ksize == 7, "h3d_pack_conv_weights: ksize must be 1, 3, 5 or 7");
-    DeviceGuard guard(ctx->device);
+    DeviceGuard guard(ctx);
     auto* h = new h3d_packed_conv();
     h->k = ksize; h->Cin = Cin; h->Cout = Cout; h->precision = precision;
     int rc = pack_conv_weights(host_w_hwio, host_bias, ksize, Cin, Cout, (int)align_up(Cin, 64), (int)align_up(Cout, 64), {}, half_of(precision),
@@ -1537,7 +1493,7 @@ int h3d_pack_conv_weights(h3d_ctx* ctx, const float* host_w_hwio, const float* h
 int h3d_free_packed_conv(h3d_ctx* ctx, h3d_packed_conv* packed) {
     if (!packed) return H3D_OK;
     H3D_REQUIRE(ctx != nullptr, "h3d_free_packed_conv: ctx is NULL");
-    DeviceGuard guard(ctx->device);
+    DeviceGuard guard(ctx);
     free_packed(packed->pw);     // cudaFree waits for kernels that still read the planes
     delete packed;
     return H3D_OK;
@@ -1581,9 +1537,7 @@ static int conv_tc_run(h3d_ctx* ctx, const float* x, float* y, int B, int H, int
     rc = tc_conv_launch(tp, s);
     tc_conv_plan_destroy(tp);
     if (rc) return rc;
-    if ((rc = launch_split_to_f32(ys, y, rows_out, Cout, Cout_pad, half, s))) return rc;
-    ctx->launches += 3;
-    return H3D_OK;
+    return launch_split_to_f32(ys, y, rows_out, Cout, Cout_pad, half, s);
 }
 }  // extern "C++"
 
@@ -1613,7 +1567,6 @@ int h3d_conv2d_tc_dev(h3d_ctx* ctx, const float* x, const float* w_hwio, const f
         pw->bias = (float*)(wbase + 2 * pb);
         if (half_of(precision) == Half16::FP16) pw->w_scale = pw->bias + Cout_pad;
         pw->Cin_pad = Cin_pad; pw->Cout_pad = Cout_pad;
-        ctx->launches += pw->w_scale ? 2 : 1;
         return launch_pack_conv_w(w_hwio, bias, pw->w, pw->bias, pw->w_scale, ksize, Cin, Cout, Cin_pad, Cout_pad, false, half_of(precision), s);
     };
     return conv_tc_run(ctx, x, y, B, H, W, Cin, Cout, ksize, stride, leaky, precision, Cin_pad, Cout_pad, 2 * pb + align_up(Cout_pad * 8, 1024),
@@ -1657,11 +1610,7 @@ int h3d_conv2d_tc_backward(h3d_ctx* ctx, const float* x, const float* y, const f
     gs.hi = (uint16_t*)base;
     if (passes == 3) gs.lo = (uint16_t*)(base + gb);
     if ((rc = launch_conv_grad_prep(dy, leaky ? y : nullptr, gs, db ? db_part : nullptr, B, H, W, Cout, Cout_pad, stride, leaky, s))) return rc;
-    ctx->launches += 1;
-    if (db) {
-        if ((rc = launch_bias_grad_reduce(db_part, nblk, Cout, Cout_pad, db, s))) return rc;
-        ctx->launches += 1;
-    }
+    if (db && (rc = launch_bias_grad_reduce(db_part, nblk, Cout, Cout_pad, db, s))) return rc;
     if (dx) {   // the stride-1 'SAME' convolution of dy' with the flipped, transposed kernel, on the forward kernel
         Split wd;
         wd.hi = (uint16_t*)wbase;
@@ -1677,7 +1626,6 @@ int h3d_conv2d_tc_backward(h3d_ctx* ctx, const float* x, const float* y, const f
         rc = tc_conv_launch(tp, s);
         tc_conv_plan_destroy(tp);
         if (rc) return rc;
-        ctx->launches += 2;
     }
     if (dw_hwio) {
         Split xs;
@@ -1689,7 +1637,6 @@ int h3d_conv2d_tc_backward(h3d_ctx* ctx, const float* x, const float* y, const f
         d.B = B; d.H = H; d.W = W; d.Cin = Cin; d.Cout = Cout; d.Cin_pad = Cin_pad; d.Cout_pad = Cout_pad; d.k = ksize; d.passes = passes;
         d.partial = wpart; d.dw = dw_hwio; d.err_flag = ctx->err_flag;
         if ((rc = launch_conv_wgrad(d, s))) return rc;
-        ctx->launches += 3;
     }
     return H3D_OK;
 }
@@ -1800,9 +1747,7 @@ int h3d_conv2d_layer_planes(h3d_ctx* ctx, const float* x, int B, int H, int W, i
         a.ys = ys; a.Cs_total = Cy_total; a.cs_off = cy_off; a.half = half;
         a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.k = ksize; a.stride = 1; a.leaky = leaky;
         a.err_flag = ctx->err_flag;
-        if ((rc = launch_conv_direct(a, s))) return rc;
-        ctx->launches += conv_direct_num_launches(a);
-        return H3D_OK;
+        return launch_conv_direct(a, s);
     }
     const int Cin_pad = (int)align_up(Cin, 64), Cout_pad = (int)align_up(Cout, 64);
     H3D_REQUIRE(Cin_pad <= Cx && Cx % 16 == 0, "h3d_conv2d_layer_planes: x needs Cx >= align_up(Cin, 64) channels, Cx a multiple of 16");
@@ -1819,7 +1764,6 @@ int h3d_conv2d_layer_planes(h3d_ctx* ctx, const float* x, int B, int H, int W, i
     if (passes == 3) xs.lo = (uint16_t*)(base + xb);
     if (passes == 4) { xs.l8 = (uint8_t*)(base + xb); xs.h8 = xs.l8 + x8; }
     if ((rc = launch_f32_to_split(x, xs, rows, Cx, Cx, half, s))) return rc;
-    ctx->launches += 1;
     PackedW pw;
     if ((rc = pack_conv_weights(host_w_hwio, host_bias, ksize, Cin, Cout, Cin_pad, Cout_pad, perm, half, passes, &pw))) {
         free_packed(pw);
@@ -1834,7 +1778,6 @@ int h3d_conv2d_layer_planes(h3d_ctx* ctx, const float* x, int B, int H, int W, i
     if (tp) {
         rc = tc_conv_launch(tp, s);
         tc_conv_plan_destroy(tp);
-        if (!rc) ctx->launches += 1;
     }
     free_packed(pw);   // host weights: the free waits for the kernel, as in h3d_conv2d_tc
     return rc;
@@ -1842,16 +1785,12 @@ int h3d_conv2d_layer_planes(h3d_ctx* ctx, const float* x, int B, int H, int W, i
 
 int h3d_maxpool2x2_f32(h3d_ctx* ctx, const float* x, float* y, int B, int H, int W, int C, void* stream) {
     H3D_OP_PROLOGUE(ctx);
-    int rc = launch_maxpool_f32(x, y, B, H, W, C, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_maxpool_f32(x, y, B, H, W, C, s);
 }
 int h3d_maxpool2x2_backward_f32(h3d_ctx* ctx, const float* x, const float* dy, float* dx, int B, int H, int W, int C, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(x && dy && dx && B > 0 && H > 0 && W > 0 && C > 0, "h3d_maxpool2x2_backward_f32: bad argument");
-    int rc = launch_maxpool_backward_f32(x, dy, dx, B, H, W, C, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_maxpool_backward_f32(x, dy, dx, B, H, W, C, s);
 }
 int h3d_fully_connected_f32(h3d_ctx* ctx, const float* x, const float* w, const float* bias, float* y, int B, int in_features,
                             int out_features, int leaky, void* stream) {
@@ -1860,28 +1799,20 @@ int h3d_fully_connected_f32(h3d_ctx* ctx, const float* x, const float* w, const 
     const int64_t scratch_floats = fc_scratch_floats(B, in_features, out_features);
     int rc = op_scratch(ctx, scratch_floats * 4, &scratch);
     if (rc) return rc;
-    rc = launch_fc(x, w, bias, y, (float*)scratch, scratch_floats, B, in_features, out_features, leaky, in_features, s);
-    if (!rc) ctx->launches += 2;
-    return rc;
+    return launch_fc(x, w, bias, y, (float*)scratch, scratch_floats, B, in_features, out_features, leaky, in_features, s);
 }
 int h3d_leaky_relu_f32(h3d_ctx* ctx, const float* x, float* y, int64_t n, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(x && y && n > 0, "h3d_leaky_relu_f32: bad argument");
-    int rc = launch_leaky_relu(x, y, n, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_leaky_relu(x, y, n, s);
 }
 int h3d_resize_bilinear_tf1(h3d_ctx* ctx, const float* x, float* y, int B, int H, int W, int C, int out_h, int out_w, void* stream) {
     H3D_OP_PROLOGUE(ctx);
-    int rc = launch_resize_bilinear_tf1(x, y, B, H, W, C, out_h, out_w, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_resize_bilinear_tf1(x, y, B, H, W, C, out_h, out_w, s);
 }
 int h3d_avgpool8(h3d_ctx* ctx, const float* x, float* y, int B, int H, int W, int C, void* stream) {
     H3D_OP_PROLOGUE(ctx);
-    int rc = launch_avgpool8(x, y, B, H, W, C, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_avgpool8(x, y, B, H, W, C, s);
 }
 int h3d_seg_postprocess(h3d_ctx* ctx, const float* logits, int B, int H, int W, uint8_t* hand_mask, int32_t* max_loc, float* center,
                         float* crop_size, float* scale_crop, void* stream) {
@@ -1893,34 +1824,24 @@ int h3d_seg_postprocess(h3d_ctx* ctx, const float* logits, int B, int H, int W, 
     char* scratch = nullptr;
     int rc = op_scratch(ctx, seg_scratch_bytes(B, H, W), &scratch);
     if (rc) return rc;
-    int nl = 0;
-    rc = launch_seg_postprocess(logits, B, H, W, scratch, hand_mask, max_loc, center, crop_size, scale_crop, s, &nl);
-    ctx->launches += nl;
-    return rc;
+    return launch_seg_postprocess(logits, B, H, W, scratch, hand_mask, max_loc, center, crop_size, scale_crop, s);
 }
 int h3d_calc_center_bb(h3d_ctx* ctx, const float* mask, int B, int H, int W, float* center, float* bb, float* crop_size, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(mask && center && B > 0 && H > 0 && W > 0, "h3d_calc_center_bb: bad argument");
-    int rc = launch_mask_bbox(mask, B, H, W, center, bb, crop_size, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_mask_bbox(mask, B, H, W, center, bb, crop_size, s);
 }
 int h3d_crop_image_from_xy(h3d_ctx* ctx, const float* image, const float* center, const float* scale, float* image_crop, int B,
                            int H, int W, int C, int crop_size, void* stream) {
     H3D_OP_PROLOGUE(ctx);
-    int rc = launch_crop_image(image, center, scale, image_crop, B, H, W, C, crop_size, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_crop_image(image, center, scale, image_crop, B, H, W, C, crop_size, s);
 }
 int h3d_detect_keypoints(h3d_ctx* ctx, const float* scoremaps, int B, int H, int W, int C, int32_t* keypoints_uv, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     char* scratch = nullptr;
     int rc = op_scratch(ctx, argmax_scratch_bytes(B, C), &scratch);
     if (rc) return rc;
-    int nl = 0;
-    rc = launch_detect_keypoints(scoremaps, B, H, W, C, scratch, keypoints_uv, s, &nl);
-    ctx->launches += nl;
-    return rc;
+    return launch_detect_keypoints(scoremaps, B, H, W, C, scratch, keypoints_uv, s);
 }
 int h3d_upsample_detect_keypoints(h3d_ctx* ctx, const float* scoremaps, int B, int H, int W, int out_h, int out_w, float* scoremaps_up,
                                   int32_t* keypoints_uv, void* stream) {
@@ -1929,18 +1850,13 @@ int h3d_upsample_detect_keypoints(h3d_ctx* ctx, const float* scoremaps, int B, i
     char* scratch = nullptr;
     int rc = op_scratch(ctx, argmax_scratch_bytes(B, 21), &scratch);
     if (rc) return rc;
-    int nl = 0;
-    rc = launch_resize_argmax21(scoremaps, scoremaps_up, B, H, W, out_h, out_w, scratch, keypoints_uv, s, &nl);
-    ctx->launches += nl;
-    return rc;
+    return launch_resize_argmax21(scoremaps, scoremaps_up, B, H, W, out_h, out_w, scratch, keypoints_uv, s);
 }
 int h3d_pack_records(h3d_ctx* ctx, const float* coord3d, const int32_t* keypoints_uv, const float* center, const float* scale_crop, int B,
                      float* records, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(coord3d && keypoints_uv && center && scale_crop && records && B > 0, "h3d_pack_records: bad argument");
-    int rc = launch_pack_records(coord3d, keypoints_uv, center, scale_crop, B, records, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_pack_records(coord3d, keypoints_uv, center, scale_crop, B, records, s);
 }
 int h3d_gather_records_p2p(h3d_ctx* ctx, const float* coord3d, const int32_t* keypoints_uv, const float* center, const float* scale_crop,
                            int B, int max_batch, const uint64_t* peer_buffers, const uint64_t* peer_signals, uint64_t multicast_ptr, int rank,
@@ -1948,10 +1864,8 @@ int h3d_gather_records_p2p(h3d_ctx* ctx, const float* coord3d, const int32_t* ke
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(coord3d && keypoints_uv && center && scale_crop && peer_buffers && peer_signals, "h3d_gather_records_p2p: NULL argument");
     H3D_REQUIRE(max_batch >= B && parity_stride_floats >= (int64_t)world * max_batch * 108, "h3d_gather_records_p2p: parity stride too small");
-    int rc = launch_gather_records_p2p(coord3d, keypoints_uv, center, scale_crop, B, peer_buffers, peer_signals, multicast_ptr, rank,
-                                       world, epoch, parity_stride_floats, max_batch, ctx->err_flag, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_gather_records_p2p(coord3d, keypoints_uv, center, scale_crop, B, peer_buffers, peer_signals, multicast_ptr, rank,
+                                     world, epoch, parity_stride_floats, max_batch, ctx->err_flag, s);
 }
 // The record layouts of both datasets; index != NULL gathers record index[b] mod n_records of a resident file.
 static int decode_dataset_records(int dataset, const uint8_t* records, const int64_t* index, int64_t n_records, int B, int step,
@@ -1972,25 +1886,19 @@ int h3d_decode_records(h3d_ctx* ctx, int dataset, const uint8_t* records, int B,
                        uint8_t* visibility, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(records && image && B > 0 && (step == 1 || step == 2 || step == 4), "h3d_decode_records: bad argument");
-    int rc = decode_dataset_records(dataset, records, nullptr, 0, B, step, header, image, mask, visibility, s, "h3d_decode_records");
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return decode_dataset_records(dataset, records, nullptr, 0, B, step, header, image, mask, visibility, s, "h3d_decode_records");
 }
 int h3d_decode_records_gather(h3d_ctx* ctx, int dataset, const uint8_t* file, int64_t n_records, const int64_t* serials, int B, int step,
                               float* header, float* image, uint8_t* mask, uint8_t* visibility, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(file && serials && image && n_records > 0 && B > 0 && B <= H3D_READER_MAX_GATHER && (step == 1 || step == 2 || step == 4),
                 "h3d_decode_records_gather: bad argument");
-    int rc = decode_dataset_records(dataset, file, serials, n_records, B, step, header, image, mask, visibility, s, "h3d_decode_records_gather");
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return decode_dataset_records(dataset, file, serials, n_records, B, step, header, image, mask, visibility, s, "h3d_decode_records_gather");
 }
 int h3d_reader_next_serials(h3d_ctx* ctx, int64_t* state, int B, uint64_t seed, int shuffle, int64_t* serials, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(state && serials && B > 0, "h3d_reader_next_serials: bad argument");
-    int rc = launch_reader_next_serials(state, B, seed, shuffle ? 1 : 0, serials, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_reader_next_serials(state, B, seed, shuffle ? 1 : 0, serials, s);
 }
 namespace {
 
@@ -2027,9 +1935,7 @@ int resize_frames(h3d_ctx* ctx, const char* fn, const uint8_t* frames, int forma
         if (!p) return H3D_ECUDA;
         it = ctx->frame_plans.emplace(key, p).first;
     }
-    rc = launch_resize_frames(it->second, frames, B, normalize, out, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_resize_frames(it->second, frames, B, normalize, out, s);
 }
 
 }  // namespace
@@ -2048,9 +1954,7 @@ int h3d_convert_frames(h3d_ctx* ctx, const uint8_t* frames, int format, int B, i
     H3D_REQUIRE(frames && out_rgb && B > 0, "h3d_convert_frames: bad argument");
     int rc = check_frame_format("h3d_convert_frames", format, H, W);
     if (rc) return rc;
-    rc = launch_convert_frames(frames, format, B, H, W, out_rgb, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_convert_frames(frames, format, B, H, W, out_rgb, s);
 }
 int h3d_draw_segments(h3d_ctx* ctx, uint8_t* images, int B, int H, int W, const float* segments, int S, const float* host_colors,
                       const int32_t* valid, float linewidth, void* stream) {
@@ -2064,13 +1968,11 @@ int h3d_draw_segments(h3d_ctx* ctx, uint8_t* images, int B, int H, int W, const 
     for (int i = 0; i < 3 * S; ++i)
         H3D_REQUIRE(std::isfinite(host_colors[i]) && host_colors[i] >= 0.f && host_colors[i] <= 255.f,
                     "h3d_draw_segments: colour %d of segment %d must be finite in 0..255, got %g", i % 3, i / 3, (double)host_colors[i]);
-    int rc = launch_draw_segments(images, B, H, W, segments, S, host_colors, valid, linewidth, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_draw_segments(images, B, H, W, segments, S, host_colors, valid, linewidth, s);
 }
 int h3d_set_dropout(h3d_ctx* ctx, int enabled, uint64_t seed) {
     H3D_REQUIRE(ctx != nullptr, "h3d_set_dropout: ctx is NULL");
-    DeviceGuard guard_(ctx->device);
+    DeviceGuard guard_(ctx);
     if (enabled && (!ctx->drop_seeded || seed != ctx->drop_seed)) {
         H3D_CUDA(cudaMemset(ctx->drop_draw, 0, sizeof(int64_t)));
         ctx->drop_seed = seed; ctx->drop_seeded = true;
@@ -2095,10 +1997,8 @@ int h3d_dropout_forward_planes(h3d_ctx* ctx, const float* x, int rows, int cols,
     H3D_REQUIRE(!hi || ((half == 0 || half == 1) && stride >= cols), "h3d_dropout_forward_planes: half must be 0 or 1 and stride >= cols");
     H3D_REQUIRE(hi || !lo, "h3d_dropout_forward_planes: lo without hi");
     Split sp; sp.hi = hi; sp.lo = lo;
-    int rc = launch_dropout(x, rows, cols, keep_prob, layer, ctx->drop_seed, ctx->drop_draw, y, keep, sp, stride,
-                            half == 1 ? Half16::FP16 : Half16::BF16, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_dropout(x, rows, cols, keep_prob, layer, ctx->drop_seed, ctx->drop_draw, y, keep, sp, stride,
+                          half == 1 ? Half16::FP16 : Half16::BF16, s);
 }
 int h3d_dropout_forward(h3d_ctx* ctx, const float* x, int rows, int cols, float keep_prob, int layer, float* y, uint8_t* keep, void* stream) {
     return h3d_dropout_forward_planes(ctx, x, rows, cols, keep_prob, layer, y, keep, 0, cols, nullptr, nullptr, stream);
@@ -2107,49 +2007,37 @@ int h3d_dropout_backward(h3d_ctx* ctx, const float* dy, const uint8_t* keep, int
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(dy && keep && dx, "h3d_dropout_backward: bad argument");
     H3D_DROPOUT_CHECKS("h3d_dropout_backward");
-    int rc = launch_dropout_backward(dy, keep, (int64_t)rows * cols, keep_prob, dx, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_dropout_backward(dy, keep, (int64_t)rows * cols, keep_prob, dx, s);
 }
 int h3d_dropout_advance(h3d_ctx* ctx, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(ctx->drop_on, "h3d_dropout_advance: dropout is not enabled on this context (h3d_set_dropout)");
-    int rc = launch_dropout_advance(ctx->drop_draw, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_dropout_advance(ctx->drop_draw, s);
 }
 int h3d_rhd_reader_items(h3d_ctx* ctx, const float* header, const uint8_t* hand_parts, const uint8_t* visibility, int B, int use_wrist_coord,
                          int hand_crop, int crop_size, float* keypoint_xyz21, float* keypoint_uv21, uint8_t* keypoint_vis21, float* hand_side,
                          float* keypoint_scale, float* keypoint_xyz21_normed, float* crop_center, float* crop_scale, float* cam_mat, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(header && hand_parts && visibility && hand_side && B > 0 && crop_size > 1, "h3d_rhd_reader_items: bad argument");
-    int rc = launch_rhd_items(header, hand_parts, visibility, B, use_wrist_coord, hand_crop, crop_size, keypoint_xyz21, keypoint_uv21, keypoint_vis21,
-                              hand_side, keypoint_scale, keypoint_xyz21_normed, crop_center, crop_scale, cam_mat, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_rhd_items(header, hand_parts, visibility, B, use_wrist_coord, hand_crop, crop_size, keypoint_xyz21, keypoint_uv21, keypoint_vis21,
+                            hand_side, keypoint_scale, keypoint_xyz21_normed, crop_center, crop_scale, cam_mat, s);
 }
 int h3d_stb_reader_items(h3d_ctx* ctx, const float* header, int B, int use_wrist_coord, float* keypoint_xyz21, float* keypoint_uv21,
                          uint8_t* keypoint_vis21, float* keypoint_scale, float* keypoint_xyz21_normed, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(header && B > 0, "h3d_stb_reader_items: bad argument");
-    int rc = launch_stb_items(header, B, use_wrist_coord, keypoint_xyz21, keypoint_uv21, keypoint_vis21, keypoint_scale, keypoint_xyz21_normed, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_stb_items(header, B, use_wrist_coord, keypoint_xyz21, keypoint_uv21, keypoint_vis21, keypoint_scale, keypoint_xyz21_normed, s);
 }
 int h3d_gaussian_scoremap(h3d_ctx* ctx, const float* coords_hw, const uint8_t* valid, int B, int N, int H, int W, float sigma, float* scoremap,
                           void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(coords_hw && scoremap && B > 0 && H > 0 && W > 0 && sigma > 0.f, "h3d_gaussian_scoremap: bad argument");
-    int rc = launch_gaussian_map(coords_hw, valid, B, N, H, W, sigma, scoremap, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_gaussian_map(coords_hw, valid, B, N, H, W, sigma, scoremap, s);
 }
 int h3d_reader_aug_params(h3d_ctx* ctx, const int64_t* serials, int B, uint64_t seed, int flags, float* params, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(serials && params && B > 0 && (flags & ~127) == 0, "h3d_reader_aug_params: bad argument");
-    int rc = launch_reader_aug_params(serials, B, seed, flags, params, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_reader_aug_params(serials, B, seed, flags, params, s);
 }
 int h3d_augment_image(h3d_ctx* ctx, const float* image, const uint8_t* hand_parts, const float* params, int B, int H, int W, int flags,
                       int window, float* out_image, int32_t* out_parts, int32_t* out_mask, void* stream) {
@@ -2157,9 +2045,7 @@ int h3d_augment_image(h3d_ctx* ctx, const float* image, const uint8_t* hand_part
     H3D_REQUIRE(image && out_image && B > 0 && H > 0 && W > 0 && (flags & ~(H3D_AUG_HUE | H3D_AUG_RANDOM_CROP)) == 0, "h3d_augment_image: bad argument");
     H3D_REQUIRE(params || !flags, "h3d_augment_image: flags need params");
     H3D_REQUIRE(hand_parts || (!out_parts && !out_mask), "h3d_augment_image: part / mask windows need hand_parts");
-    int rc = launch_augment_image(image, hand_parts, params, B, H, W, flags, window, out_image, out_parts, out_mask, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_augment_image(image, hand_parts, params, B, H, W, flags, window, out_image, out_parts, out_mask, s);
 }
 int h3d_rhd_reader_items_aug(h3d_ctx* ctx, const float* header, const uint8_t* hand_parts, const uint8_t* visibility, int B, int use_wrist_coord,
                              int hand_crop, int crop_size, const float* params, int flags, float* keypoint_uv, float* keypoint_xyz21,
@@ -2169,33 +2055,25 @@ int h3d_rhd_reader_items_aug(h3d_ctx* ctx, const float* header, const uint8_t* h
     H3D_REQUIRE(header && hand_parts && visibility && hand_side && B > 0 && crop_size > 1, "h3d_rhd_reader_items_aug: bad argument");
     const int noise = H3D_AUG_COORD_UV_NOISE | H3D_AUG_CROP_CENTER_NOISE | H3D_AUG_CROP_SCALE_NOISE | H3D_AUG_CROP_OFFSET_NOISE;
     H3D_REQUIRE((flags & ~noise) == 0, "h3d_rhd_reader_items_aug: flags other than the coordinate / crop noises");
-    int rc = launch_rhd_items(header, hand_parts, visibility, B, use_wrist_coord, hand_crop, crop_size, keypoint_xyz21, keypoint_uv21, keypoint_vis21,
-                              hand_side, keypoint_scale, keypoint_xyz21_normed, crop_center, crop_scale, cam_mat, s, params, flags, keypoint_uv);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_rhd_items(header, hand_parts, visibility, B, use_wrist_coord, hand_crop, crop_size, keypoint_xyz21, keypoint_uv21, keypoint_vis21,
+                            hand_side, keypoint_scale, keypoint_xyz21_normed, crop_center, crop_scale, cam_mat, s, params, flags, keypoint_uv);
 }
 int h3d_gaussian_scoremap_dropout(h3d_ctx* ctx, const float* coords_hw, const uint8_t* valid, const float* keep, int keep_stride, float keep_prob,
                                   int B, int N, int H, int W, float sigma, float* scoremap, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(coords_hw && keep && scoremap && B > 0 && H > 0 && W > 0 && sigma > 0.f, "h3d_gaussian_scoremap_dropout: bad argument");
-    int rc = launch_gaussian_map(coords_hw, valid, B, N, H, W, sigma, scoremap, s, keep, keep_stride, keep_prob);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_gaussian_map(coords_hw, valid, B, N, H, W, sigma, scoremap, s, keep, keep_stride, keep_prob);
 }
 int h3d_canonical_trafo(h3d_ctx* ctx, const float* coords_xyz, const uint8_t* cond_right, int B, float* coords_can, float* rot_mat,
                         float* rot_mat_inv, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(coords_xyz && B > 0, "h3d_canonical_trafo: bad argument");
-    int rc = launch_canonical_trafo(coords_xyz, cond_right, B, coords_can, rot_mat, rot_mat_inv, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_canonical_trafo(coords_xyz, cond_right, B, coords_can, rot_mat, rot_mat_inv, s);
 }
 int h3d_eval_keypoint_dist(h3d_ctx* ctx, const float* gt, const uint8_t* vis, const float* pred, int n, int D, float* dist, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(gt && vis && pred && dist && n > 0 && D >= 1 && D <= 4, "h3d_eval_keypoint_dist: bad argument");
-    int rc = launch_eval_dist(gt, vis, pred, n, D, dist, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_eval_dist(gt, vis, pred, n, D, dist, s);
 }
 static int eval_store_check(const char* what, int K, int num_samples, int dtype) {
     H3D_REQUIRE(K >= 1 && K <= H3D_EVAL_MAX_KP, "%s: K = %d key-points, the store holds 1..%d", what, K, H3D_EVAL_MAX_KP);
@@ -2215,9 +2093,7 @@ int h3d_eval_feed(h3d_ctx* ctx, void* store, int K, int num_samples, int dtype, 
     H3D_REQUIRE(D >= 1 && D <= H3D_EVAL_MAX_DIM, "h3d_eval_feed: D = %d coordinates, 1..%d are supported", D, H3D_EVAL_MAX_DIM);
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(store && gt && vis && pred && n > 0, "h3d_eval_feed: bad argument");
-    int rc = launch_eval_feed(store, K, num_samples, dtype, gt, vis, pred, n, D, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_eval_feed(store, K, num_samples, dtype, gt, vis, pred, n, D, s);
 }
 int h3d_eval_stats(h3d_ctx* ctx, const void* store, int K, int num_samples, int dtype, const double* thresholds, int T, int64_t* out,
                    void* stream) {
@@ -2226,30 +2102,22 @@ int h3d_eval_stats(h3d_ctx* ctx, const void* store, int K, int num_samples, int 
                 H3D_EVAL_MAX_THRESHOLDS);
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(store && thresholds && out, "h3d_eval_stats: bad argument");
-    int rc = launch_eval_stats(store, K, num_samples, dtype, thresholds, T, out, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_eval_stats(store, K, num_samples, dtype, thresholds, T, out, s);
 }
 int h3d_bone_rel_trafo_inv(h3d_ctx* ctx, const float* coords_rel, float* coords_xyz, int B, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(coords_rel && coords_xyz && B > 0, "h3d_bone_rel_trafo_inv: bad argument");
-    int rc = launch_bone_rel_trafo_inv(coords_rel, coords_xyz, B, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_bone_rel_trafo_inv(coords_rel, coords_xyz, B, s);
 }
 int h3d_rotate_canonical(h3d_ctx* ctx, const float* coord_can, const float* uxyz, const float* hand_side, int B, float* rot_mat,
                          float* coord_out, void* stream) {
     H3D_OP_PROLOGUE(ctx);
-    int rc = launch_rotate_canonical(coord_can, uxyz, hand_side, B, rot_mat, coord_out, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_rotate_canonical(coord_can, uxyz, hand_side, B, rot_mat, coord_out, s);
 }
 int h3d_flip_right_hand(h3d_ctx* ctx, const float* coords_xyz, const uint8_t* cond_right, int B, float* out, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(coords_xyz && cond_right && out && B > 0, "h3d_flip_right_hand: bad argument");
-    int rc = launch_flip_right_hand(coords_xyz, cond_right, B, out, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_flip_right_hand(coords_xyz, cond_right, B, out, s);
 }
 
 // ---------------------------------------------------------------------------------------------- training (train.cu)
@@ -2262,10 +2130,7 @@ int h3d_resize_bilinear_tf1_backward(h3d_ctx* ctx, const float* dy, float* dx, i
     char* scratch = nullptr;
     int rc = op_scratch(ctx, std::max<int64_t>(4, resize_grad_scratch_floats(B, H, W, C, out_h, out_w) * 4), &scratch);
     if (rc) return rc;
-    int nl = 0;
-    rc = launch_resize_bilinear_tf1_grad(dy, dx, (float*)scratch, B, H, W, C, out_h, out_w, s, &nl);
-    ctx->launches += nl;
-    return rc;
+    return launch_resize_bilinear_tf1_grad(dy, dx, (float*)scratch, B, H, W, C, out_h, out_w, s);
 }
 int h3d_scoremap_loss_forward(h3d_ctx* ctx, const float* pred, const float* target, const float* vis, int B, int H, int W, float* loss,
                               float* rms, void* stream) {
@@ -2275,18 +2140,14 @@ int h3d_scoremap_loss_forward(h3d_ctx* ctx, const float* pred, const float* targ
     char* scratch = nullptr;
     int rc = op_scratch(ctx, scoremap_loss_scratch_floats(B, H, W) * 4, &scratch);
     if (rc) return rc;
-    rc = launch_scoremap_loss(pred, target, vis, (float*)scratch, B, H, W, loss, rms, s);
-    if (!rc) ctx->launches += 2;
-    return rc;
+    return launch_scoremap_loss(pred, target, vis, (float*)scratch, B, H, W, loss, rms, s);
 }
 int h3d_scoremap_loss_backward(h3d_ctx* ctx, const float* pred, const float* target, const float* vis, const float* rms,
                                const float* grad_loss, int B, int H, int W, float* dpred, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(pred && target && vis && rms && dpred, "h3d_scoremap_loss_backward: pred, target, vis, rms and dpred are required");
     H3D_REQUIRE(B > 0 && H > 0 && W > 0 && (int64_t)H * W <= (1 << 30), "h3d_scoremap_loss_backward: bad shape B=%d H=%d W=%d", B, H, W);
-    int rc = launch_scoremap_loss_grad(pred, target, vis, rms, grad_loss, dpred, B, H, W, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_scoremap_loss_grad(pred, target, vis, rms, grad_loss, dpred, B, H, W, s);
 }
 int h3d_softmax_xent_forward(h3d_ctx* ctx, const float* logits, const float* labels, int64_t rows, float* loss, void* stream) {
     H3D_OP_PROLOGUE(ctx);
@@ -2296,9 +2157,7 @@ int h3d_softmax_xent_forward(h3d_ctx* ctx, const float* logits, const float* lab
     char* scratch = nullptr;
     int rc = op_scratch(ctx, softmax_xent_scratch_floats(rows) * 4, &scratch);
     if (rc) return rc;
-    rc = launch_softmax_xent(logits, labels, (float*)scratch, rows, loss, s);
-    if (!rc) ctx->launches += 2;
-    return rc;
+    return launch_softmax_xent(logits, labels, (float*)scratch, rows, loss, s);
 }
 int h3d_softmax_xent_backward(h3d_ctx* ctx, const float* logits, const float* labels, const float* grad_loss, int64_t rows, float* dlogits,
                               void* stream) {
@@ -2307,23 +2166,17 @@ int h3d_softmax_xent_backward(h3d_ctx* ctx, const float* logits, const float* la
     H3D_REQUIRE(rows > 0, "h3d_softmax_xent_backward: rows must be positive, got %lld", (long long)rows);
     H3D_REQUIRE(((uintptr_t)logits | (uintptr_t)labels | (uintptr_t)dlogits) % 8 == 0,
                 "h3d_softmax_xent_backward: logits, labels and dlogits must be 8-byte aligned");
-    int rc = launch_softmax_xent_grad(logits, labels, grad_loss, dlogits, rows, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_softmax_xent_grad(logits, labels, grad_loss, dlogits, rows, s);
 }
 int h3d_adam_state_set(h3d_ctx* ctx, float* state, float lr, float beta1_power, float beta2_power, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(state && ((uintptr_t)state % 16) == 0, "h3d_adam_state_set: state must be a 16-byte aligned device pointer");
-    int rc = launch_adam_state_set(state, 7, lr, beta1_power, beta2_power, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_adam_state_set(state, 7, lr, beta1_power, beta2_power, s);
 }
 int h3d_adam_set_lr(h3d_ctx* ctx, float* state, float lr, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(state && ((uintptr_t)state % 16) == 0, "h3d_adam_set_lr: state must be a 16-byte aligned device pointer");
-    int rc = launch_adam_state_set(state, 1, lr, 0.f, 0.f, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_adam_state_set(state, 1, lr, 0.f, 0.f, s);
 }
 int h3d_adam_step(h3d_ctx* ctx, const h3d_adam_tensor* table, int num_tensors, float* state, float beta1, float beta2, float epsilon,
                   void* stream) {
@@ -2331,9 +2184,7 @@ int h3d_adam_step(h3d_ctx* ctx, const h3d_adam_tensor* table, int num_tensors, f
     H3D_REQUIRE(table && state && ((uintptr_t)state % 16) == 0, "h3d_adam_step: table and a 16-byte aligned state are required");
     H3D_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && epsilon >= 0.f,
                 "h3d_adam_step: need 0 <= beta1, beta2 < 1 and epsilon >= 0");
-    int rc = launch_adam_step(table, num_tensors, state, beta1, beta2, epsilon, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_adam_step(table, num_tensors, state, beta1, beta2, epsilon, s);
 }
 
 // ---------------------------------------------------------------------------------------------- lifting training (train_lift.cu)
@@ -2343,25 +2194,19 @@ int h3d_rotate_canonical_backward(h3d_ctx* ctx, const float* coord_can, const fl
     H3D_REQUIRE(coord_can && uxyz && hand_side && d_can && d_uxyz,
                 "h3d_rotate_canonical_backward: coord_can, uxyz, hand_side, d_can and d_uxyz are required");
     H3D_REQUIRE(B > 0, "h3d_rotate_canonical_backward: bad shape B=%d", B);
-    int rc = launch_rotate_canonical_backward(coord_can, uxyz, hand_side, d_out, d_rot_mat, B, d_can, d_uxyz, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_rotate_canonical_backward(coord_can, uxyz, hand_side, d_out, d_rot_mat, B, d_can, d_uxyz, s);
 }
 int h3d_bone_rel_trafo_inv_backward(h3d_ctx* ctx, const float* coords_rel, const float* d_xyz, float* d_rel, int B, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(coords_rel && d_xyz && d_rel, "h3d_bone_rel_trafo_inv_backward: coords_rel, d_xyz and d_rel are required");
     H3D_REQUIRE(B > 0, "h3d_bone_rel_trafo_inv_backward: bad shape B=%d", B);
-    int rc = launch_bone_rel_trafo_inv_backward(coords_rel, d_xyz, d_rel, B, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_bone_rel_trafo_inv_backward(coords_rel, d_xyz, d_rel, B, s);
 }
 int h3d_bone_rel_trafo(h3d_ctx* ctx, const float* coords_xyz, float* coords_rel, int B, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(coords_xyz && coords_rel, "h3d_bone_rel_trafo: coords_xyz and coords_rel are required");
     H3D_REQUIRE(B > 0, "h3d_bone_rel_trafo: bad shape B=%d", B);
-    int rc = launch_bone_rel_trafo(coords_xyz, coords_rel, B, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_bone_rel_trafo(coords_xyz, coords_rel, B, s);
 }
 int h3d_mse_loss_forward(h3d_ctx* ctx, const float* pred, const float* target, int64_t n, float* loss, void* stream) {
     H3D_OP_PROLOGUE(ctx);
@@ -2370,18 +2215,14 @@ int h3d_mse_loss_forward(h3d_ctx* ctx, const float* pred, const float* target, i
     char* scratch = nullptr;
     int rc = op_scratch(ctx, mse_scratch_floats(n) * 4, &scratch);
     if (rc) return rc;
-    rc = launch_mse(pred, target, (float*)scratch, n, loss, s);
-    if (!rc) ctx->launches += 2;
-    return rc;
+    return launch_mse(pred, target, (float*)scratch, n, loss, s);
 }
 int h3d_mse_loss_backward(h3d_ctx* ctx, const float* pred, const float* target, const float* grad_loss, int64_t n, float* dpred,
                           void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(pred && target && dpred, "h3d_mse_loss_backward: pred, target and dpred are required");
     H3D_REQUIRE(n > 0, "h3d_mse_loss_backward: n must be positive, got %lld", (long long)n);
-    int rc = launch_mse_grad(pred, target, grad_loss, dpred, n, s);
-    if (!rc) ctx->launches += 1;
-    return rc;
+    return launch_mse_grad(pred, target, grad_loss, dpred, n, s);
 }
 
 }  // extern "C"

@@ -23,7 +23,16 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
         if (_e != cudaSuccess) return h3d::cuda_fail(_e, #expr, __FILE__, __LINE__); \
     } while (0)
 
-#define H3D_CHECK_LAUNCH() H3D_CUDA(cudaGetLastError())
+// Kernels this thread has enqueued: every launch is followed by H3D_CHECK_LAUNCH() (or goes through conv_wgmma.cu's launch_pdl),
+// which bumps it once the launch succeeded.  The outermost DeviceGuard of a C entry (api.cu) adds what the entry enqueued to its
+// context's h3d_launch_count.
+extern thread_local int64_t t_launches;
+
+#define H3D_CHECK_LAUNCH()                 \
+    do {                                   \
+        H3D_CUDA(cudaGetLastError());      \
+        ++h3d::t_launches;                 \
+    } while (0)
 
 #define H3D_REQUIRE(cond, ...)                 \
     do {                                       \
@@ -103,11 +112,6 @@ __device__ __forceinline__ T keypoint_dist(const T* __restrict__ gt, const T* __
     return rn_sqrt(acc);
 }
 
-// ---------------------------------------------------------------- launch counter
-struct LaunchCounter {
-    int64_t n = 0;
-};
-
 // ---------------------------------------------------------------- kernels (elementwise.cu)
 // count (optional, device int): only images [0, *count) are resized (needs a size change)
 int launch_resize_bilinear_tf1(const float* x, float* y, int B, int H, int W, int C, int oh, int ow, cudaStream_t s,
@@ -125,15 +129,13 @@ int launch_split_to_f32(Split x, float* y, int64_t rows, int C, int Cpad, Half16
 int64_t seg_scratch_bytes(int B, int H, int W);
 int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scratch, uint8_t* hand_mask,
                            int32_t* max_loc, float* center, float* crop_size, float* scale_crop, cudaStream_t s,
-                           int* n_launch, const float* low = nullptr, int LH = 0, int LW = 0, const int* count = nullptr);
+                           const float* low = nullptr, int LH = 0, int LW = 0, const int* count = nullptr);
 int launch_crop_image(const float* image, const float* center, const float* scale, float* out, int B, int H, int W,
                       int C, int crop, cudaStream_t s);
 int64_t argmax_scratch_bytes(int B, int C);
-int launch_detect_keypoints(const float* sm, int B, int H, int W, int C, void* scratch, int32_t* uv, cudaStream_t s,
-                            int* n_launch);
+int launch_detect_keypoints(const float* sm, int B, int H, int W, int C, void* scratch, int32_t* uv, cudaStream_t s);
 // fused x8 up-sampling of a [B,H,W,21] score map + per-channel arg-max (scratch: argmax_scratch_bytes(B, 21))
-int launch_resize_argmax21(const float* x, float* y, int B, int H, int W, int oh, int ow, void* scratch, int32_t* uv, cudaStream_t s,
-                           int* n_launch);
+int launch_resize_argmax21(const float* x, float* y, int B, int H, int W, int oh, int ow, void* scratch, int32_t* uv, cudaStream_t s);
 // dst[r, dst_off + c] = src[r, c] for c < C (fp32 channel copy into a wider NHWC tensor)
 int launch_copy_channels(const float* src, float* dst, int64_t rows, int C, int dst_total, int dst_off, cudaStream_t s);
 // index != NULL: sample b is record index[b] mod n_records of `rec` (a resident file), B <= kMaxGatherRecords
@@ -222,7 +224,6 @@ struct DirectConvArgs {
 };
 constexpr int64_t kConvSplitKScratchFloats = H3D_CONV_SPLITK_SCRATCH_FLOATS;   // upper bound used by launch_conv_direct's split-K policy
 int launch_conv_direct(const DirectConvArgs& a, cudaStream_t s);
-int conv_direct_num_launches(const DirectConvArgs& a);   // 1, or 2 when the split-K policy applies
 // out[6] of h3d_conv2d_f32_geometry for a (host only: the pointers of a are only tested for NULL and x for its alignment)
 void conv_direct_geometry(const DirectConvArgs& a, int* out);
 // scratch: fc_scratch_floats(B, in_f, out_f) floats (split-K partial sums); two kernels per call.  scratch_floats is the capacity
@@ -330,10 +331,9 @@ void conv_wgrad_geometry(int B, int H, int W, int k, int Cin_pad, int Cout_pad, 
 int launch_conv_wgrad(const WgradDesc& d, cudaStream_t s);
 
 // ---------------------------------------------------------------- kernels (train.cu): resize gradient, training losses, Adam
-// scratch: resize_grad_scratch_floats(...) floats (the column pass's [B,oh,W,C] when both dimensions change); *n_launch kernels
+// scratch: resize_grad_scratch_floats(...) floats (the column pass's [B,oh,W,C] when both dimensions change)
 int64_t resize_grad_scratch_floats(int B, int H, int W, int C, int oh, int ow);
-int launch_resize_bilinear_tf1_grad(const float* dy, float* dx, float* scratch, int B, int H, int W, int C, int oh, int ow, cudaStream_t s,
-                                    int* n_launch);
+int launch_resize_bilinear_tf1_grad(const float* dy, float* dx, float* scratch, int B, int H, int W, int C, int oh, int ow, cudaStream_t s);
 int64_t scoremap_loss_scratch_floats(int B, int H, int W);   // two kernels
 int launch_scoremap_loss(const float* P, const float* T, const float* vis, float* scratch, int B, int H, int W, float* loss, float* rms,
                          cudaStream_t s);

@@ -314,7 +314,7 @@ static bool is_c3_case(const DirectConvArgs& a) {
            (!a.y || ((a.Cout_total % 4) == 0 && (a.cout_off % 4) == 0)) && (!a.ys.hi || ((a.Cs_total % 8) == 0 && (a.cs_off % 8) == 0));
 }
 
-// Launch geometry + split-K policy shared by the launcher and by conv_direct_num_launches().
+// Launch geometry + split-K policy shared by the launcher and by conv_direct_geometry().
 static void plan_direct(const DirectConvArgs& a, ConvGeom* gp, dim3* gridp, int* ksplitp) {
     ConvGeom& g = *gp;
     g.B = a.B; g.H = a.H; g.W = a.W; g.Cin = a.Cin; g.Cout = a.Cout; g.k = a.k; g.stride = a.stride;
@@ -355,13 +355,6 @@ static int direct_kernel(const DirectConvArgs& a) {
 }
 
 static int c3_ctas(const DirectConvArgs& a) { return ceil_div(ceil_div(a.W, C3_TW) * ceil_div(a.H, C3_TH) * a.B, C3_TILES_PER_CTA); }
-
-int conv_direct_num_launches(const DirectConvArgs& a) {
-    if (is_c3_case(a)) return 1;
-    ConvGeom g; dim3 grid; int ksplit;
-    plan_direct(a, &g, &grid, &ksplit);
-    return ksplit > 1 ? 2 : 1;
-}
 
 void conv_direct_geometry(const DirectConvArgs& a, int* out) {
     const int kernel = direct_kernel(a);

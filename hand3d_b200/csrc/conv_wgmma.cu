@@ -787,7 +787,9 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = tc_tuning().pdl ? 1 : 0;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+    if (e == cudaSuccess) ++t_launches;   // as H3D_CHECK_LAUNCH
+    return e;
 }
 
 // Tuning switches (A/B experiments, forced variants in the tests).  Read from the environment ONCE, when the library is first

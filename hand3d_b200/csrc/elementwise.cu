@@ -817,15 +817,16 @@ static int launch_mask_grow_cluster(const unsigned long long* key, const uint32_
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    H3D_CUDA(cudaLaunchKernelEx(&cfg, mask_grow_cluster_kernel, key, det, H, W, Ww, num_passes, hand_mask, max_loc, center, crop_size,
-                                scale_crop, count));
+    cudaLaunchKernelEx(&cfg, mask_grow_cluster_kernel, key, det, H, W, Ww, num_passes, hand_mask, max_loc, center, crop_size, scale_crop,
+                       count);
+    H3D_CHECK_LAUNCH();
     return H3D_OK;
 }
 
 // low != nullptr: fused form for the pipeline - `low` [B,LH,LW,2] is up-sampled to `logits` [B,H,W,2] (written) and classified in one pass
 int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scratch, uint8_t* hand_mask, int32_t* max_loc,
-                           float* center, float* crop_size, float* scale_crop, cudaStream_t s, int* n_launch, const float* low, int LH,
-                           int LW, const int* count) {
+                           float* center, float* crop_size, float* scale_crop, cudaStream_t s, const float* low, int LH, int LW,
+                           const int* count) {
     H3D_REQUIRE(H > 0 && W > 0 && H <= H3D_PIPELINE_MAX_SIDE && W <= H3D_PIPELINE_MAX_SIDE,
                 "seg_postprocess: H, W must be in [1, %d] (H3D_PIPELINE_MAX_SIDE), got %dx%d", H3D_PIPELINE_MAX_SIDE, H, W);
     const int Ww = seg_words(W);
@@ -842,11 +843,8 @@ int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scrat
         seg_prob_kernel<false><<<grid, 256, 0, s>>>((const float2*)(low ? low : logits), nullptr, 0, 0, 0.f, 0.f, H, W, Ww, key, det, count);
     H3D_CHECK_LAUNCH();
     const int num_passes = std::max(H, W) / (21 / 2);   // utils/general.py:256
-    if (std::max(H, W) > 512) {   // one CTA's shared memory holds the masks up to 512 x 512; larger images are banded over a cluster
-        const int rc = launch_mask_grow_cluster(key, det, B, H, W, Ww, num_passes, hand_mask, max_loc, center, crop_size, scale_crop, s, count);
-        if (rc == H3D_OK && n_launch) *n_launch += 2;
-        return rc;
-    }
+    if (std::max(H, W) > 512)   // one CTA's shared memory holds the masks up to 512 x 512; larger images are banded over a cluster
+        return launch_mask_grow_cluster(key, det, B, H, W, Ww, num_passes, hand_mask, max_loc, center, crop_size, scale_crop, s, count);
     const size_t smem = grow_smem_bytes(H, Ww);    // det, obj, hor (+ zero padding rows)
     static bool attr_set[64] = {};   // per device (one process may drive several GPUs)
     int dev = 0;
@@ -858,7 +856,6 @@ int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scrat
     mask_grow_kernel<<<B, kGrowThreads, smem, s>>>(key, det, H, W, Ww, num_passes, hand_mask, max_loc, center, crop_size,
                                                    scale_crop, count);
     H3D_CHECK_LAUNCH();
-    if (n_launch) *n_launch += 2;
     return H3D_OK;
 }
 
@@ -986,8 +983,7 @@ __global__ void argmax_decode_kernel(const unsigned long long* __restrict__ key,
     }
 }
 
-int launch_detect_keypoints(const float* sm, int B, int H, int W, int C, void* scratch, int32_t* uv, cudaStream_t s,
-                            int* n_launch) {
+int launch_detect_keypoints(const float* sm, int B, int H, int W, int C, void* scratch, int32_t* uv, cudaStream_t s) {
     H3D_REQUIRE(C >= 1 && C <= 256, "detect_keypoints: C must be in [1,256]");
     unsigned long long* key = (unsigned long long*)scratch;
     H3D_CUDA(cudaMemsetAsync(key, 0, (size_t)B * C * 8, s));
@@ -999,7 +995,6 @@ int launch_detect_keypoints(const float* sm, int B, int H, int W, int C, void* s
     H3D_CHECK_LAUNCH();
     argmax_decode_kernel<<<ceil_div(B * C, 256), 256, 0, s>>>(key, B * C, W, uv);
     H3D_CHECK_LAUNCH();
-    if (n_launch) *n_launch += 2;
     return H3D_OK;
 }
 
@@ -1141,8 +1136,7 @@ __global__ void resize_argmax_pow2_kernel(const float* __restrict__ x, float* __
     }
 }
 
-int launch_resize_argmax21(const float* x, float* y, int B, int H, int W, int oh, int ow, void* scratch, int32_t* uv, cudaStream_t s,
-                           int* n_launch) {
+int launch_resize_argmax21(const float* x, float* y, int B, int H, int W, int oh, int ow, void* scratch, int32_t* uv, cudaStream_t s) {
     constexpr int C = 21;
     unsigned long long* key = (unsigned long long*)scratch;
     H3D_CUDA(cudaMemsetAsync(key, 0, (size_t)B * C * 8, s));
@@ -1157,7 +1151,6 @@ int launch_resize_argmax21(const float* x, float* y, int B, int H, int W, int oh
         H3D_CHECK_LAUNCH();
         argmax_decode_kernel<<<ceil_div(B * C, 256), 256, 0, s>>>(key, B * C, ow, uv);
         H3D_CHECK_LAUNCH();
-        if (n_launch) *n_launch += 2;
         return H3D_OK;
     }
     const int P = 256 / C;
@@ -1166,7 +1159,6 @@ int launch_resize_argmax21(const float* x, float* y, int B, int H, int W, int oh
     H3D_CHECK_LAUNCH();
     argmax_decode_kernel<<<ceil_div(B * C, 256), 256, 0, s>>>(key, B * C, ow, uv);
     H3D_CHECK_LAUNCH();
-    if (n_launch) *n_launch += 2;
     return H3D_OK;
 }
 

@@ -333,9 +333,7 @@ int64_t resize_grad_scratch_floats(int B, int H, int W, int C, int oh, int ow) {
     return (W != ow && H != oh) ? (int64_t)B * oh * W * C : 0;
 }
 
-int launch_resize_bilinear_tf1_grad(const float* dy, float* dx, float* scratch, int B, int H, int W, int C, int oh, int ow, cudaStream_t s,
-                                    int* n_launch) {
-    *n_launch = 0;
+int launch_resize_bilinear_tf1_grad(const float* dy, float* dx, float* scratch, int B, int H, int W, int C, int oh, int ow, cudaStream_t s) {
     if (H == oh && W == ow) {   // the forward copies
         H3D_CUDA(cudaMemcpyAsync(dx, dy, (size_t)B * H * W * C * sizeof(float), cudaMemcpyDeviceToDevice, s));
         return H3D_OK;
@@ -351,13 +349,11 @@ int launch_resize_bilinear_tf1_grad(const float* dy, float* dx, float* scratch, 
         else if (C == 2) resize_grad_cols_kernel<2><<<blocks, 256, 0, s>>>(dy, out, (int64_t)B * oh, W, ow, C, wscale);
         else resize_grad_cols_kernel<0><<<blocks, 256, 0, s>>>(dy, out, (int64_t)B * oh, W, ow, C, wscale);
         H3D_CHECK_LAUNCH();
-        ++*n_launch;
         t = out;
     }
     if (H != oh) {
         resize_grad_rows_kernel<<<grid_for((int64_t)B * H * W * C, 256), 256, 0, s>>>(t, dx, B, H, oh, (int64_t)W * C, hscale);
         H3D_CHECK_LAUNCH();
-        ++*n_launch;
     }
     return H3D_OK;
 }

@@ -86,12 +86,15 @@ H3D_API int h3d_set_tuning(h3d_ctx* ctx, const char* key, int value);
  * kernel trapped; 100 + r = h3d_gather_records_p2p
  * never saw peer rank r's records.  Returns H3D_OK or H3D_ECUDA (message in h3d_last_error); *code (optional) = the word. */
 H3D_API int h3d_check_errors(h3d_ctx* ctx, int* code);
-/* Number of kernels this library launched through `ctx` since creation (bench "gpu_launches"). */
+/* Number of kernels this library enqueued through `ctx` since creation (bench "gpu_launches"): every kernel an entry point
+ * taking `ctx` enqueues counts, kernels enqueued under stream capture included, whatever the entry returns.  Memory sets and
+ * copies do not count. */
 H3D_API int64_t h3d_launch_count(const h3d_ctx* ctx);
 
-/* Per-kernel-class device timing for bench.py's roofline: between begin and end every plan step is
- * bracketed by CUDA events on its launch stream.  Classes: 0 = tensor-core conv, 1 = CUDA-core conv,
- * 2 = fully connected, 3 = other.  end() synchronises and fills three arrays of length 4. */
+/* Per-kernel-class device timing for bench.py's roofline: between begin and end every plan step that
+ * launches a kernel is bracketed by CUDA events on its launch stream.  Classes: 0 = tensor-core conv,
+ * 1 = CUDA-core conv, 2 = fully connected, 3 = other.  end() synchronises and fills three arrays of
+ * length 4; launches_by_kind counts the bracketed steps. */
 H3D_API int h3d_profile_begin(h3d_ctx* ctx);
 H3D_API int h3d_profile_end(h3d_ctx* ctx, double* ms_by_kind, int64_t* flops_by_kind, int64_t* launches_by_kind);
 
