@@ -1785,6 +1785,8 @@ int h3d_conv2d_layer_planes(h3d_ctx* ctx, const float* x, int B, int H, int W, i
 
 int h3d_maxpool2x2_f32(h3d_ctx* ctx, const float* x, float* y, int B, int H, int W, int C, void* stream) {
     H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(x && y, "h3d_maxpool2x2_f32: x and y are required");
+    H3D_REQUIRE(B > 0 && H >= 2 && W >= 2 && C > 0, "h3d_maxpool2x2_f32: bad shape B=%d H=%d W=%d C=%d (H, W >= 2)", B, H, W, C);
     return launch_maxpool_f32(x, y, B, H, W, C, s);
 }
 int h3d_maxpool2x2_backward_f32(h3d_ctx* ctx, const float* x, const float* dy, float* dx, int B, int H, int W, int C, void* stream) {
@@ -1808,10 +1810,15 @@ int h3d_leaky_relu_f32(h3d_ctx* ctx, const float* x, float* y, int64_t n, void* 
 }
 int h3d_resize_bilinear_tf1(h3d_ctx* ctx, const float* x, float* y, int B, int H, int W, int C, int out_h, int out_w, void* stream) {
     H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(x && y, "h3d_resize_bilinear_tf1: x and y are required");
+    H3D_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && out_h > 0 && out_w > 0,
+                "h3d_resize_bilinear_tf1: bad shape B=%d H=%d W=%d C=%d out=%dx%d", B, H, W, C, out_h, out_w);
     return launch_resize_bilinear_tf1(x, y, B, H, W, C, out_h, out_w, s);
 }
 int h3d_avgpool8(h3d_ctx* ctx, const float* x, float* y, int B, int H, int W, int C, void* stream) {
     H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(x && y, "h3d_avgpool8: x and y are required");
+    H3D_REQUIRE(B > 0 && H >= 8 && W >= 8 && C > 0, "h3d_avgpool8: bad shape B=%d H=%d W=%d C=%d (H, W >= 8)", B, H, W, C);
     return launch_avgpool8(x, y, B, H, W, C, s);
 }
 int h3d_seg_postprocess(h3d_ctx* ctx, const float* logits, int B, int H, int W, uint8_t* hand_mask, int32_t* max_loc, float* center,
@@ -1834,10 +1841,15 @@ int h3d_calc_center_bb(h3d_ctx* ctx, const float* mask, int B, int H, int W, flo
 int h3d_crop_image_from_xy(h3d_ctx* ctx, const float* image, const float* center, const float* scale, float* image_crop, int B,
                            int H, int W, int C, int crop_size, void* stream) {
     H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(image && center && scale && image_crop, "h3d_crop_image_from_xy: image, center, scale and image_crop are required");
+    H3D_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && crop_size > 0 && (int64_t)crop_size * crop_size <= INT32_MAX,
+                "h3d_crop_image_from_xy: bad shape B=%d H=%d W=%d C=%d crop_size=%d", B, H, W, C, crop_size);
     return launch_crop_image(image, center, scale, image_crop, B, H, W, C, crop_size, s);
 }
 int h3d_detect_keypoints(h3d_ctx* ctx, const float* scoremaps, int B, int H, int W, int C, int32_t* keypoints_uv, void* stream) {
     H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(scoremaps && keypoints_uv, "h3d_detect_keypoints: scoremaps and keypoints_uv are required");
+    H3D_REQUIRE(B > 0 && H > 0 && W > 0 && (int64_t)H * W <= INT32_MAX, "h3d_detect_keypoints: bad shape B=%d H=%d W=%d", B, H, W);
     char* scratch = nullptr;
     int rc = op_scratch(ctx, argmax_scratch_bytes(B, C), &scratch);
     if (rc) return rc;
@@ -1846,7 +1858,9 @@ int h3d_detect_keypoints(h3d_ctx* ctx, const float* scoremaps, int B, int H, int
 int h3d_upsample_detect_keypoints(h3d_ctx* ctx, const float* scoremaps, int B, int H, int W, int out_h, int out_w, float* scoremaps_up,
                                   int32_t* keypoints_uv, void* stream) {
     H3D_OP_PROLOGUE(ctx);
-    H3D_REQUIRE(scoremaps && scoremaps_up && keypoints_uv && B > 0, "h3d_upsample_detect_keypoints: bad argument");
+    H3D_REQUIRE(scoremaps && scoremaps_up && keypoints_uv, "h3d_upsample_detect_keypoints: scoremaps, scoremaps_up and keypoints_uv are required");
+    H3D_REQUIRE(B > 0 && H > 0 && W > 0 && out_h > 0 && out_w > 0 && (int64_t)out_h * out_w <= INT32_MAX,
+                "h3d_upsample_detect_keypoints: bad shape B=%d H=%d W=%d out=%dx%d", B, H, W, out_h, out_w);
     char* scratch = nullptr;
     int rc = op_scratch(ctx, argmax_scratch_bytes(B, 21), &scratch);
     if (rc) return rc;

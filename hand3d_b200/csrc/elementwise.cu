@@ -18,6 +18,10 @@ __device__ __forceinline__ float lerp_tf(float a, float b, float t) {
     return __fadd_rn(a, __fmul_rn(__fsub_rn(b, a), t));
 }
 
+// The kernels that give each image its own grid row (blockIdx.y: seg_prob_kernel, crop_image_kernel and the three arg-max kernels) take
+// at most gridDim.y's limit of images per launch; their launchers refuse a larger batch before anything is enqueued.
+constexpr int kMaxGridImages = 65535;
+
 // =============================================================================================
 // tf.image.resize_images bilinear, align_corners=False, legacy (nets/ColorHandPose3DNetwork.py:97,128,166)
 // One thread produces 4 consecutive floats of the flattened (ox, c) output row -> float4 stores.
@@ -829,6 +833,7 @@ int launch_seg_postprocess(const float* logits, int B, int H, int W, void* scrat
                            const int* count) {
     H3D_REQUIRE(H > 0 && W > 0 && H <= H3D_PIPELINE_MAX_SIDE && W <= H3D_PIPELINE_MAX_SIDE,
                 "seg_postprocess: H, W must be in [1, %d] (H3D_PIPELINE_MAX_SIDE), got %dx%d", H3D_PIPELINE_MAX_SIDE, H, W);
+    H3D_REQUIRE(B <= kMaxGridImages, "seg_postprocess: B = %d is more than %d images per call", B, kMaxGridImages);
     const int Ww = seg_words(W);
     unsigned long long* key = (unsigned long long*)scratch;
     uint32_t* det = (uint32_t*)((char*)scratch + align_up((int64_t)B * 8, 256));
@@ -930,6 +935,7 @@ crop_image_kernel(const float* __restrict__ image, const float* __restrict__ cen
 
 int launch_crop_image(const float* image, const float* center, const float* scale, float* out, int B, int H, int W, int C,
                       int crop, cudaStream_t s) {
+    H3D_REQUIRE(B <= kMaxGridImages, "crop_image: B = %d is more than %d images per call", B, kMaxGridImages);
     const int total = crop * crop;
     // about one resident wave: 132 SMs x 8 CTAs of 256 threads, split over the images (at least 1, at most one CTA per 256 pixels)
     const int per_image = std::max(1, std::min(ceil_div(total, 256), ceil_div(132 * 8, std::max(1, B))));
@@ -943,9 +949,17 @@ int launch_crop_image(const float* image, const float* center, const float* scal
 // p, p+P, ... of channel c: consecutive threads read consecutive floats (NHWC), keys are reduced in
 // shared memory and merged with one 64-bit atomicMax per (block, channel).
 // =============================================================================================
-__device__ __forceinline__ uint32_t float_orderable(float v) {
-    const uint32_t u = __float_as_uint(v);
+// The rank of a value in np.argmax's order, as an unsigned integer: -0.0 ties +0.0, and every NaN (either sign, any payload) ranks above
+// +inf, so that the first NaN wins.  Every value ranks above 0, the key of "no pixel seen".  The 64-bit key of the three arg-max kernels
+// is (argmax_rank(v) << 32) | ~index: its maximum is the first occurrence of the maximum.
+__device__ __forceinline__ uint32_t argmax_rank(float v) {
+    if (v != v) return 0xFFFFFFFFu;
+    uint32_t u = __float_as_uint(v);
+    if (u == 0x80000000u) u = 0u;   // -0.0
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ unsigned long long argmax_key(float v, int p) {
+    return ((unsigned long long)argmax_rank(v) << 32) | (uint32_t)(0xFFFFFFFFu - (uint32_t)p);
 }
 
 int64_t argmax_scratch_bytes(int B, int C) { return align_up((int64_t)B * C * 8, 256); }
@@ -959,8 +973,7 @@ __global__ void heatmap_argmax_kernel(const float* __restrict__ sm, int HW, int 
     if (p_sub < P) {
         const float* base = sm + (int64_t)b * HW * C;
         for (int p = blockIdx.x * P + p_sub; p < HW; p += gridDim.x * P) {
-            const float v = __ldg(base + (int64_t)p * C + c);
-            const unsigned long long k = ((unsigned long long)float_orderable(v) << 32) | (uint32_t)(0xFFFFFFFFu - (uint32_t)p);
+            const unsigned long long k = argmax_key(__ldg(base + (int64_t)p * C + c), p);
             best = k > best ? k : best;
         }
         skey[p_sub * C + c] = best;
@@ -985,6 +998,7 @@ __global__ void argmax_decode_kernel(const unsigned long long* __restrict__ key,
 
 int launch_detect_keypoints(const float* sm, int B, int H, int W, int C, void* scratch, int32_t* uv, cudaStream_t s) {
     H3D_REQUIRE(C >= 1 && C <= 256, "detect_keypoints: C must be in [1,256]");
+    H3D_REQUIRE(B <= kMaxGridImages, "detect_keypoints: B = %d is more than %d images per call", B, kMaxGridImages);
     unsigned long long* key = (unsigned long long*)scratch;
     H3D_CUDA(cudaMemsetAsync(key, 0, (size_t)B * C * 8, s));
     const int P = std::max(1, 256 / C);
@@ -1043,7 +1057,7 @@ __global__ void resize_argmax_kernel(const float* __restrict__ x, float* __restr
             const float bl = __ldg(xb + (y1 * W + x0) * C + c), br = __ldg(xb + (y1 * W + x1) * C + c);
             const float v = lerp_tf(lerp_tf(tl, tr, lx), lerp_tf(bl, br, lx), ly);
             yb[(int64_t)p * C + c] = v;
-            const unsigned long long k = ((unsigned long long)float_orderable(v) << 32) | (uint32_t)(0xFFFFFFFFu - (uint32_t)p);
+            const unsigned long long k = argmax_key(v, p);
             best = k > best ? k : best;
         }
         skey[p_sub * C + c] = best;
@@ -1083,9 +1097,9 @@ __global__ void resize_argmax_pow2_kernel(const float* __restrict__ x, float* __
     int pofs[4], cc[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) { pofs[i] = (4 * j + i) / C; cc[i] = (4 * j + i) % C; }
-    float bv[4] = {0.f, 0.f, 0.f, 0.f};
+    // best rank and pixel per value slot; a thread's pixels are not in row-major order (rows inside groups), hence the explicit tie test
+    uint32_t bk[4] = {0u, 0u, 0u, 0u};
     int bp[4] = {0x7fffffff, 0x7fffffff, 0x7fffffff, 0x7fffffff};
-    bool have[4] = {false, false, false, false};
     const int groups = ow >> 2;                   // 4-pixel groups per output row
     float* yb = y + (int64_t)b * (int64_t)(H << s_log2) * ow * C;
     if (gsub < gstep) {
@@ -1109,7 +1123,8 @@ __global__ void resize_argmax_pow2_kernel(const float* __restrict__ x, float* __
                 for (int i = 0; i < 4; ++i) {
                     o[i] = lerp_tf(top[i], bot[i], ly);
                     const int pidx = oy * ow + 4 * g + pofs[i];
-                    if (!have[i] || o[i] > bv[i] || (o[i] == bv[i] && pidx < bp[i])) { bv[i] = o[i]; bp[i] = pidx; have[i] = true; }
+                    const uint32_t k = argmax_rank(o[i]);
+                    if (k > bk[i] || (k == bk[i] && pidx < bp[i])) { bk[i] = k; bp[i] = pidx; }
                 }
                 *reinterpret_cast<float4*>(yb + ((int64_t)oy * ow + 4 * g) * C + 4 * j) = make_float4(o[0], o[1], o[2], o[3]);
             }
@@ -1122,10 +1137,8 @@ __global__ void resize_argmax_pow2_kernel(const float* __restrict__ x, float* __
     if (gsub < gstep) {
 #pragma unroll
         for (int i = 0; i < 4; ++i)
-            if (have[i]) {
-                const unsigned long long k = ((unsigned long long)float_orderable(bv[i]) << 32) | (uint32_t)(0xFFFFFFFFu - (uint32_t)bp[i]);
-                skey[cc[i] * slots + gsub * 4 + pofs[i]] = k;            // (gsub, pixel offset) is unique per channel
-            }
+            if (bk[i])   // (gsub, pixel offset) is unique per channel
+                skey[cc[i] * slots + gsub * 4 + pofs[i]] = ((unsigned long long)bk[i] << 32) | (uint32_t)(0xFFFFFFFFu - (uint32_t)bp[i]);
     }
     __syncthreads();
     H3D_SKEW(SKEW_TICKET, 0);
@@ -1138,6 +1151,7 @@ __global__ void resize_argmax_pow2_kernel(const float* __restrict__ x, float* __
 
 int launch_resize_argmax21(const float* x, float* y, int B, int H, int W, int oh, int ow, void* scratch, int32_t* uv, cudaStream_t s) {
     constexpr int C = 21;
+    H3D_REQUIRE(B <= kMaxGridImages, "upsample_detect_keypoints: B = %d is more than %d images per call", B, kMaxGridImages);
     unsigned long long* key = (unsigned long long*)scratch;
     H3D_CUDA(cudaMemsetAsync(key, 0, (size_t)B * C * 8, s));
     // integer power-of-two up-sampling in both directions (x8 on the hot path): row-group kernel

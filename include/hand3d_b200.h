@@ -317,7 +317,7 @@ H3D_API int h3d_avgpool8(h3d_ctx* ctx, const float* x, float* y, int B, int H, i
 /* single_obj_scoremap + calc_center_bb + crop-scale glue (utils/general.py:233-328,
  * nets/ColorHandPose3DNetwork.py:83-85).  logits [B,H,W,2] -> hand_mask [B,H,W] uint8 (optional),
  * max_loc [B,2] int32 (optional, find_max_location), center [B,2], crop_size [B,1] (raw, optional),
- * scale_crop [B,1].  1 <= H, W <= H3D_PIPELINE_MAX_SIDE (a larger map returns H3D_EINVAL before anything is enqueued),
+ * scale_crop [B,1].  1 <= H, W <= H3D_PIPELINE_MAX_SIDE and B <= 65535 (else H3D_EINVAL before anything is enqueued),
  * W % 32 == 0 not required.  Up to 512 a side one CTA grows the mask; larger maps are split into row bands over a thread-block
  * cluster, with the same result. */
 H3D_API int h3d_seg_postprocess(h3d_ctx* ctx, const float* logits, int B, int H, int W, uint8_t* hand_mask,
@@ -327,15 +327,18 @@ H3D_API int h3d_seg_postprocess(h3d_ctx* ctx, const float* logits, int B, int H,
  * gives center (160, 160), crop_size 100, bb (+inf, -inf) as the reference's tf.cond fall-backs do. */
 H3D_API int h3d_calc_center_bb(h3d_ctx* ctx, const float* mask, int B, int H, int W, float* center, float* bb, float* crop_size,
                                void* stream);
-/* crop_image_from_xy (utils/general.py:163-196) incl. tf.image.crop_and_resize bilinear/extrapolation 0. */
+/* crop_image_from_xy (utils/general.py:163-196) incl. tf.image.crop_and_resize bilinear/extrapolation 0.  1 <= B <= 65535,
+ * crop_size^2 <= 2^31 - 1. */
 H3D_API int h3d_crop_image_from_xy(h3d_ctx* ctx, const float* image, const float* center, const float* scale,
                            float* image_crop, int B, int H, int W, int C, int crop_size, void* stream);
-/* detect_keypoints (utils/general.py:331-344), batched: scoremaps [B,H,W,C] -> [B,C,2] int32 (row,col),
- * first occurrence of the maximum in row-major order. */
+/* detect_keypoints (utils/general.py:331-344), batched: scoremaps [B,H,W,C] -> [B,C,2] int32 (row,col) of np.argmax per channel:
+ * the first occurrence of the maximum in row-major order, where -0.0 ties +0.0 and every NaN (either sign) ranks above +inf, so the
+ * first NaN wins.  1 <= C <= 256, 1 <= B <= 65535, H W <= 2^31 - 1. */
 H3D_API int h3d_detect_keypoints(h3d_ctx* ctx, const float* scoremaps, int B, int H, int W, int C,
                          int32_t* keypoints_uv, void* stream);
 /* tf.image.resize_images (nets/ColorHandPose3DNetwork.py:96-97) fused with detect_keypoints: 21-channel score maps [B,H,W,21] ->
- * scoremaps_up [B,out_h,out_w,21] and keypoints_uv [B,21,2] int32 (row, col) of the up-sampled maps in one pass. */
+ * scoremaps_up [B,out_h,out_w,21] and keypoints_uv [B,21,2] int32 (row, col) of the up-sampled maps in one pass, with the arg-max
+ * rules of h3d_detect_keypoints.  1 <= B <= 65535, out_h out_w <= 2^31 - 1. */
 H3D_API int h3d_upsample_detect_keypoints(h3d_ctx* ctx, const float* scoremaps, int B, int H, int W, int out_h, int out_w,
                                           float* scoremaps_up, int32_t* keypoints_uv, void* stream);
 /* Per-image result record (SURVEY.md 8(e)): coord3d [21,3] | keypoints_uv [21,2] i32 (bit-cast) | center [2] | scale_crop [1]
