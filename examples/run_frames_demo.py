@@ -9,6 +9,9 @@
     python examples/run_frames_demo.py --weights weights/   # the reference's pickled weights
     python examples/run_frames_demo.py --track --draw-dir out   # also writes the frames of the first batch with the skeleton and
                                                                 # the crop square drawn on the device (PNG, Pillow)
+    python examples/run_frames_demo.py --source video:main.mp4 --source raw:side.nv12:nv12:720x1280 \
+        --source synthetic:yuyv:480x640 --track --detect slots  # a camera rig: one batch slot per source, each with its own size
+                                                                # and pixel format, served by one FrameRunner
 """
 import argparse
 import os
@@ -55,6 +58,28 @@ def raw_video_batches(path, pixel_format, B, H, W, max_batches):
         yield np.ascontiguousarray(frames[i * B:(i + 1) * B])
 
 
+def source(spec, n_frames, seed):
+    """--source SPEC -> (pixel_format, (H, W), iterator of frames): video:PATH (decoded with OpenCV, BGR), raw:PATH:FMT:HxW
+    (concatenated raw frames) or synthetic:FMT:HxW (seeded random bytes of that layout)."""
+    kind, _, rest = spec.partition(":")
+    if kind == "video":
+        import cv2
+        cap = cv2.VideoCapture(rest)
+        hw = (int(cap.get(cv2.CAP_PROP_FRAME_HEIGHT)), int(cap.get(cv2.CAP_PROP_FRAME_WIDTH)))
+        cap.release()
+        return "bgr", hw, (b[0] for b in video_batches(rest, 1, n_frames))
+    path, fmt, size = rest.rsplit(":", 2) if kind == "raw" else (None,) + tuple(rest.split(":", 1))
+    if kind not in ("raw", "synthetic") or "x" not in size:
+        raise SystemExit("--source %r: expected video:PATH, raw:PATH:FMT:HxW or synthetic:FMT:HxW" % spec)
+    hw = tuple(int(v) for v in size.split("x"))
+    if kind == "raw":
+        return fmt, hw, (b[0] for b in raw_video_batches(path, fmt, 1, hw[0], hw[1], n_frames))
+    from hand3d_b200.frames import frame_shape
+    shape = frame_shape(fmt, *hw)
+    rng = np.random.default_rng(seed)
+    return fmt, hw, (rng.integers(0, 256, shape, dtype=np.uint8) for _ in range(n_frames))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--video", default=None, help="video file (cv2 decodes it); default: synthetic frames")
@@ -76,6 +101,9 @@ def main():
     ap.add_argument("--draw-dir", default=None, help="draw the skeleton and the crop square into the frames on the device and write "
                                                      "them there as PNG files")
     ap.add_argument("--draw-batches", type=int, default=1, help="with --draw-dir: how many batches to write")
+    ap.add_argument("--source", action="append", default=None,
+                    help="a camera of a rig, repeated once per batch slot: video:PATH, raw:PATH:FMT:HxW or synthetic:FMT:HxW (FMT one of "
+                         "rgb, bgr, nv12, i420, yuyv); --batches steps of one frame per camera, --batch is ignored")
     args = ap.parse_args()
 
     from hand3d_b200 import runtime, weights as Wt
@@ -91,7 +119,12 @@ def main():
     ctx = runtime.default_context()
 
     pixel_format = "rgb"
-    if args.raw_video:
+    if args.source:
+        cams = [source(spec, args.batches, args.seed + i) for i, spec in enumerate(args.source)]
+        pixel_format, hw = [c[0] for c in cams], [c[1] for c in cams]
+        args.batch = len(cams)
+        batches = (list(frames) for frames in zip(*[c[2] for c in cams]))
+    elif args.raw_video:
         if args.pixel_format is None:
             ap.error("--raw-video needs --pixel-format")
         hw = (args.height, args.width)
@@ -126,7 +159,8 @@ def main():
         if args.draw_dir and i < args.draw_batches:
             for b, frame in enumerate(r["frame_drawn"]):
                 Image.fromarray(frame).save(os.path.join(args.draw_dir, "batch%03d_frame%02d.png" % (i, b)))
-        print("batch %d: frame 0 key-points (row, col) in %dx%d pixels: wrist %s, index tip %s%s" % (i, hw[0], hw[1], np.round(kp[0], 1),
+        H, W = hw[0] if args.source else hw
+        print("batch %d: frame 0 key-points (row, col) in %dx%d pixels: wrist %s, index tip %s%s" % (i, H, W, np.round(kp[0], 1),
                                                                                                  np.round(kp[8], 1), track))
     dt = time.perf_counter() - t0
     print("%d frames in %.3f s: %.1f frames/s" % (n, dt, n / dt if dt > 0 else 0.0))

@@ -117,6 +117,13 @@ SIGNATURES = {
     "h3d_dropout_backward": (_i, [_p, _p, _p, _i, _i, _f, _p, _p]),
     "h3d_dropout_advance": (_i, [_p, _p]),
 }
+# the camera-rig entries (include/hand3d_b200_rig.h, included by hand3d_b200.h), bound by load() like the ones above; their launch
+# counts are checked against the profiler by tests/test_gpu_frames_rig.py
+RIG_SIGNATURES = {
+    "h3d_frame_rig_query": (_i, [_i, _p, _p, _i, _i, _p, C.POINTER(_i64), _p, C.POINTER(_i64)]),
+    "h3d_frame_rig_plan": (_i, [_p, _i, _p, _p, _i, _i, _p]),
+    "h3d_resize_frames_rig": (_i, [_p, _p, _i, _p, _p, _i, _i, _i, _p, _p]),
+}
 ADAM_STATE_WORDS = 4   # H3D_ADAM_STATE_WORDS
 # training-mode reader augmentation (H3D_AUG_*): flags, and the per-sample parameter layout
 AUG_COORD_UV_NOISE, AUG_CROP_CENTER_NOISE, AUG_CROP_SCALE_NOISE, AUG_CROP_OFFSET_NOISE, AUG_HUE, AUG_RANDOM_CROP, AUG_SCOREMAP_DROPOUT = 1, 2, 4, 8, 16, 32, 64
@@ -128,6 +135,11 @@ READER_QUEUE_CAPACITY, READER_STATE_COUNT, READER_STATE_NEXT, READER_STATE_SLOTS
 FRAME_MAX_SIDE, FRAME_MAX_OUT = 4096, 512
 # pixel formats of camera frames (H3D_PIXEL_*), by the names hand3d_b200.frames takes
 PIXEL_FORMATS = {"rgb": 0, "bgr": 1, "nv12": 2, "i420": 3, "yuyv": 4}
+# camera rigs (H3D_FRAME_RIG_*, H3D_RIG_*): the most slots, and the layout of h3d_frame_rig_query's table
+FRAME_RIG_MAX_SLOTS, FRAME_RIG_SLOT_WORDS, FRAME_RIG_LAUNCH_WORDS = 64, 24, 4
+RIG_FORMAT, RIG_H, RIG_W, RIG_KXS, RIG_KYS, RIG_BAND, RIG_CHUNK, RIG_ROW_STRIDE, RIG_NBANDS = 0, 1, 2, 3, 4, 5, 6, 7, 8
+RIG_ACC_BYTES, RIG_INTER_BYTES, RIG_SMEM, RIG_SEG_OFF, RIG_RGB_STRIDE, RIG_XB, RIG_KX, RIG_YB, RIG_KY, RIG_CTA0, RIG_SIZE = 9, 10, 11, 12, 15, 16, 17, 18, 19, 20, 21
+RIG_LAUNCH_FIRST, RIG_LAUNCH_SLOTS, RIG_LAUNCH_CTAS, RIG_LAUNCH_SMEM = 0, 1, 2, 3
 # the largest image side of h3d_pipeline_forward and h3d_seg_postprocess (H3D_PIPELINE_MAX_SIDE)
 PIPELINE_MAX_SIDE = 2048
 # tracking state (H3D_TRACK_*): the word offset of each array, in units of B words
@@ -156,7 +168,7 @@ def load():
         from . import build as _build
         _build.build()
     lib = C.CDLL(LIB_PATH)
-    for name, (res, args) in SIGNATURES.items():
+    for name, (res, args) in list(SIGNATURES.items()) + list(RIG_SIGNATURES.items()):
         fn = getattr(lib, name)   # AttributeError if the header and the library drifted apart
         fn.restype = res
         fn.argtypes = args

@@ -44,7 +44,7 @@ def _nvcc():
 
 def _digest(skew=False):
     h = hashlib.sha256()
-    names = sorted(os.listdir(CSRC)) + [os.path.join("..", "..", "include", "hand3d_b200.h")]
+    names = sorted(os.listdir(CSRC)) + [os.path.join("..", "..", "include", h) for h in ("hand3d_b200.h", "hand3d_b200_rig.h")]
     for n in names:
         p = os.path.join(CSRC, n)
         if os.path.isfile(p):

@@ -198,6 +198,8 @@ struct h3d_ctx {
     // h3d_resize_frames(_fmt) plans by (format, Hf, Wf, h, w): created outside graph capture, freed only by h3d_destroy (captured graphs
     // point into their coefficients, so adding a plan never frees or moves another)
     std::map<std::array<int, 5>, FramePlan*> frame_plans;
+    // h3d_resize_frames_rig plans by (out_h, out_w, then format, H, W per slot): the same lifetime rule
+    std::map<std::vector<int>, FrameRigPlan*> frame_rig_plans;
 };
 
 namespace h3d {
@@ -1008,7 +1010,7 @@ static int check_device() {
 extern "C" {
 
 const char* h3d_last_error(void) { return g_err; }
-int h3d_version(void) { return 111; }
+int h3d_version(void) { return 112; }
 
 int h3d_device_available(void) {
     int n = 0;
@@ -1096,6 +1098,7 @@ int h3d_destroy(h3d_ctx* ctx) {
     if (ctx->track_sel) cudaFree(ctx->track_sel);
     if (ctx->track_crop) cudaFree(ctx->track_crop);
     for (auto& kv : ctx->frame_plans) frame_plan_destroy(kv.second);
+    for (auto& kv : ctx->frame_rig_plans) frame_rig_plan_destroy(kv.second);
     return H3D_OK;
 }
 
@@ -1952,7 +1955,78 @@ int resize_frames(h3d_ctx* ctx, const char* fn, const uint8_t* frames, int forma
     return launch_resize_frames(it->second, frames, B, normalize, out, s);
 }
 
+// A rig's slots, each by the pixel-format table with its index in the message, and the output size.
+int check_frame_rig(const char* fn, int B, const int* formats, const int* hw, int out_h, int out_w) {
+    H3D_REQUIRE(formats && hw, "%s: bad argument", fn);
+    H3D_REQUIRE(B >= 1 && B <= H3D_FRAME_RIG_MAX_SLOTS, "%s: a rig has 1..%d slots, got %d", fn, H3D_FRAME_RIG_MAX_SLOTS, B);
+    H3D_REQUIRE(out_h >= 1 && out_h <= H3D_FRAME_MAX_OUT && out_w >= 1 && out_w <= H3D_FRAME_MAX_OUT, "%s: the output must be 1..%d a side, "
+                "got %dx%d", fn, H3D_FRAME_MAX_OUT, out_h, out_w);
+    for (int b = 0; b < B; ++b) {
+        char name[96];
+        snprintf(name, sizeof(name), "%s: slot %d", fn, b);
+        const int rc = check_frame_format(name, formats[b], hw[2 * b], hw[2 * b + 1]);
+        if (rc) return rc;
+    }
+    return H3D_OK;
+}
+
+int frame_rig_plan(h3d_ctx* ctx, const char* fn, int B, const int* formats, const int* hw, int out_h, int out_w, cudaStream_t s,
+                   FrameRigPlan** plan) {
+    std::vector<int> key{out_h, out_w};
+    for (int b = 0; b < B; ++b) key.insert(key.end(), {formats[b], hw[2 * b], hw[2 * b + 1]});
+    auto it = ctx->frame_rig_plans.find(key);
+    if (it == ctx->frame_rig_plans.end()) {
+        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+        H3D_CUDA(cudaStreamIsCapturing(s, &cs));
+        H3D_REQUIRE(cs == cudaStreamCaptureStatusNone,
+                    "%s: this rig of %d slots -> %dx%d has no plan, and its plan cannot be built under capture (its table is uploaded with "
+                    "a host-to-device copy): build it first (h3d_frame_rig_plan, or one resize outside capture)", fn, B, out_h, out_w);
+        FrameRigPlan* p = frame_rig_plan_create(B, formats, hw, out_h, out_w, s);
+        if (!p) return H3D_ECUDA;
+        it = ctx->frame_rig_plans.emplace(key, p).first;
+    }
+    *plan = it->second;
+    return H3D_OK;
+}
+
 }  // namespace
+
+int h3d_frame_rig_query(int B, const int* formats, const int* hw, int out_h, int out_w, int32_t* table, int64_t* table_words, int32_t* coef,
+                        int64_t* coef_words) {
+    H3D_REQUIRE(table_words && coef_words, "h3d_frame_rig_query: bad argument");
+    int rc = check_frame_rig("h3d_frame_rig_query", B, formats, hw, out_h, out_w);
+    if (rc) return rc;
+    std::vector<int32_t> t, c;
+    frame_rig_layout(B, formats, hw, out_h, out_w, t, c);
+    H3D_REQUIRE(!table || *table_words >= (int64_t)t.size(), "h3d_frame_rig_query: the table needs %lld words, got %lld",
+                (long long)t.size(), (long long)*table_words);
+    H3D_REQUIRE(!coef || *coef_words >= (int64_t)c.size(), "h3d_frame_rig_query: the coefficients need %lld words, got %lld",
+                (long long)c.size(), (long long)*coef_words);
+    if (table) memcpy(table, t.data(), t.size() * 4);
+    if (coef) memcpy(coef, c.data(), c.size() * 4);
+    *table_words = (int64_t)t.size();
+    *coef_words = (int64_t)c.size();
+    return H3D_OK;
+}
+int h3d_frame_rig_plan(h3d_ctx* ctx, int B, const int* formats, const int* hw, int out_h, int out_w, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    int rc = check_frame_rig("h3d_frame_rig_plan", B, formats, hw, out_h, out_w);
+    if (rc) return rc;
+    FrameRigPlan* p = nullptr;
+    return frame_rig_plan(ctx, "h3d_frame_rig_plan", B, formats, hw, out_h, out_w, s, &p);
+}
+int h3d_resize_frames_rig(h3d_ctx* ctx, const uint8_t* const* frames, int B, const int* formats, const int* hw, int out_h, int out_w,
+                          int normalize, void* out, void* stream) {
+    H3D_OP_PROLOGUE(ctx);
+    H3D_REQUIRE(frames && out && (normalize == 0 || normalize == 1), "h3d_resize_frames_rig: bad argument");
+    int rc = check_frame_rig("h3d_resize_frames_rig", B, formats, hw, out_h, out_w);
+    if (rc) return rc;
+    for (int b = 0; b < B; ++b) H3D_REQUIRE(frames[b], "h3d_resize_frames_rig: slot %d: frames[%d] is NULL", b, b);
+    FrameRigPlan* p = nullptr;
+    rc = frame_rig_plan(ctx, "h3d_resize_frames_rig", B, formats, hw, out_h, out_w, s, &p);
+    if (rc) return rc;
+    return launch_resize_frames_rig(p, frames, normalize, out, s);
+}
 
 int h3d_resize_frames(h3d_ctx* ctx, const uint8_t* frames, int B, int H, int W, int out_h, int out_w, int normalize, void* out, void* stream) {
     H3D_OP_PROLOGUE(ctx);

@@ -8,6 +8,7 @@
 #include <algorithm>
 #include <cmath>
 #include <string>
+#include <vector>
 
 #include "../../include/hand3d_b200.h"
 
@@ -176,6 +177,11 @@ struct FramePlan;   // opaque: the coefficients of one (format, Hf, Wf, h, w) on
 FramePlan* frame_plan_create(int fmt, int Hf, int Wf, int h, int w, cudaStream_t s);
 void frame_plan_destroy(FramePlan* p);
 int launch_resize_frames(const FramePlan* p, const uint8_t* frames, int B, int normalize, void* out, cudaStream_t s);
+struct FrameRigPlan;   // opaque: a camera rig's slot table and coefficients on the device (include/hand3d_b200.h)
+void frame_rig_layout(int B, const int* fmt, const int* hw, int h, int w, std::vector<int32_t>& table, std::vector<int32_t>& coef);
+FrameRigPlan* frame_rig_plan_create(int B, const int* fmt, const int* hw, int h, int w, cudaStream_t s);
+void frame_rig_plan_destroy(FrameRigPlan* p);
+int launch_resize_frames_rig(const FrameRigPlan* p, const uint8_t* const* frames, int normalize, void* out, cudaStream_t s);
 // frames of format fmt (H3D_PIXEL_*, arguments checked) -> uint8 RGB [B,H,W,3]
 int launch_convert_frames(const uint8_t* frames, int fmt, int B, int H, int W, uint8_t* out, cudaStream_t s);
 

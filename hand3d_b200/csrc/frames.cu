@@ -17,6 +17,7 @@
 // I420: the Y row, its U row and its V row; YUYV: the packed row), each 16-byte aligned in its own slot, and convert them once per
 // source pixel into an RGB chunk in shared memory (OpenCV's cvtColor BT.601 rule below), which the horizontal pass reads as the RGB
 // instance reads its stage.  The plan pays for that chunk with fewer rows per stage.
+#include <array>
 #include <cstring>
 #include <vector>
 
@@ -147,11 +148,11 @@ __device__ __forceinline__ void yuv_pair(const FrameArgs& a, const YuvArgs& ya, 
     }
 }
 
+// One CTA's work: output rows [band * a.band, +a.band) of output image b, read from the frame at img.  Shared by the batch kernel
+// (one size and format per launch) and the rig kernel (a size per slot), force-inlined so that each keeps its own register allocation.
 template <int FMT>
-__global__ void __launch_bounds__(kFrameThreads, 2) resize_frames_kernel(FrameArgs a, YuvArgs ya) {
+__device__ __forceinline__ void resize_band(const FrameArgs& a, const YuvArgs& ya, const uint8_t* img, int band, int64_t b) {
     extern __shared__ __align__(16) uint8_t smem[];
-    const int band = blockIdx.x % a.nbands;
-    const int64_t b = blockIdx.x / a.nbands;
     const int y0 = band * a.band, y1 = min(a.h, y0 + a.band), ny = y1 - y0;
     const int w3 = a.w * 3;
     int32_t* acc = reinterpret_cast<int32_t*>(smem);                     // [band][w3]
@@ -160,7 +161,6 @@ __global__ void __launch_bounds__(kFrameThreads, 2) resize_frames_kernel(FrameAr
     const int64_t stage_bytes = (int64_t)a.chunk * a.row_stride;
     uint8_t* rgb = stage + 2 * stage_bytes;                              // YUV formats: [chunk][rgb_stride], the converted chunk
     const int64_t rb = (int64_t)a.Wf * 3;
-    const uint8_t* img = is_yuv(FMT) ? a.in + b * ya.frame_bytes : a.in + b * a.Hf * rb;
     const int r0 = a.yb[2 * y0], r1 = a.yb[2 * (y1 - 1)] + a.yb[2 * (y1 - 1) + 1];   // the band's input rows (bounds are monotone)
     const int nchunks = (r1 - r0 + a.chunk - 1) / a.chunk;
 
@@ -233,6 +233,53 @@ __global__ void __launch_bounds__(kFrameThreads, 2) resize_frames_kernel(FrameAr
         uint8_t* out = static_cast<uint8_t*>(a.out) + o;
         for (int i = threadIdx.x; i < ny * w3; i += kFrameThreads) out[i] = (uint8_t)clip8(acc[i]);
     }
+}
+
+template <int FMT>
+__global__ void __launch_bounds__(kFrameThreads, 2) resize_frames_kernel(FrameArgs a, YuvArgs ya) {
+    const int band = blockIdx.x % a.nbands;
+    const int64_t b = blockIdx.x / a.nbands;
+    const uint8_t* img = is_yuv(FMT) ? a.in + b * ya.frame_bytes : a.in + b * a.Hf * ((int64_t)a.Wf * 3);
+    resize_band<FMT>(a, ya, img, band, b);
+}
+
+// A camera rig (DESIGN.md section 4.19): the slots of one format, each with its own size, in one launch.  The plan's table (in device
+// memory) holds each slot's geometry and coefficient offsets; the frame pointers are kernel parameters, so the plan serves any buffers.
+struct RigArgs {
+    const int32_t* table;    // include/hand3d_b200.h: B slot records, the order [B], the launch records
+    const int32_t* coef;     // the normalisation table, then the coefficient tables of each distinct size
+    void* out;
+    int B, h, w, normalize, first, nslots;    // first: this launch's first position in the order
+    const uint8_t* in[H3D_FRAME_RIG_MAX_SLOTS];
+};
+
+// The slot's arguments are read once into shared memory, where the band reads them as the batch kernel reads its parameters: held
+// in registers, they would not fit the 64 that two CTAs per SM leave.
+template <int FMT>
+__global__ void __launch_bounds__(kFrameThreads, 2) resize_frames_rig_kernel(const __grid_constant__ RigArgs r) {
+    __shared__ FrameArgs a;
+    __shared__ YuvArgs ya;
+    __shared__ int slot, band;
+    if (threadIdx.x == 0) {
+        const int32_t* order = r.table + (int64_t)r.B * H3D_FRAME_RIG_SLOT_WORDS + r.first;
+        int i = 0;           // the launch's slots cover consecutive CTA ranges in order: the last one starting at or before this CTA
+        while (i + 1 < r.nslots && r.table[order[i + 1] * H3D_FRAME_RIG_SLOT_WORDS + H3D_RIG_CTA0] <= (int)blockIdx.x) ++i;
+        const int b = order[i];
+        const int32_t* e = r.table + b * H3D_FRAME_RIG_SLOT_WORDS;
+        a.in = r.in[b]; a.out = r.out; a.Hf = e[H3D_RIG_H]; a.Wf = e[H3D_RIG_W]; a.h = r.h; a.w = r.w; a.normalize = r.normalize;
+        a.kxs = e[H3D_RIG_KXS]; a.kys = e[H3D_RIG_KYS]; a.band = e[H3D_RIG_BAND]; a.chunk = e[H3D_RIG_CHUNK];
+        a.row_stride = e[H3D_RIG_ROW_STRIDE]; a.nbands = e[H3D_RIG_NBANDS];
+        a.acc_bytes = e[H3D_RIG_ACC_BYTES]; a.inter_bytes = e[H3D_RIG_INTER_BYTES];
+        a.xb = r.coef + e[H3D_RIG_XB]; a.kx = r.coef + e[H3D_RIG_KX]; a.yb = r.coef + e[H3D_RIG_YB]; a.ky = r.coef + e[H3D_RIG_KY];
+        a.lut = reinterpret_cast<const float*>(r.coef);
+        ya.frame_bytes = 0;
+        for (int k = 0; k < 3; ++k) ya.seg_off[k] = e[H3D_RIG_SEG_OFF + k];
+        ya.rgb_stride = e[H3D_RIG_RGB_STRIDE];
+        slot = b;
+        band = (int)blockIdx.x - e[H3D_RIG_CTA0];
+    }
+    __syncthreads();
+    resize_band<FMT>(a, ya, a.in, band, slot);
 }
 
 // Full-size conversion of any format into packed RGB: one thread per chroma block (2x2 for NV12 and I420, 2x1 for YUYV; one pixel for
@@ -342,6 +389,30 @@ const void* resize_kernel_of(int fmt) {
     }
 }
 
+// The launch geometry of a plan of p.fmt, p.Hf x p.Wf -> p.h x p.w (p.kxs and p.kys set): shared by single-size plans and rig slots.
+void frame_geometry(FramePlan& p) {
+    const int w3 = 3 * p.w;
+    if (is_yuv(p.fmt)) {
+        // a staged row is one 16-byte aligned slot per segment; the converted chunk takes its share of both stage buffers' budget
+        const int n = p.fmt == H3D_PIXEL_I420 ? 3 : p.fmt == H3D_PIXEL_NV12 ? 2 : 1;
+        const int len[3] = {p.fmt == H3D_PIXEL_YUYV ? 2 * p.Wf : p.Wf, p.fmt == H3D_PIXEL_NV12 ? p.Wf : p.Wf / 2, p.Wf / 2};
+        for (int i = 0; i < n; ++i) {
+            p.seg_off[i] = p.row_stride;
+            p.row_stride += (int)align_up((int64_t)len[i] + 15, 16);
+        }
+        p.rgb_stride = (int)align_up((int64_t)p.Wf * 3, 16);
+        p.chunk = std::max(1, std::min(kMaxChunk, 2 * kStageBudget / (2 * p.row_stride + p.rgb_stride)));
+    } else {
+        p.row_stride = (int)align_up((int64_t)p.Wf * 3 + 15, 16);
+        p.chunk = std::max(1, std::min(kMaxChunk, kStageBudget / p.row_stride));
+    }
+    p.band = std::max(1, std::min({kMaxBand, p.h, kAccBudget / (w3 * 4)}));
+    p.nbands = ceil_div(p.h, p.band);
+    p.acc_bytes = (int)align_up((int64_t)p.band * w3 * 4, 16);
+    p.inter_bytes = (int)align_up((int64_t)p.chunk * w3, 16);
+    p.smem = p.acc_bytes + p.inter_bytes + 2 * p.chunk * p.row_stride + p.chunk * p.rgb_stride;
+}
+
 }  // namespace
 
 FramePlan* frame_plan_create(int fmt, int Hf, int Wf, int h, int w, cudaStream_t s) {
@@ -350,26 +421,7 @@ FramePlan* frame_plan_create(int fmt, int Hf, int Wf, int h, int w, cudaStream_t
     std::vector<int32_t> xb, kx, yb, ky;
     p->kxs = pil_bilinear_coeffs(Wf, w, xb, kx);
     p->kys = pil_bilinear_coeffs(Hf, h, yb, ky);
-    const int w3 = 3 * w;
-    if (is_yuv(fmt)) {
-        // a staged row is one 16-byte aligned slot per segment; the converted chunk takes its share of both stage buffers' budget
-        const int n = fmt == H3D_PIXEL_I420 ? 3 : fmt == H3D_PIXEL_NV12 ? 2 : 1;
-        const int len[3] = {fmt == H3D_PIXEL_YUYV ? 2 * Wf : Wf, fmt == H3D_PIXEL_NV12 ? Wf : Wf / 2, Wf / 2};
-        for (int i = 0; i < n; ++i) {
-            p->seg_off[i] = p->row_stride;
-            p->row_stride += (int)align_up((int64_t)len[i] + 15, 16);
-        }
-        p->rgb_stride = (int)align_up((int64_t)Wf * 3, 16);
-        p->chunk = std::max(1, std::min(kMaxChunk, 2 * kStageBudget / (2 * p->row_stride + p->rgb_stride)));
-    } else {
-        p->row_stride = (int)align_up((int64_t)Wf * 3 + 15, 16);
-        p->chunk = std::max(1, std::min(kMaxChunk, kStageBudget / p->row_stride));
-    }
-    p->band = std::max(1, std::min({kMaxBand, h, kAccBudget / (w3 * 4)}));
-    p->nbands = ceil_div(h, p->band);
-    p->acc_bytes = (int)align_up((int64_t)p->band * w3 * 4, 16);
-    p->inter_bytes = (int)align_up((int64_t)p->chunk * w3, 16);
-    p->smem = p->acc_bytes + p->inter_bytes + 2 * p->chunk * p->row_stride + p->chunk * p->rgb_stride;
+    frame_geometry(*p);
     auto& v = p->host;
     const size_t oxb = 0, okx = oxb + xb.size(), oyb = okx + kx.size(), oky = oyb + yb.size(), olut = oky + ky.size();
     v.resize(olut + 256);
@@ -443,6 +495,146 @@ int launch_convert_frames(const uint8_t* frames, int fmt, int B, int H, int W, u
         default: convert_frames_kernel<H3D_PIXEL_RGB><<<(unsigned)grid, 256, 0, s>>>(frames, out, H, W, blocks); break;
     }
     H3D_CHECK_LAUNCH();
+    return H3D_OK;
+}
+
+// ---- camera rigs (DESIGN.md section 4.19)
+
+struct FrameRigPlan {
+    int B = 0, h = 0, w = 0;
+    int launch[H3D_PIXEL_YUYV + 1][H3D_FRAME_RIG_LAUNCH_WORDS] = {};
+    std::vector<int32_t> host;      // [table | coef], the source of the asynchronous upload, kept for the plan's lifetime
+    int32_t* dev = nullptr;
+    const int32_t *table = nullptr, *coef = nullptr;
+};
+
+namespace {
+
+const void* rig_kernel_of(int fmt) {
+    switch (fmt) {
+        case H3D_PIXEL_BGR: return (const void*)resize_frames_rig_kernel<H3D_PIXEL_BGR>;
+        case H3D_PIXEL_NV12: return (const void*)resize_frames_rig_kernel<H3D_PIXEL_NV12>;
+        case H3D_PIXEL_I420: return (const void*)resize_frames_rig_kernel<H3D_PIXEL_I420>;
+        case H3D_PIXEL_YUYV: return (const void*)resize_frames_rig_kernel<H3D_PIXEL_YUYV>;
+        default: return (const void*)resize_frames_rig_kernel<H3D_PIXEL_RGB>;
+    }
+}
+
+}  // namespace
+
+// include/hand3d_b200.h's rig table and coefficient buffer; the caller has checked the formats and sizes.  Each distinct (H, W) gets
+// its coefficients once, from the same host code (and the same -ffp-contract=off) as a single-size plan.
+void frame_rig_layout(int B, const int* fmt, const int* hw, int h, int w, std::vector<int32_t>& table, std::vector<int32_t>& coef) {
+    constexpr int SW = H3D_FRAME_RIG_SLOT_WORDS, LW = H3D_FRAME_RIG_LAUNCH_WORDS;
+    table.assign((size_t)B * SW + B + (H3D_PIXEL_YUYV + 1) * LW, 0);
+    coef.assign(256, 0);
+    for (int u = 0; u < 256; ++u) {
+        const float f = (float)((double)u / 255.0 - 0.5);
+        memcpy(&coef[u], &f, 4);
+    }
+    std::vector<std::array<int, 8>> sizes;   // H, W, then the offsets of xb, kx, yb, ky and kxs, kys
+    for (int b = 0; b < B; ++b) {
+        const int H = hw[2 * b], W = hw[2 * b + 1];
+        int si = 0;
+        while (si < (int)sizes.size() && (sizes[si][0] != H || sizes[si][1] != W)) ++si;
+        if (si == (int)sizes.size()) {
+            std::vector<int32_t> xb, kx, yb, ky;
+            std::array<int, 8> z{H, W, 0, 0, 0, 0, 0, 0};
+            z[6] = pil_bilinear_coeffs(W, w, xb, kx);
+            z[7] = pil_bilinear_coeffs(H, h, yb, ky);
+            for (int t = 0; t < 4; ++t) {
+                const std::vector<int32_t>& v = t == 0 ? xb : t == 1 ? kx : t == 2 ? yb : ky;
+                z[2 + t] = (int)coef.size();
+                coef.insert(coef.end(), v.begin(), v.end());
+            }
+            sizes.push_back(z);
+        }
+        FramePlan g;
+        g.fmt = fmt[b]; g.Hf = H; g.Wf = W; g.h = h; g.w = w; g.kxs = sizes[si][6]; g.kys = sizes[si][7];
+        frame_geometry(g);
+        int32_t* e = &table[(size_t)b * SW];
+        e[H3D_RIG_FORMAT] = g.fmt; e[H3D_RIG_H] = H; e[H3D_RIG_W] = W; e[H3D_RIG_KXS] = g.kxs; e[H3D_RIG_KYS] = g.kys;
+        e[H3D_RIG_BAND] = g.band; e[H3D_RIG_CHUNK] = g.chunk; e[H3D_RIG_ROW_STRIDE] = g.row_stride; e[H3D_RIG_NBANDS] = g.nbands;
+        e[H3D_RIG_ACC_BYTES] = g.acc_bytes; e[H3D_RIG_INTER_BYTES] = g.inter_bytes; e[H3D_RIG_SMEM] = g.smem;
+        for (int k = 0; k < 3; ++k) e[H3D_RIG_SEG_OFF + k] = g.seg_off[k];
+        e[H3D_RIG_RGB_STRIDE] = g.rgb_stride;
+        for (int t = 0; t < 4; ++t) e[H3D_RIG_XB + t] = sizes[si][2 + t];
+        e[H3D_RIG_SIZE] = si;
+    }
+    int32_t* order = &table[(size_t)B * SW];
+    int32_t* launch = order + B;
+    int pos = 0;
+    for (int f = 0; f <= H3D_PIXEL_YUYV; ++f) {
+        int32_t* l = launch + f * LW;
+        l[H3D_RIG_LAUNCH_FIRST] = pos;
+        for (int b = 0; b < B; ++b) {
+            int32_t* e = &table[(size_t)b * SW];
+            if (e[H3D_RIG_FORMAT] != f) continue;
+            order[pos++] = b;
+            e[H3D_RIG_CTA0] = l[H3D_RIG_LAUNCH_CTAS];
+            l[H3D_RIG_LAUNCH_SLOTS] += 1;
+            l[H3D_RIG_LAUNCH_CTAS] += e[H3D_RIG_NBANDS];
+            l[H3D_RIG_LAUNCH_SMEM] = std::max(l[H3D_RIG_LAUNCH_SMEM], e[H3D_RIG_SMEM]);
+        }
+    }
+}
+
+FrameRigPlan* frame_rig_plan_create(int B, const int* fmt, const int* hw, int h, int w, cudaStream_t s) {
+    auto* p = new FrameRigPlan();
+    p->B = B; p->h = h; p->w = w;
+    std::vector<int32_t> table, coef;
+    frame_rig_layout(B, fmt, hw, h, w, table, coef);
+    const int32_t* launch = &table[(size_t)B * H3D_FRAME_RIG_SLOT_WORDS + B];
+    memcpy(p->launch, launch, sizeof(p->launch));
+    p->host = table;
+    p->host.insert(p->host.end(), coef.begin(), coef.end());
+    cudaError_t e = cudaSuccess;
+    for (int f = 0; f <= H3D_PIXEL_YUYV && e == cudaSuccess; ++f) {   // raise-only, as frame_plan_create does
+        if (p->launch[f][H3D_RIG_LAUNCH_SLOTS] == 0) continue;
+        cudaFuncAttributes fa;
+        const void* kern = rig_kernel_of(f);
+        e = cudaFuncGetAttributes(&fa, kern);
+        if (e == cudaSuccess && fa.maxDynamicSharedSizeBytes < p->launch[f][H3D_RIG_LAUNCH_SMEM])
+            e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, p->launch[f][H3D_RIG_LAUNCH_SMEM]);
+    }
+    if (e == cudaSuccess) e = cudaMalloc(&p->dev, p->host.size() * 4);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(p->dev, p->host.data(), p->host.size() * 4, cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) {
+        cuda_fail(e, "frame_rig_plan_create", __FILE__, __LINE__);
+        frame_rig_plan_destroy(p);
+        return nullptr;
+    }
+    p->table = p->dev;
+    p->coef = p->dev + table.size();
+    return p;
+}
+
+void frame_rig_plan_destroy(FrameRigPlan* p) {
+    if (!p) return;
+    if (p->dev) cudaFree(p->dev);
+    delete p;
+}
+
+int launch_resize_frames_rig(const FrameRigPlan* p, const uint8_t* const* frames, int normalize, void* out, cudaStream_t s) {
+    RigArgs r;
+    r.table = p->table; r.coef = p->coef; r.out = out;
+    r.B = p->B; r.h = p->h; r.w = p->w; r.normalize = normalize;
+    for (int b = 0; b < H3D_FRAME_RIG_MAX_SLOTS; ++b) r.in[b] = b < p->B ? frames[b] : nullptr;
+    for (int f = 0; f <= H3D_PIXEL_YUYV; ++f) {
+        const int* l = p->launch[f];
+        if (l[H3D_RIG_LAUNCH_SLOTS] == 0) continue;
+        r.first = l[H3D_RIG_LAUNCH_FIRST]; r.nslots = l[H3D_RIG_LAUNCH_SLOTS];
+        const unsigned grid = (unsigned)l[H3D_RIG_LAUNCH_CTAS];
+        const int smem = l[H3D_RIG_LAUNCH_SMEM];
+        switch (f) {
+            case H3D_PIXEL_BGR: resize_frames_rig_kernel<H3D_PIXEL_BGR><<<grid, kFrameThreads, smem, s>>>(r); break;
+            case H3D_PIXEL_NV12: resize_frames_rig_kernel<H3D_PIXEL_NV12><<<grid, kFrameThreads, smem, s>>>(r); break;
+            case H3D_PIXEL_I420: resize_frames_rig_kernel<H3D_PIXEL_I420><<<grid, kFrameThreads, smem, s>>>(r); break;
+            case H3D_PIXEL_YUYV: resize_frames_rig_kernel<H3D_PIXEL_YUYV><<<grid, kFrameThreads, smem, s>>>(r); break;
+            default: resize_frames_rig_kernel<H3D_PIXEL_RGB><<<grid, kFrameThreads, smem, s>>>(r); break;
+        }
+        H3D_CHECK_LAUNCH();
+    }
     return H3D_OK;
 }
 

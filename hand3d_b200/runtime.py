@@ -687,6 +687,59 @@ class Context:
                                                   int(bool(normalize)), _ptr(out), _stream()), "h3d_resize_frames_fmt")
         return out
 
+    def _rig_args(self, B, pixel_formats, frame_hw, out_h, out_w):
+        if len(pixel_formats) != B or len(frame_hw) != B:
+            raise ValueError("a rig of %d slots needs %d pixel formats and %d sizes, got %d and %d" % (B, B, B, len(pixel_formats), len(frame_hw)))
+        for b, f in enumerate(pixel_formats):
+            if f not in _lib.PIXEL_FORMATS:
+                raise ValueError("slot %d: pixel_format must be one of %s, got %r" % (b, sorted(_lib.PIXEL_FORMATS), f))
+        fmts = (C.c_int * B)(*[_lib.PIXEL_FORMATS[f] for f in pixel_formats])
+        hw = (C.c_int * (2 * B))(*[int(v) for s in frame_hw for v in s])
+        return fmts, hw
+
+    def frame_rig_plan(self, pixel_formats, frame_hw, out_h, out_w):
+        """h3d_frame_rig_plan: builds the plan of a rig (slot b in pixel_formats[b] at frame_hw[b]) for resize_frames_rig, outside
+        graph capture, so that a later captured call only enqueues."""
+        B = len(frame_hw)
+        fmts, hw = self._rig_args(B, pixel_formats, frame_hw, out_h, out_w)
+        _lib.check(self.lib.h3d_frame_rig_plan(self.h, B, fmts, hw, int(out_h), int(out_w), _stream()), "h3d_frame_rig_plan")
+
+    def resize_frames_rig(self, frames, out_h, out_w, normalize, out=None, pixel_formats=None):
+        """resize_frames for a camera rig: frames is a list of B CUDA uint8 frames, one per slot, each of its own size and pixel format
+        (pixel_formats[b], "rgb" when None; one frame of frame_shape(fmt, H, W), with or without a leading 1) -> [B,out_h,out_w,3], slot b
+        bit for bit resize_frames of frame b alone.  One kernel per pixel format present; the first call of a new rig builds its plan
+        (not under graph capture)."""
+        B = len(frames)
+        pixel_formats = ["rgb"] * B if pixel_formats is None else list(pixel_formats)
+        if len(pixel_formats) != B:
+            raise ValueError("a rig of %d frames needs %d pixel formats, got %d" % (B, B, len(pixel_formats)))
+        hw, dev = [], None
+        for b, (f, fmt) in enumerate(zip(frames, pixel_formats)):
+            if fmt not in _lib.PIXEL_FORMATS:
+                raise ValueError("slot %d: pixel_format must be one of %s, got %r" % (b, sorted(_lib.PIXEL_FORMATS), fmt))
+            if isinstance(f, torch.Tensor) and f.dim() == len(frame_shape(fmt, 2, 2)):
+                f = f.unsqueeze(0)
+            try:
+                n, H, W = _frames_bhw(f, fmt)
+            except (TypeError, ValueError, RuntimeError) as e:
+                raise type(e)("slot %d: %s" % (b, e)) from None
+            if n != 1:
+                raise ValueError("slot %d: one frame per slot, got a batch of %d" % (b, n))
+            if dev is not None and f.device != dev:
+                raise ValueError("slot %d: the frames must be on one device" % b)
+            dev = f.device
+            hw.append((H, W))
+        fmts, hwa = self._rig_args(B, pixel_formats, hw, out_h, out_w)
+        dt = torch.float32 if normalize else torch.uint8
+        if out is None:
+            out = torch.empty((B, int(out_h), int(out_w), 3), dtype=dt, device=dev)
+        elif out.dtype != dt or tuple(out.shape) != (B, int(out_h), int(out_w), 3) or not out.is_contiguous() or out.device != dev:
+            raise ValueError("out must be a contiguous %s tensor [%d,%d,%d,3] on the frames' device" % (dt, B, out_h, out_w))
+        ptrs = (C.c_void_p * B)(*[f.data_ptr() for f in frames])
+        _lib.check(self.lib.h3d_resize_frames_rig(self.h, ptrs, B, fmts, hwa, int(out_h), int(out_w), int(bool(normalize)), _ptr(out),
+                                                  _stream()), "h3d_resize_frames_rig")
+        return out
+
     def convert_frames(self, frames, pixel_format, out=None):
         """h3d_convert_frames: frames uint8 CUDA in pixel_format's layout -> uint8 RGB [B,H,W,3] at full size (OpenCV's cvtColor
         rule).  With `out` (contiguous uint8 [B,H,W,3]) it writes there and allocates nothing, so it can be captured."""

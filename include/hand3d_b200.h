@@ -485,6 +485,8 @@ H3D_API int h3d_resize_frames_fmt(h3d_ctx* ctx, const uint8_t* frames, int forma
 /* frames in `format` -> out_rgb [B,H,W,3] uint8 RGB at full size, by the rule above (RGB: a copy; BGR: the channels reversed).  Sizes
  * per the table above, else H3D_EINVAL before anything is enqueued.  Enqueues one kernel and allocates nothing (capturable). */
 H3D_API int h3d_convert_frames(h3d_ctx* ctx, const uint8_t* frames, int format, int B, int H, int W, uint8_t* out_rgb, void* stream);
+/* Camera rigs (a size and a pixel format per batch slot): include/hand3d_b200_rig.h. */
+#include "hand3d_b200_rig.h"
 /* tf.image.random_hue (TF 1.3 adjust_hue, non-fused: rgb_to_hsv, h = mod(h + (delta + 1), 1), hsv_to_rgb, in the functors' fp32 order)
  * and / or the random_crop window, in one pass.  image [B,H,W,3] fp32, hand_parts [B,H,W] u8, params as above (delta at
  * H3D_AUG_HUE_DELTA when flags has H3D_AUG_HUE, window at H3D_AUG_WINDOW when flags has H3D_AUG_RANDOM_CROP) -> out_image [B,h,w,3]
