@@ -89,8 +89,12 @@ static const std::map<std::string, VarShape>& known_vars() {
 
 // ------------------------------------------------------------------------------------------ context
 struct HostTensor { std::vector<float> data; std::vector<int64_t> shape; };
-// w_scale: fp16 planes with passes 1 / 3, the per-channel shift factors 2^-s (split_fmt.cuh), stored after the padded bias
-struct PackedW { Split w; float* bias = nullptr; float* w_scale = nullptr; int Cin_pad = 0, Cout_pad = 0; float corr_scale = 0.f; };
+// w_scale: fp16 planes with passes 1 / 3, the per-channel shift factors 2^-s (split_fmt.cuh), stored after the padded bias.
+// passes / half: the format of the planes, which the activation planes of a layer using them share.
+struct PackedW {
+    Split w; float* bias = nullptr; float* w_scale = nullptr; int Cin_pad = 0, Cout_pad = 0; float corr_scale = 0.f;
+    int passes = 0; Half16 half = Half16::BF16;
+};
 
 struct Arena {   // bump allocator over the caller-owned workspace (base == nullptr -> size query)
     char* base = nullptr; int64_t off = 0;
@@ -288,7 +292,7 @@ static int pack_conv_weights(const float* w, const float* bias, int k, int Cin, 
     H3D_CUDA(cudaMalloc(&out->bias, bv.size() * 4));
     H3D_CUDA(cudaMemcpy(out->bias, bv.data(), bv.size() * 4, cudaMemcpyHostToDevice));
     if (shifted) out->w_scale = out->bias + Cout_pad;
-    out->Cin_pad = Cin_pad; out->Cout_pad = Cout_pad;
+    out->Cin_pad = Cin_pad; out->Cout_pad = Cout_pad; out->passes = passes; out->half = t;
     return H3D_OK;
 }
 
@@ -446,21 +450,33 @@ static Act slot_view(char* p, int64_t elems, int C, bool split, int passes) {
     return a;
 }
 
-static int add_direct(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, const LayerSpec& l, int B, int H, int W,
-                      const float* x /*null -> Ext.in*/, int Cin_total, int cin_off, float* y, int Cout_total, int cout_off,
-                      Split ys, int Cs_total, int cs_off, float* splitk_scratch = nullptr) {
-    const float *w, *b;
-    int rc;
-    if ((rc = dev_weight(ctx, scope + "/" + l.name + "/weights", &w))) return rc;
-    if ((rc = dev_weight(ctx, scope + "/" + l.name + "/biases", &b))) return rc;
+// The CUDA-core convolution of layer l (k, stride, cin, cout, leaky) with HWIO fp32 weights w / b: input channels
+// [cin_off, cin_off + l.cin) of x, output at channel offsets of fp32 y and / or of the planes ys in format half.
+static DirectConvArgs direct_args(const LayerSpec& l, const float* w, const float* b, Half16 half, int B, int H, int W, const float* x,
+                                  int Cin_total, int cin_off, float* y, int Cout_total, int cout_off, Split ys, int Cs_total, int cs_off,
+                                  float* splitk_scratch, int64_t splitk_scratch_floats, int* err_flag, const int* count = nullptr,
+                                  const int* slots = nullptr) {
     DirectConvArgs a;
     a.x = x; a.Cin_total = Cin_total; a.cin_off = cin_off; a.w = w; a.bias = b; a.y = y; a.Cout_total = Cout_total; a.cout_off = cout_off;
-    a.ys = ys; a.Cs_total = Cs_total; a.cs_off = cs_off; a.half = half_of(ctx->precision);
+    a.ys = ys; a.Cs_total = Cs_total; a.cs_off = cs_off; a.half = half;
     a.B = B; a.H = H; a.W = W; a.Cin = l.cin; a.Cout = l.cout; a.k = l.k; a.stride = l.stride; a.leaky = l.leaky;
-    a.splitk_scratch = splitk_scratch; a.splitk_scratch_floats = splitk_scratch ? kConvSplitKScratchFloats : 0;
-    a.err_flag = ctx->err_flag;
-    a.count = pl->count;
-    a.slots = x ? nullptr : pl->slots;   // the plan's external input is indexed through the slot list
+    a.splitk_scratch = splitk_scratch; a.splitk_scratch_floats = splitk_scratch_floats;
+    a.err_flag = err_flag;
+    a.count = count;
+    a.slots = slots;
+    return a;
+}
+
+// An operator entry's one-step plan (add_tc / add_direct), run outside run_plan: only stage plans are profiled
+static int run_step(const StagePlan& pl, cudaStream_t s) { return pl.steps.front().fn(Ext(), s); }
+
+// One CUDA-core convolution layer as a plan step, with the weights w / b given
+static int add_direct(h3d_ctx* ctx, StagePlan* pl, const LayerSpec& l, const float* w, const float* b, Half16 half, int B, int H, int W,
+                      const float* x /*null -> Ext.in*/, int Cin_total, int cin_off, float* y, int Cout_total, int cout_off,
+                      Split ys, int Cs_total, int cs_off, float* splitk_scratch = nullptr) {
+    const DirectConvArgs a = direct_args(l, w, b, half, B, H, W, x, Cin_total, cin_off, y, Cout_total, cout_off, ys, Cs_total, cs_off,
+                                         splitk_scratch, splitk_scratch ? kConvSplitKScratchFloats : 0, ctx->err_flag, pl->count,
+                                         x ? nullptr : pl->slots);   // the plan's external input is indexed through the slot list
     Step& st = pl->add([a](const Ext& e, cudaStream_t s) {
         DirectConvArgs aa = a;
         if (!aa.x) aa.x = e.in;
@@ -472,22 +488,31 @@ static int add_direct(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, con
     return H3D_OK;
 }
 
-static int add_tc(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, const LayerSpec& l, int B, int H, int W, Split x,
-                  int Cin_total, int Cin_pad, const std::vector<int>& perm, Split y, int Cy_total, int cy_off, float* yf,
-                  int Cyf_total, int cyf_off, int pool = 0, int force_passes = 0) {
-    const PackedW* pw;
-    int rc = get_packed(ctx, scope, l, Cin_pad, perm, &pw, force_passes);
-    if (rc) return rc;
+// add_direct with the loaded weights of scope/l.name, in the context's precision
+static int add_direct(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, const LayerSpec& l, int B, int H, int W,
+                      const float* x /*null -> Ext.in*/, int Cin_total, int cin_off, float* y, int Cout_total, int cout_off,
+                      Split ys, int Cs_total, int cs_off, float* splitk_scratch = nullptr) {
+    const float *w, *b;
+    int rc;
+    if ((rc = dev_weight(ctx, scope + "/" + l.name + "/weights", &w))) return rc;
+    if ((rc = dev_weight(ctx, scope + "/" + l.name + "/biases", &b))) return rc;
+    return add_direct(ctx, pl, l, w, b, half_of(ctx->precision), B, H, W, x, Cin_total, cin_off, y, Cout_total, cout_off, ys, Cs_total,
+                      cs_off, splitk_scratch);
+}
+
+// One tensor-core convolution layer as a plan step, with the packed weights pw (whose format the activation planes share)
+static int add_tc(h3d_ctx* ctx, StagePlan* pl, const LayerSpec& l, const PackedW& pw, int B, int H, int W, Split x, int Cin_total,
+                  Split y, int Cy_total, int cy_off, float* yf, int Cyf_total, int cyf_off, int pool = 0) {
     TcConvDesc d;
-    d.x = x; d.Cin_total = Cin_total; d.Cin_pad = Cin_pad; d.w = pw->w; d.bias = pw->bias; d.w_scale = pw->w_scale; d.Cout = l.cout;
-    d.Cout_pad = pw->Cout_pad;
+    d.x = x; d.Cin_total = Cin_total; d.Cin_pad = pw.Cin_pad; d.w = pw.w; d.bias = pw.bias; d.w_scale = pw.w_scale; d.Cout = l.cout;
+    d.Cout_pad = pw.Cout_pad;
     d.y = y; d.Cy_total = Cy_total; d.cy_off = cy_off; d.yf = yf; d.Cyf_total = Cyf_total; d.cyf_off = cyf_off;
-    d.B = B; d.H = H; d.W = W; d.k = l.k; d.leaky = l.leaky; d.passes = force_passes ? force_passes : passes_of(ctx->precision);
-    d.half = half_of(ctx->precision);
-    d.corr_scale = pw->corr_scale;
+    d.B = B; d.H = H; d.W = W; d.k = l.k; d.leaky = l.leaky; d.passes = pw.passes; d.half = pw.half;
+    d.corr_scale = pw.corr_scale;
     d.pool = pool;
     d.err_flag = ctx->err_flag;
     d.count = pl->count;
+    int rc;
     TcConvPlan* tp = tc_conv_plan_create(d, &rc);
     if (!tp) return rc;
     pl->tc.push_back(tp);
@@ -496,6 +521,16 @@ static int add_tc(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, const L
     pl->flops += fl;
     st.kind = KIND_TC; st.flops = fl;
     return H3D_OK;
+}
+
+// add_tc with the loaded weights of scope/l.name, packed for the context's precision (or force_passes) with Cin_pad input channels
+static int add_tc(h3d_ctx* ctx, StagePlan* pl, const std::string& scope, const LayerSpec& l, int B, int H, int W, Split x,
+                  int Cin_total, int Cin_pad, const std::vector<int>& perm, Split y, int Cy_total, int cy_off, float* yf,
+                  int Cyf_total, int cyf_off, int pool = 0, int force_passes = 0) {
+    const PackedW* pw;
+    int rc = get_packed(ctx, scope, l, Cin_pad, perm, &pw, force_passes);
+    if (rc) return rc;
+    return add_tc(ctx, pl, l, *pw, B, H, W, x, Cin_total, y, Cy_total, cy_off, yf, Cyf_total, cyf_off, pool);
 }
 
 // VGG-style trunk shared by HandSegNet and PoseNet2D: conv layers [0, n) of `layers` with 2x2 pools after
@@ -682,6 +717,9 @@ static int add_fc(h3d_ctx* ctx, StagePlan* pl, const std::string& name, const fl
     return H3D_OK;
 }
 
+// One FC layer of the lifting stage; with dropout on (h3d_set_dropout), dropout layer drop_layer follows it (none when < 0)
+struct LiftFc { const char* name; int in, out, leaky, drop_layer; float keep_prob; };
+
 // PosePrior (+ ViewpointNet for the 'proposed' variant): two 6-layer stride-1 / stride-2 conv pyramids on the 32x32 score map
 // and their FC stacks.  With a 3-pass tensor-core precision the pyramids run on the wgmma kernel (stride 2 = odd pixels of
 // the stride-1 result, Cin / Cout padded to 64 with zero channels); otherwise on the fp32 CUDA-core kernel.  The two networks
@@ -696,20 +734,37 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
     const Half16 half = half_of(ctx->precision);
     const bool tc_lift = is_tc(ctx->precision) && passes_of(ctx->precision) != 4 && !tc_tuning().lift_direct;
     const bool drop = ctx->drop_on;
+    // FC stacks + Rodrigues / flip / rotate as ONE kernel (fc_chain_kernel) after both pyramids and their concats; tune.fc_chain = 0
+    // and dropout take one launch per layer
+    const bool use_chain = tc_lift && tc_tuning().fc_chain != 0 && !drop;
+    const bool bott = variant == H3D_VARIANT_BOTTLENECK, proposed = variant == H3D_VARIANT_PROPOSED;
     const int64_t slot_bytes = align_up((int64_t)B * 32 * 32 * 64 * 4, 1024);
     char* slot_in = a.alloc<char>(slot_bytes);
     const int64_t fcs_floats = lift_fc_scratch_floats(B);
-    struct Branch { char* slot[2]; float *xcat, *t1, *t2, *t3, *fcs, *cvs; } br[2];
+    struct Branch { char* slot[2]; float *xcat, *t[3], *fcs, *cvs; } br[2];   // [0] PosePrior, [1] ViewpointNet
     for (auto& b : br) {
         b.slot[0] = a.alloc<char>(slot_bytes); b.slot[1] = a.alloc<char>(slot_bytes);
         b.xcat = a.alloc<float>((int64_t)B * 4100);
-        b.t1 = a.alloc<float>((int64_t)B * 512); b.t2 = a.alloc<float>((int64_t)B * 512); b.t3 = a.alloc<float>((int64_t)B * 64);
+        b.t[0] = a.alloc<float>((int64_t)B * 512); b.t[1] = a.alloc<float>((int64_t)B * 512); b.t[2] = a.alloc<float>((int64_t)B * 64);
         b.fcs = a.alloc<float>(fcs_floats);
         b.cvs = a.alloc<float>(kConvSplitKScratchFloats);
     }
     float* can = a.alloc<float>((int64_t)B * 63);
     float* uxyz = a.alloc<float>((int64_t)B * 4);
     H3D_REQUIRE(ctx->lay.lift_off + a.off <= ctx->lay.total, "lifting workspace region too small (internal error)");
+    auto xyz = ctx->host_w.find("PosePrior/fc_xyz/weights");
+    if (xyz == ctx->host_w.end()) { set_error("weights PosePrior/fc_xyz not loaded"); return H3D_EWEIGHTS; }
+    const int xyz_in = (int)xyz->second.shape[0];
+    if (bott) H3D_REQUIRE(xyz_in == 30, "bottleneck variant needs PosePrior/fc_xyz/weights of shape [30,63]");
+    else H3D_REQUIRE(xyz_in == 512, "PosePrior/fc_xyz/weights must have shape [512,63] for this variant");
+    // the FC stacks: PosePrior (nets/ColorHandPose3DNetwork.py:249-272; bottleneck nets/PosePriorNetwork.py:113-116) and ViewpointNet
+    // (:274-309), with the reference's dropout after the hidden layers
+    std::vector<LiftFc> pp_fc = {{"fc_rel0", 2050, 512, 1, H3D_DROPOUT_LAYER_FC_REL0, 0.8f}, {"fc_rel1", 512, 512, 1, H3D_DROPOUT_LAYER_FC_REL1, 0.8f}};
+    if (bott) pp_fc.push_back({"fc_bottleneck", 512, 30, 0, -1, 0.f});
+    pp_fc.push_back({"fc_xyz", xyz_in, 63, 0, -1, 0.f});
+    std::vector<LiftFc> vp_fc = {{"fc_vp0", 4098, 256, 1, H3D_DROPOUT_LAYER_FC_VP0, 0.75f}, {"fc_vp1", 256, 128, 1, H3D_DROPOUT_LAYER_FC_VP1, 0.75f}};
+    // the heads ux | uy | uz (:303-308) as one 128 -> 3 layer: the chain's last, on the other routes a CUDA-core FC step on fp32 t[1]
+    if (use_chain) vp_fc.push_back({"fc_vp_heads", 128, 3, 0, -1, 0.f});
     int rc;
     Act xin;   // tensor-core path: the 21-channel score map as split planes with 64 channels (43 zero)
     if (tc_lift) {
@@ -749,11 +804,6 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
         }
         return H3D_OK;
     };
-    // ---- PosePrior on the caller's stream (nets/ColorHandPose3DNetwork.py:249-272; bottleneck nets/PosePriorNetwork.py:113-116)
-    const bool bott = variant == H3D_VARIANT_BOTTLENECK;
-    auto xyz = ctx->host_w.find("PosePrior/fc_xyz/weights");
-    if (xyz == ctx->host_w.end()) { set_error("weights PosePrior/fc_xyz not loaded"); return H3D_EWEIGHTS; }
-    const int xyz_in = (int)xyz->second.shape[0];
     // FC layers on the tensor-core kernel: a fully connected layer is a 1x1 convolution over B "images" of 1x1 pixels (tile =
     // 128 batch rows, K = in_features padded to 64, weights [in,out] = HWIO [1,1,in,out]); activations stay split planes
     struct Planes { Split s; int stride; };
@@ -763,11 +813,6 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
         pz.s.hi = (uint16_t*)cur; pz.s.lo = (uint16_t*)(cur + bytes);
         cur += 2 * bytes;
         return pz;
-    };
-    auto fc_tc = [&](const std::string& scope, const char* name, int in_f, int out_f, int leaky, const Planes& x, const Planes* y, float* yf) -> int {
-        LayerSpec l{name, 1, 1, in_f, out_f, leaky};
-        return add_tc(ctx, pl.get(), scope, l, B, 1, 1, x.s, x.stride, (int)align_up(in_f, 64), {}, y ? y->s : Split(), y ? y->stride : 0, 0, yf,
-                      out_f, 0, 0, passes);
     };
     // dropout after a hidden FC layer: fp32 x [B, cols] in place, or (y != nullptr) into the next tensor-core layer's planes.  The seed is
     // read when the step is enqueued, the draw on the device.
@@ -781,167 +826,96 @@ static int build_lifting(h3d_ctx* ctx, int B, int variant) {
             return launch_dropout(x, B, cols, keep_prob, layer, cx->drop_seed, draw, yf, nullptr, ys, stride, half, s);
         });
     };
-    // the tensor-core hidden layer: straight into the next layer's planes, or with dropout through fp32 t
-    auto fc_tc_hidden = [&](const std::string& scope, const char* name, int in_f, int out_f, const Planes& x, const Planes& y, float* t,
-                            float keep_prob, int layer) -> int {
-        if (!drop) return fc_tc(scope, name, in_f, out_f, 1, x, &y, nullptr);
-        int rc2 = fc_tc(scope, name, in_f, out_f, 1, x, nullptr, t);
-        if (!rc2) add_dropout(t, out_f, keep_prob, layer, &y);
-        return rc2;
-    };
-    // ---- FC stacks + Rodrigues / flip / rotate as ONE kernel (fc_chain_kernel): both pyramids first (ViewpointNet on the side
-    //      stream), their concat kernels, one join, one launch.  tune.fc_chain = 0 keeps the layer-by-layer path below.
-    const bool use_chain = tc_lift && tc_tuning().fc_chain != 0 && !drop;
-    if (use_chain) {
-        if (bott) H3D_REQUIRE(xyz_in == 30, "bottleneck variant needs PosePrior/fc_xyz/weights of shape [30,63]");
-        else H3D_REQUIRE(xyz_in == 512, "PosePrior/fc_xyz/weights must have shape [512,63] for this variant");
-        FcChainDesc chains[2];
-        int64_t fl = 0;
-        auto fc_layer = [&](FcChainDesc& cd, const std::string& scope, const char* name, int in_f, int out_f, int leaky, const Planes& x, const Planes* y,
-                            float* yf, int yf_stride) -> int {
-            LayerSpec l{name, 1, 1, in_f, out_f, leaky};
-            const PackedW* pw;
-            int rc2 = get_packed(ctx, scope, l, (int)align_up(in_f, 64), {}, &pw, passes);
-            if (rc2) return rc2;
-            FcLayerDesc& d = cd.layer[cd.num_layers++];
-            d.x = x.s; d.x_stride = x.stride; d.in_features = in_f;
-            d.w = pw->w; d.bias = pw->bias; d.w_scale = pw->w_scale; d.out_features = out_f; d.out_pad = pw->Cout_pad;
-            d.y = y ? y->s : Split(); d.y_stride = y ? y->stride : 0; d.yf = yf; d.yf_stride = yf_stride; d.leaky = leaky;
-            fl += 2ll * B * in_f * out_f;
-            return H3D_OK;
-        };
-        const bool proposed = variant == H3D_VARIANT_PROPOSED;
-        if (proposed) {
-            if ((rc = ensure_vp_heads(ctx))) return rc;
-            const Branch& b = br[1];
-            float* feat = nullptr;
-            pl->cur_lane = 1;
-            if ((rc = pyramid("ViewpointNet", kViewpoint, b, &feat))) return rc;
-            char* cur = b.slot[0];
-            const Planes xp = carve_planes(cur, 4098), p1 = carve_planes(cur, 256), p2 = carve_planes(cur, 128);
-            pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 4096, xp.stride, half, s); });
-            pl->cur_lane = 0;
-            if ((rc = fc_layer(chains[1], "ViewpointNet", "fc_vp0", 4098, 256, 1, xp, &p1, nullptr, 0))) return rc;
-            if ((rc = fc_layer(chains[1], "ViewpointNet", "fc_vp1", 256, 128, 1, p1, &p2, nullptr, 0))) return rc;
-            if ((rc = fc_layer(chains[1], "ViewpointNet", "fc_vp_heads", 128, 3, 0, p2, nullptr, uxyz, 3))) return rc;    // ux | uy | uz (:303-308)
-        }
-        {
-            const Branch& b = br[0];
-            float* feat = nullptr;
-            if ((rc = pyramid("PosePrior", kPosePrior, b, &feat))) return rc;
-            char* cur = b.slot[0];
-            const Planes xp = carve_planes(cur, 2050), p1 = carve_planes(cur, 512), p2 = carve_planes(cur, 512), p3 = carve_planes(cur, 64);
-            pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 2048, xp.stride, half, s); });
-            if ((rc = fc_layer(chains[0], "PosePrior", "fc_rel0", 2050, 512, 1, xp, &p1, nullptr, 0))) return rc;
-            if ((rc = fc_layer(chains[0], "PosePrior", "fc_rel1", 512, 512, 1, p1, &p2, nullptr, 0))) return rc;
-            if (bott) {
-                if ((rc = fc_layer(chains[0], "PosePrior", "fc_bottleneck", 512, 30, 0, p2, &p3, nullptr, 0))) return rc;
-                if ((rc = fc_layer(chains[0], "PosePrior", "fc_xyz", 30, 63, 0, p3, nullptr, can, 63))) return rc;
-            } else {
-                if ((rc = fc_layer(chains[0], "PosePrior", "fc_xyz", 512, 63, 0, p2, nullptr, can, 63))) return rc;
+    FcChainDesc chains[2];   // as br
+    int64_t chain_flops = 0;
+    // One branch: its conv pyramid, the concat with hand_side and the FC stack fc, whose last layer writes fp32 out (nullptr: t[n - 1])
+    auto branch = [&](const char* scope, const LayerSpec* convs, const std::vector<LiftFc>& fc, const Branch& b, FcChainDesc& chain,
+                      float* out) -> int {
+        float* feat = nullptr;
+        int rc2;
+        if ((rc2 = pyramid(scope, convs, b, &feat))) return rc2;
+        const int n = (int)fc.size(), feat_n = fc[0].in - 2;
+        if (!tc_lift) {   // CUDA-core layers xcat -> t[0] -> t[1] ..., dropout in place
+            float* xcat = b.xcat;
+            pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside(feat, e.hand_side, xcat, B, feat_n, s); });
+            const float* x = xcat;
+            for (int i = 0; i < n; ++i) {
+                const LiftFc& f = fc[i];
+                float* y = i == n - 1 && out ? out : b.t[i];
+                if ((rc2 = add_fc(ctx, pl.get(), std::string(scope) + "/" + f.name, x, y, b.fcs, fcs_floats, B, f.in, f.out, f.leaky))) return rc2;
+                if (drop && f.drop_layer >= 0) add_dropout(y, f.out, f.keep_prob, f.drop_layer, nullptr);
+                x = y;
             }
+            return H3D_OK;
         }
+        // tensor-core layers on planes carved from slot[0] (the layer-4 output, dead by now): p[0] the concat, p[i + 1] hidden layer i's output
+        char* cur = b.slot[0];
+        std::vector<Planes> p{carve_planes(cur, fc[0].in)};
+        for (int i = 0; i + 1 < n; ++i) p.push_back(carve_planes(cur, fc[i].out));
+        const Planes xp = p[0];
+        pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, feat_n, xp.stride, half, s); });
+        for (int i = 0; i < n; ++i) {
+            const LiftFc& f = fc[i];
+            const LayerSpec l{f.name, 1, 1, f.in, f.out, f.leaky};
+            const bool last = i == n - 1, dropout = drop && f.drop_layer >= 0;
+            // the last layer writes fp32; a hidden one the next layer's planes, or with dropout fp32 t[i], which the dropout splits into them
+            const Planes* y = last || dropout ? nullptr : &p[i + 1];
+            float* yf = nullptr;
+            if (last) yf = out ? out : b.t[i];
+            else if (dropout) yf = b.t[i];
+            const PackedW* pw;
+            if ((rc2 = get_packed(ctx, scope, l, (int)align_up(f.in, 64), {}, &pw, passes))) return rc2;
+            if (use_chain) {
+                FcLayerDesc& d = chain.layer[chain.num_layers++];
+                d.x = p[i].s; d.x_stride = p[i].stride; d.in_features = f.in;
+                d.w = pw->w; d.bias = pw->bias; d.w_scale = pw->w_scale; d.out_features = f.out; d.out_pad = pw->Cout_pad;
+                d.y = y ? y->s : Split(); d.y_stride = y ? y->stride : 0; d.yf = yf; d.yf_stride = yf ? f.out : 0; d.leaky = f.leaky;
+                chain_flops += 2ll * B * f.in * f.out;
+                continue;
+            }
+            if ((rc2 = add_tc(ctx, pl.get(), l, *pw, B, 1, 1, p[i].s, p[i].stride, y ? y->s : Split(), y ? y->stride : 0, 0, yf, f.out, 0)))
+                return rc2;
+            if (dropout) add_dropout(yf, f.out, f.keep_prob, f.drop_layer, last ? nullptr : &p[i + 1]);
+        }
+        return H3D_OK;
+    };
+    if (proposed) {
+        // ViewpointNet on the side stream, enqueued first so that both branches are in flight while the host builds the second one
+        if ((rc = ensure_vp_heads(ctx))) return rc;
+        pl->cur_lane = 1;
+        if ((rc = branch("ViewpointNet", kViewpoint, vp_fc, br[1], chains[1], use_chain ? uxyz : nullptr))) return rc;
+        if (!use_chain) {
+            const float* hw = ctx->vp_head_w; const float* hb = ctx->vp_head_b;
+            float* vp1 = br[1].t[1]; float* fcs = br[1].fcs;
+            Step& st = pl->add([=](const Ext&, cudaStream_t s) { return launch_fc(vp1, hw, hb, uxyz, fcs, fcs_floats, B, 128, 3, 0, 128, s); });
+            st.kind = KIND_FC; st.flops = 2ll * B * 128 * 3;
+        }
+        pl->cur_lane = 0;
+    }
+    if ((rc = branch("PosePrior", kPosePrior, pp_fc, br[0], chains[0], can))) return rc;
+    // the outputs taken from can: 'local' assembles xyz from its bone-relative coordinates by forward kinematics
+    // (nets/PosePriorNetwork.py:70-75), 'proposed' leaves out to the rotation, the other variants copy can; out2 (optional) gets can
+    auto tail = [=](const Ext& e, cudaStream_t s) -> int {
+        if (variant != H3D_VARIANT_LOCAL && !proposed) H3D_CUDA(cudaMemcpyAsync(e.out, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
+        if (e.out2) H3D_CUDA(cudaMemcpyAsync(e.out2, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
+        return variant == H3D_VARIANT_LOCAL ? launch_bone_rel_trafo_inv(can, e.out, B, s) : H3D_OK;
+    };
+    // Rodrigues / flip / rotate (nets/ColorHandPose3DNetwork.py:239-247,311-334) needs both branches: the last step joins ViewpointNet's
+    pl->join_next = true;
+    if (use_chain) {
         FcChainPlan* fp = fc_chain_plan_create(chains, proposed ? 2 : 1, B, half, can, uxyz, ctx->fc_counter, ctx->err_flag);
         if (!fp) return H3D_ECUDA;
         pl->fc.push_back(fp);
-        const int var = variant;
-        pl->join_next = true;                                 // joins the ViewpointNet branch before the launch
         Step& st = pl->add([=](const Ext& e, cudaStream_t s) {
-            int rc2 = fc_chain_launch(fp, e.hand_side, var == H3D_VARIANT_PROPOSED ? e.out3 : nullptr, var == H3D_VARIANT_PROPOSED ? e.out : nullptr, s);
-            if (rc2) return rc2;
-            if (var == H3D_VARIANT_LOCAL) {
-                if (e.out2) H3D_CUDA(cudaMemcpyAsync(e.out2, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
-                return launch_bone_rel_trafo_inv(can, e.out, B, s);     // nets/PosePriorNetwork.py:70-75
-            }
-            if (var != H3D_VARIANT_PROPOSED) H3D_CUDA(cudaMemcpyAsync(e.out, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
-            if (e.out2) H3D_CUDA(cudaMemcpyAsync(e.out2, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
-            return H3D_OK;
+            const int rc2 = fc_chain_launch(fp, e.hand_side, proposed ? e.out3 : nullptr, proposed ? e.out : nullptr, s);
+            return rc2 ? rc2 : tail(e, s);
         });
-        pl->flops += fl;
-        st.kind = KIND_TC; st.flops = fl;
-        ctx->lift = std::move(pl);
-        return H3D_OK;
-    }
-    auto pose_prior = [&]() -> int {
-        const Branch& b = br[0];
-        float* feat = nullptr;
-        int rc2;
-        if ((rc2 = pyramid("PosePrior", kPosePrior, b, &feat))) return rc2;
-        if (bott) H3D_REQUIRE(xyz_in == 30, "bottleneck variant needs PosePrior/fc_xyz/weights of shape [30,63]");
-        else H3D_REQUIRE(xyz_in == 512, "PosePrior/fc_xyz/weights must have shape [512,63] for this variant");
-        if (tc_lift) {   // slot[0] (layer-4 output, dead by now) holds the FC activations
-            char* cur = b.slot[0];
-            const Planes xp = carve_planes(cur, 2050), p1 = carve_planes(cur, 512), p2 = carve_planes(cur, 512), p3 = carve_planes(cur, 64);
-            pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 2048, xp.stride, half, s); });
-            if ((rc2 = fc_tc_hidden("PosePrior", "fc_rel0", 2050, 512, xp, p1, b.t1, 0.8f, H3D_DROPOUT_LAYER_FC_REL0))) return rc2;
-            if ((rc2 = fc_tc_hidden("PosePrior", "fc_rel1", 512, 512, p1, p2, b.t2, 0.8f, H3D_DROPOUT_LAYER_FC_REL1))) return rc2;
-            if (bott) {
-                if ((rc2 = fc_tc("PosePrior", "fc_bottleneck", 512, 30, 0, p2, &p3, nullptr))) return rc2;
-                return fc_tc("PosePrior", "fc_xyz", 30, 63, 0, p3, nullptr, can);
-            }
-            return fc_tc("PosePrior", "fc_xyz", 512, 63, 0, p2, nullptr, can);
-        }
-        float* xcat = b.xcat;
-        pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside(feat, e.hand_side, xcat, B, 2048, s); });
-        if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_rel0", b.xcat, b.t1, b.fcs, fcs_floats, B, 2050, 512, 1))) return rc2;
-        if (drop) add_dropout(b.t1, 512, 0.8f, H3D_DROPOUT_LAYER_FC_REL0, nullptr);
-        if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_rel1", b.t1, b.t2, b.fcs, fcs_floats, B, 512, 512, 1))) return rc2;
-        if (drop) add_dropout(b.t2, 512, 0.8f, H3D_DROPOUT_LAYER_FC_REL1, nullptr);
-        if (bott) {
-            if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_bottleneck", b.t2, b.t3, b.fcs, fcs_floats, B, 512, 30, 0))) return rc2;
-            if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_xyz", b.t3, can, b.fcs, fcs_floats, B, 30, 63, 0))) return rc2;
-        } else {
-            if ((rc2 = add_fc(ctx, pl.get(), "PosePrior/fc_xyz", b.t2, can, b.fcs, fcs_floats, B, 512, 63, 0))) return rc2;
-        }
-        return H3D_OK;
-    };
-    if (variant == H3D_VARIANT_PROPOSED) {
-        // ---- ViewpointNet on the side stream (nets/ColorHandPose3DNetwork.py:274-309), enqueued first so that both branches
-        //      are in flight while the host builds the second one
-        if ((rc = ensure_vp_heads(ctx))) return rc;
-        const Branch& b = br[1];
-        float* feat = nullptr;
-        pl->cur_lane = 1;
-        if ((rc = pyramid("ViewpointNet", kViewpoint, b, &feat))) return rc;
-        if (tc_lift) {
-            char* cur = b.slot[0];
-            const Planes xp = carve_planes(cur, 4098), p1 = carve_planes(cur, 256);
-            pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside_split(feat, e.hand_side, xp.s, B, 4096, xp.stride, half, s); });
-            if ((rc = fc_tc_hidden("ViewpointNet", "fc_vp0", 4098, 256, xp, p1, b.t1, 0.75f, H3D_DROPOUT_LAYER_FC_VP0))) return rc;
-            if ((rc = fc_tc("ViewpointNet", "fc_vp1", 256, 128, 1, p1, nullptr, b.t2))) return rc;   // fp32 [B,128] for the three 128 -> 1 heads
-        } else {
-            float* xcat = b.xcat;
-            pl->add([=](const Ext& e, cudaStream_t s) { return launch_concat_handside(feat, e.hand_side, xcat, B, 4096, s); });
-            if ((rc = add_fc(ctx, pl.get(), "ViewpointNet/fc_vp0", b.xcat, b.t1, b.fcs, fcs_floats, B, 4098, 256, 1))) return rc;
-            if (drop) add_dropout(b.t1, 256, 0.75f, H3D_DROPOUT_LAYER_FC_VP0, nullptr);
-            if ((rc = add_fc(ctx, pl.get(), "ViewpointNet/fc_vp1", b.t1, b.t2, b.fcs, fcs_floats, B, 256, 128, 1))) return rc;
-        }
-        if (drop) add_dropout(b.t2, 128, 0.75f, H3D_DROPOUT_LAYER_FC_VP1, nullptr);
-        const float* hw = ctx->vp_head_w; const float* hb = ctx->vp_head_b;
-        float* t2 = b.t2; float* fcs = b.fcs;
-        Step& st = pl->add([=](const Ext&, cudaStream_t s) { return launch_fc(t2, hw, hb, uxyz, fcs, fcs_floats, B, 128, 3, 0, 128, s); });
-        st.kind = KIND_FC; st.flops = 2ll * B * 128 * 3;
-        pl->cur_lane = 0;
-    }
-    if ((rc = pose_prior())) return rc;
-    if (variant == H3D_VARIANT_PROPOSED) {
-        // Rodrigues / flip / rotate (:239-247,311-334): needs both branches
-        pl->join_next = true;
-        pl->add([=](const Ext& e, cudaStream_t s) {
-            if (e.out2) H3D_CUDA(cudaMemcpyAsync(e.out2, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
-            return launch_rotate_canonical(can, uxyz, e.hand_side, B, e.out3, e.out, s);
-        });
-    } else if (variant == H3D_VARIANT_LOCAL) {
-        // nets/PosePriorNetwork.py:70-75: the network predicts bone-relative coordinates; assemble xyz by forward kinematics
-        pl->add([=](const Ext& e, cudaStream_t s) {
-            if (e.out2) H3D_CUDA(cudaMemcpyAsync(e.out2, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
-            return launch_bone_rel_trafo_inv(can, e.out, B, s);
-        });
+        pl->flops += chain_flops;
+        st.kind = KIND_TC; st.flops = chain_flops;
     } else {
         pl->add([=](const Ext& e, cudaStream_t s) {
-            H3D_CUDA(cudaMemcpyAsync(e.out, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
-            if (e.out2) H3D_CUDA(cudaMemcpyAsync(e.out2, can, (size_t)B * 63 * 4, cudaMemcpyDeviceToDevice, s));
-            return H3D_OK;
+            const int rc2 = tail(e, s);
+            return rc2 || !proposed ? rc2 : launch_rotate_canonical(can, uxyz, e.hand_side, B, e.out3, e.out, s);
         });
     }
     if (drop) {   // after the join: every dropout layer of this forward has read the draw
@@ -1457,25 +1431,22 @@ int h3d_track_step_slots(h3d_ctx* ctx, const float* image, const float* hand_sid
     DeviceGuard guard_(ctx);                              \
     cudaStream_t s = (cudaStream_t)stream;
 
-struct h3d_packed_conv { PackedW pw; int k = 0, Cin = 0, Cout = 0, precision = 0; };
+struct h3d_packed_conv { PackedW pw; int k = 0, Cin = 0, Cout = 0; };
 
 int h3d_conv2d_f32(h3d_ctx* ctx, const float* x, const float* w_hwio, const float* bias, float* y, int B, int H, int W, int Cin,
                    int Cout, int ksize, int stride, int leaky, void* stream) {
     H3D_OP_PROLOGUE(ctx);
-    DirectConvArgs a;
-    a.x = x; a.Cin_total = Cin; a.cin_off = 0; a.w = w_hwio; a.bias = bias; a.y = y; a.Cout_total = Cout; a.cout_off = 0;
-    a.ys = Split(); a.Cs_total = 0; a.cs_off = 0; a.half = Half16::BF16;
-    a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.k = ksize; a.stride = stride; a.leaky = leaky;
-    a.err_flag = ctx->err_flag;
     // lets tiny layers take the split-K path exactly as the lifting stage does
     const bool tiny = (int64_t)B * ceil_div(H, stride) * ceil_div(W, stride) <= 64 * 295;
+    char* scratch = nullptr;
     if (tiny) {
-        char* scratch = nullptr;
         int rc0 = op_scratch(ctx, kConvSplitKScratchFloats * 4, &scratch);
         if (rc0) return rc0;
-        a.splitk_scratch = (float*)scratch; a.splitk_scratch_floats = kConvSplitKScratchFloats;
     }
-    return launch_conv_direct(a, s);
+    const LayerSpec l{nullptr, ksize, stride, Cin, Cout, leaky};
+    return launch_conv_direct(direct_args(l, w_hwio, bias, Half16::BF16, B, H, W, x, Cin, 0, y, Cout, 0, Split(), 0, 0, (float*)scratch,
+                                          tiny ? kConvSplitKScratchFloats : 0, ctx->err_flag),
+                              s);
 }
 
 int h3d_pack_conv_weights(h3d_ctx* ctx, const float* host_w_hwio, const float* host_bias, int ksize, int Cin, int Cout, int precision,
@@ -1485,7 +1456,7 @@ int h3d_pack_conv_weights(h3d_ctx* ctx, const float* host_w_hwio, const float* h
     H3D_REQUIRE(ksize == 1 || ksize == 3 || ksize == 5 || ksize == 7, "h3d_pack_conv_weights: ksize must be 1, 3, 5 or 7");
     DeviceGuard guard(ctx);
     auto* h = new h3d_packed_conv();
-    h->k = ksize; h->Cin = Cin; h->Cout = Cout; h->precision = precision;
+    h->k = ksize; h->Cin = Cin; h->Cout = Cout;
     int rc = pack_conv_weights(host_w_hwio, host_bias, ksize, Cin, Cout, (int)align_up(Cin, 64), (int)align_up(Cout, 64), {}, half_of(precision),
                                passes_of(precision), &h->pw);
     if (rc) { free_packed(h->pw); delete h; return rc; }
@@ -1502,54 +1473,50 @@ int h3d_free_packed_conv(h3d_ctx* ctx, h3d_packed_conv* packed) {
     return H3D_OK;
 }
 
-// Body shared by h3d_conv2d_tc_packed and h3d_conv2d_tc_dev.  Operand planes are carved from the context's operator scratch:
-// [x hi | x lo / l8 h8 | y hi | y lo / l8 h8 | wbytes for the caller's weight planes]; pack(wbase, &pw) provides the packed weights
-// (enqueueing their packing when they live in the scratch) before x is split and the convolution runs.
-extern "C++" {   // a template inside the C ABI block
-template <class PackFn>
-static int conv_tc_run(h3d_ctx* ctx, const float* x, float* y, int B, int H, int W, int Cin, int Cout, int ksize, int stride, int leaky,
-                       int precision, int Cin_pad, int Cout_pad, int64_t wbytes, PackFn pack, cudaStream_t s) {
+// Operand planes of h3d_conv2d_tc_packed / _dev in the context's operator scratch: [x hi | x lo / l8 h8 | y hi | y lo / l8 h8 | wbytes],
+// the last part (*w) for the weight planes h3d_conv2d_tc_dev packs on the device
+static int tc_op_planes(h3d_ctx* ctx, int B, int H, int W, int ksize, int stride, int Cin_pad, int Cout_pad, int passes, int64_t wbytes,
+                        Split* xs, Split* ys, char** w) {
     H3D_REQUIRE(stride == 1 || (stride == 2 && H % 2 == 0 && W % 2 == 0 && ksize >= 3),
                 "h3d_conv2d_tc: stride must be 1, or 2 with even H and W and ksize >= 3 (for ksize 1 TF's 'SAME' samples the even pixels)");
-    const Half16 half = half_of(precision);
-    const int passes = passes_of(precision);
     const int64_t rows = (int64_t)B * H * W, rows_out = rows / (stride * stride);
     const int64_t xb = align_up(rows * Cin_pad * 2, 1024), yb = align_up(rows_out * Cout_pad * 2, 1024);
     char* base = nullptr;
     int rc = op_scratch(ctx, 2 * xb + 2 * yb + wbytes, &base);
     if (rc) return rc;
-    PackedW pw;
-    if ((rc = pack(base + 2 * xb + 2 * yb, &pw))) return rc;
-    Split xs, ys;
-    xs.hi = (uint16_t*)base; ys.hi = (uint16_t*)(base + 2 * xb);
-    if (passes == 3) { xs.lo = (uint16_t*)(base + xb); ys.lo = (uint16_t*)(base + 2 * xb + yb); }
+    xs->hi = (uint16_t*)base; ys->hi = (uint16_t*)(base + 2 * xb);
+    if (passes == 3) { xs->lo = (uint16_t*)(base + xb); ys->lo = (uint16_t*)(base + 2 * xb + yb); }
     if (passes == 4) {
-        xs.l8 = (uint8_t*)(base + xb); xs.h8 = xs.l8 + align_up(rows * Cin_pad, 1024);
-        ys.l8 = (uint8_t*)(base + 2 * xb + yb); ys.h8 = ys.l8 + align_up(rows_out * Cout_pad, 1024);
+        xs->l8 = (uint8_t*)(base + xb); xs->h8 = xs->l8 + align_up(rows * Cin_pad, 1024);
+        ys->l8 = (uint8_t*)(base + 2 * xb + yb); ys->h8 = ys->l8 + align_up(rows_out * Cout_pad, 1024);
     }
-    if ((rc = launch_f32_to_split(x, xs, rows, Cin, Cin_pad, half, s))) return rc;
-    TcConvDesc d;
-    d.x = xs; d.Cin_total = Cin_pad; d.Cin_pad = Cin_pad; d.w = pw.w; d.bias = pw.bias; d.w_scale = pw.w_scale; d.Cout = Cout;
-    d.Cout_pad = Cout_pad;
-    d.y = ys; d.Cy_total = Cout_pad; d.cy_off = 0; d.yf = nullptr; d.Cyf_total = 0; d.cyf_off = 0;
-    d.B = B; d.H = H; d.W = W; d.k = ksize; d.leaky = leaky; d.passes = passes; d.half = half; d.corr_scale = pw.corr_scale;
-    d.pool = stride == 2 ? 2 : 0;
-    d.err_flag = ctx->err_flag;
-    TcConvPlan* tp = tc_conv_plan_create(d, &rc);     // host-side only: tensor maps + launch geometry (passed to the kernel by value)
-    if (!tp) return rc;
-    rc = tc_conv_launch(tp, s);
-    tc_conv_plan_destroy(tp);
-    if (rc) return rc;
-    return launch_split_to_f32(ys, y, rows_out, Cout, Cout_pad, half, s);
+    if (w) *w = base + 2 * xb + 2 * yb;
+    return H3D_OK;
 }
-}  // extern "C++"
+
+// Body shared by h3d_conv2d_tc_packed and h3d_conv2d_tc_dev: x split into the planes xs, the layer with the weights pw into ys, ys
+// converted to fp32 y
+static int conv_tc_run(h3d_ctx* ctx, const float* x, float* y, int B, int H, int W, int Cin, int Cout, int ksize, int stride, int leaky,
+                       const PackedW& pw, Split xs, Split ys, cudaStream_t s) {
+    const int64_t rows = (int64_t)B * H * W;
+    int rc;
+    if ((rc = launch_f32_to_split(x, xs, rows, Cin, pw.Cin_pad, pw.half, s))) return rc;
+    StagePlan pl;
+    const LayerSpec l{nullptr, ksize, stride, Cin, Cout, leaky};
+    if ((rc = add_tc(ctx, &pl, l, pw, B, H, W, xs, pw.Cin_pad, ys, pw.Cout_pad, 0, nullptr, 0, 0, stride == 2 ? 2 : 0))) return rc;
+    if ((rc = run_step(pl, s))) return rc;
+    return launch_split_to_f32(ys, y, rows / (stride * stride), Cout, pw.Cout_pad, pw.half, s);
+}
 
 int h3d_conv2d_tc_packed(h3d_ctx* ctx, const float* x, const h3d_packed_conv* packed, float* y, int B, int H, int W, int stride,
                          int leaky, void* stream) {
     H3D_OP_PROLOGUE(ctx);
     H3D_REQUIRE(x && packed && y && B > 0, "h3d_conv2d_tc_packed: bad argument");
-    return conv_tc_run(ctx, x, y, B, H, W, packed->Cin, packed->Cout, packed->k, stride, leaky, packed->precision, packed->pw.Cin_pad,
-                       packed->pw.Cout_pad, 0, [&](char*, PackedW* pw) { *pw = packed->pw; return (int)H3D_OK; }, s);
+    const PackedW& pw = packed->pw;
+    Split xs, ys;
+    int rc = tc_op_planes(ctx, B, H, W, packed->k, stride, pw.Cin_pad, pw.Cout_pad, pw.passes, 0, &xs, &ys, nullptr);
+    if (rc) return rc;
+    return conv_tc_run(ctx, x, y, B, H, W, packed->Cin, packed->Cout, packed->k, stride, leaky, pw, xs, ys, s);
 }
 
 // Weight planes of a device-weight convolution in the operator scratch: [hi | lo | bias padded to Cout_pad | fp16: w_scale [Cout_pad]]
@@ -1564,16 +1531,19 @@ int h3d_conv2d_tc_dev(h3d_ctx* ctx, const float* x, const float* w_hwio, const f
     H3D_REQUIRE(ksize == 1 || ksize == 3 || ksize == 5 || ksize == 7, "h3d_conv2d_tc_dev: ksize must be 1, 3, 5 or 7");
     const int Cin_pad = (int)align_up(Cin, 64), Cout_pad = (int)align_up(Cout, 64);
     const int64_t pb = dev_plane_bytes(ksize, Cin_pad, Cout_pad);
-    auto pack = [&](char* wbase, PackedW* pw) {
-        pw->w.hi = (uint16_t*)wbase;
-        if (passes_of(precision) == 3) pw->w.lo = (uint16_t*)(wbase + pb);
-        pw->bias = (float*)(wbase + 2 * pb);
-        if (half_of(precision) == Half16::FP16) pw->w_scale = pw->bias + Cout_pad;
-        pw->Cin_pad = Cin_pad; pw->Cout_pad = Cout_pad;
-        return launch_pack_conv_w(w_hwio, bias, pw->w, pw->bias, pw->w_scale, ksize, Cin, Cout, Cin_pad, Cout_pad, false, half_of(precision), s);
-    };
-    return conv_tc_run(ctx, x, y, B, H, W, Cin, Cout, ksize, stride, leaky, precision, Cin_pad, Cout_pad, 2 * pb + align_up(Cout_pad * 8, 1024),
-                       pack, s);
+    PackedW pw;
+    pw.passes = passes_of(precision); pw.half = half_of(precision);
+    Split xs, ys;
+    char* wbase = nullptr;
+    int rc = tc_op_planes(ctx, B, H, W, ksize, stride, Cin_pad, Cout_pad, pw.passes, 2 * pb + align_up(Cout_pad * 8, 1024), &xs, &ys, &wbase);
+    if (rc) return rc;
+    pw.w.hi = (uint16_t*)wbase;
+    if (pw.passes == 3) pw.w.lo = (uint16_t*)(wbase + pb);
+    pw.bias = (float*)(wbase + 2 * pb);
+    if (pw.half == Half16::FP16) pw.w_scale = pw.bias + Cout_pad;
+    pw.Cin_pad = Cin_pad; pw.Cout_pad = Cout_pad;
+    if ((rc = launch_pack_conv_w(w_hwio, bias, pw.w, pw.bias, pw.w_scale, ksize, Cin, Cout, Cin_pad, Cout_pad, false, pw.half, s))) return rc;
+    return conv_tc_run(ctx, x, y, B, H, W, Cin, Cout, ksize, stride, leaky, pw, xs, ys, s);
 }
 
 int h3d_conv2d_tc_backward(h3d_ctx* ctx, const float* x, const float* y, const float* dy, const float* w_hwio, float* dx, float* dw_hwio,
@@ -1615,20 +1585,15 @@ int h3d_conv2d_tc_backward(h3d_ctx* ctx, const float* x, const float* y, const f
     if ((rc = launch_conv_grad_prep(dy, leaky ? y : nullptr, gs, db ? db_part : nullptr, B, H, W, Cout, Cout_pad, stride, leaky, s))) return rc;
     if (db && (rc = launch_bias_grad_reduce(db_part, nblk, Cout, Cout_pad, db, s))) return rc;
     if (dx) {   // the stride-1 'SAME' convolution of dy' with the flipped, transposed kernel, on the forward kernel
-        Split wd;
-        wd.hi = (uint16_t*)wbase;
-        if (passes == 3) wd.lo = (uint16_t*)(wbase + wb);
-        if ((rc = launch_pack_conv_w(w_hwio, nullptr, wd, zbias, nullptr, ksize, Cin, Cout, Cin_pad, Cout_pad, true, Half16::BF16, s))) return rc;
-        TcConvDesc d;
-        d.x = gs; d.Cin_total = Cout_pad; d.Cin_pad = Cout_pad; d.w = wd; d.bias = zbias; d.Cout = Cin; d.Cout_pad = Cin_pad;
-        d.y = Split(); d.Cy_total = 0; d.cy_off = 0; d.yf = dx; d.Cyf_total = Cin; d.cyf_off = 0;
-        d.B = B; d.H = H; d.W = W; d.k = ksize; d.leaky = 0; d.passes = passes; d.half = Half16::BF16; d.pool = 0;
-        d.err_flag = ctx->err_flag;
-        TcConvPlan* tp = tc_conv_plan_create(d, &rc);
-        if (!tp) return rc;
-        rc = tc_conv_launch(tp, s);
-        tc_conv_plan_destroy(tp);
-        if (rc) return rc;
+        PackedW wd;   // [Cin_pad][k][k][Cout_pad] planes, zero bias
+        wd.w.hi = (uint16_t*)wbase;
+        if (passes == 3) wd.w.lo = (uint16_t*)(wbase + wb);
+        wd.bias = zbias; wd.Cin_pad = Cout_pad; wd.Cout_pad = Cin_pad; wd.passes = passes; wd.half = Half16::BF16;
+        if ((rc = launch_pack_conv_w(w_hwio, nullptr, wd.w, zbias, nullptr, ksize, Cin, Cout, Cin_pad, Cout_pad, true, wd.half, s))) return rc;
+        StagePlan pl;
+        const LayerSpec l{nullptr, ksize, 1, Cout, Cin, 0};
+        if ((rc = add_tc(ctx, &pl, l, wd, B, H, W, gs, Cout_pad, Split(), 0, 0, dx, Cin, 0))) return rc;
+        if ((rc = run_step(pl, s))) return rc;
     }
     if (dw_hwio) {
         Split xs;
@@ -1673,19 +1638,17 @@ int h3d_conv2d_f32_geometry(int B, int H, int W, int Cin, int Cin_total, int cin
     // the choosers test these pointers for NULL (and x for its alignment) and never dereference them
     alignas(16) static float probe[4];
     const int passes = planes == H3D_PREC_FP32_FFMA ? 0 : passes_of(planes);
-    DirectConvArgs a;
-    a.x = x_aligned ? probe : probe + 1; a.Cin_total = Cin_total; a.cin_off = cin_off; a.w = probe; a.bias = probe;
-    a.y = yf ? probe : nullptr; a.Cout_total = Cout_total; a.cout_off = cout_off;
-    a.ys = Split();
+    Split ys;
     if (passes) {
-        a.ys.hi = (uint16_t*)probe;
-        if (passes == 3) a.ys.lo = (uint16_t*)probe;
-        if (passes == 4) { a.ys.l8 = (uint8_t*)probe; a.ys.h8 = (uint8_t*)probe; }
+        ys.hi = (uint16_t*)probe;
+        if (passes == 3) ys.lo = (uint16_t*)probe;
+        if (passes == 4) { ys.l8 = (uint8_t*)probe; ys.h8 = (uint8_t*)probe; }
     }
-    a.Cs_total = Cs_total; a.cs_off = cs_off; a.half = passes ? half_of(planes) : Half16::BF16;
-    a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.k = ksize; a.stride = stride; a.leaky = 0;
-    a.splitk_scratch = splitk_scratch_floats ? probe : nullptr; a.splitk_scratch_floats = splitk_scratch_floats;
-    conv_direct_geometry(a, out);
+    const LayerSpec l{nullptr, ksize, stride, Cin, Cout, 0};
+    conv_direct_geometry(direct_args(l, probe, probe, passes ? half_of(planes) : Half16::BF16, B, H, W, x_aligned ? probe : probe + 1,
+                                     Cin_total, cin_off, yf ? probe : nullptr, Cout_total, cout_off, ys, Cs_total, cs_off,
+                                     splitk_scratch_floats ? probe : nullptr, splitk_scratch_floats, nullptr),
+                         out);
     return H3D_OK;
 }
 
@@ -1711,8 +1674,9 @@ int h3d_conv2d_tc_strided(h3d_ctx* ctx, const float* x, const float* host_w_hwio
     return rc;
 }
 
-// One network layer as build_trunk / build_handsegnet / build_posenet issue it through add_tc (route 0) or add_direct (route 1), with
-// the layer's planes, channel offsets, fused pool and input permutation given explicitly instead of taken from a stage plan.
+// One network layer issued by add_tc (route 0) or add_direct (route 1), the step builders of build_trunk / build_handsegnet /
+// build_posenet, from the host weights given; the layer's planes, channel offsets, fused pool and input permutation are given
+// explicitly instead of taken from a stage plan.
 int h3d_conv2d_layer_planes(h3d_ctx* ctx, const float* x, int B, int H, int W, int Cx, const float* host_w_hwio, const float* host_bias,
                             int ksize, int Cin, int Cout, const int32_t* host_perm, int pool, int leaky, int precision, int route,
                             void* y_hi, void* y_lo, void* y_l8, void* y_h8, int Cy_total, int cy_off, float* yf, int Cyf_total,
@@ -1736,6 +1700,8 @@ int h3d_conv2d_layer_planes(h3d_ctx* ctx, const float* x, int B, int H, int W, i
         if (passes == 4) { ys.l8 = (uint8_t*)y_l8; ys.h8 = (uint8_t*)y_h8; }
     }
     const int64_t rows = (int64_t)B * H * W;
+    const LayerSpec l{nullptr, ksize, 1, Cin, Cout, leaky};
+    StagePlan pl;
     char* base = nullptr;
     int rc;
     if (route == 1) {
@@ -1745,12 +1711,8 @@ int h3d_conv2d_layer_planes(h3d_ctx* ctx, const float* x, int B, int H, int W, i
         float* w = (float*)base; float* b = (float*)(base + wb);
         H3D_CUDA(cudaMemcpyAsync(w, host_w_hwio, wn * 4, cudaMemcpyHostToDevice, s));   // pageable: returns once the source is staged
         H3D_CUDA(cudaMemcpyAsync(b, host_bias, Cout * 4, cudaMemcpyHostToDevice, s));
-        DirectConvArgs a;
-        a.x = x; a.Cin_total = Cx; a.cin_off = 0; a.w = w; a.bias = b; a.y = yf; a.Cout_total = Cyf_total; a.cout_off = cyf_off;
-        a.ys = ys; a.Cs_total = Cy_total; a.cs_off = cy_off; a.half = half;
-        a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.k = ksize; a.stride = 1; a.leaky = leaky;
-        a.err_flag = ctx->err_flag;
-        return launch_conv_direct(a, s);
+        if ((rc = add_direct(ctx, &pl, l, w, b, half, B, H, W, x, Cx, 0, yf, Cyf_total, cyf_off, ys, Cy_total, cy_off))) return rc;
+        return run_step(pl, s);
     }
     const int Cin_pad = (int)align_up(Cin, 64), Cout_pad = (int)align_up(Cout, 64);
     H3D_REQUIRE(Cin_pad <= Cx && Cx % 16 == 0, "h3d_conv2d_layer_planes: x needs Cx >= align_up(Cin, 64) channels, Cx a multiple of 16");
@@ -1772,16 +1734,7 @@ int h3d_conv2d_layer_planes(h3d_ctx* ctx, const float* x, int B, int H, int W, i
         free_packed(pw);
         return rc;
     }
-    TcConvDesc d;
-    d.x = xs; d.Cin_total = Cx; d.Cin_pad = Cin_pad; d.w = pw.w; d.bias = pw.bias; d.w_scale = pw.w_scale; d.Cout = Cout; d.Cout_pad = Cout_pad;
-    d.y = ys; d.Cy_total = Cy_total; d.cy_off = cy_off; d.yf = yf; d.Cyf_total = Cyf_total; d.cyf_off = cyf_off;
-    d.B = B; d.H = H; d.W = W; d.k = ksize; d.leaky = leaky; d.passes = passes; d.half = half; d.corr_scale = pw.corr_scale; d.pool = pool;
-    d.err_flag = ctx->err_flag;
-    TcConvPlan* tp = tc_conv_plan_create(d, &rc);
-    if (tp) {
-        rc = tc_conv_launch(tp, s);
-        tc_conv_plan_destroy(tp);
-    }
+    if (!(rc = add_tc(ctx, &pl, l, pw, B, H, W, xs, Cx, ys, Cy_total, cy_off, yf, Cyf_total, cyf_off, pool))) rc = run_step(pl, s);
     free_packed(pw);   // host weights: the free waits for the kernel, as in h3d_conv2d_tc
     return rc;
 }
