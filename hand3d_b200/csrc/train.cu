@@ -124,11 +124,12 @@ __global__ void resize_grad_rows_kernel(const float* __restrict__ t, float* __re
 // =============================================================================================
 constexpr int kSmK = 21, kSmGroups = 12, kSmThreads = kSmK * kSmGroups;   // 252 threads: thread t = (pixel group t / 21, channel t % 21)
 
-// partial[b][chunk][k] = sum over the chunk's pixels (group-strided, then the 12 groups in order) of (P - T)^2
+// partial[b][chunk][k] = sum over the chunk's pixels (group-strided, then the 12 groups in order) of (P - T)^2.  One block per
+// (image, chunk), blockIdx.x = b nchunk + chunk: x takes any batch, where a grid row per image would stop at 65 535 images.
 __global__ void __launch_bounds__(kSmThreads) scoremap_sq_partial_kernel(const float* __restrict__ P, const float* __restrict__ T,
                                                                           float* __restrict__ partial, int HW, int ppc, int nchunk) {
     __shared__ float red[kSmGroups][kSmK];
-    const int b = blockIdx.y, chunk = blockIdx.x, t = threadIdx.x, k = t % kSmK, j = t / kSmK;
+    const int b = blockIdx.x / nchunk, chunk = blockIdx.x - b * nchunk, t = threadIdx.x, k = t % kSmK, j = t / kSmK;
     const int p0 = chunk * ppc, p1 = min(HW, p0 + ppc);
     const int64_t base = (int64_t)b * HW * kSmK;
     float s = 0.f;
@@ -366,7 +367,7 @@ int64_t scoremap_loss_scratch_floats(int B, int H, int W) { return (int64_t)B * 
 int launch_scoremap_loss(const float* P, const float* T, const float* vis, float* scratch, int B, int H, int W, float* loss, float* rms,
                          cudaStream_t s) {
     const int HW = H * W, nchunk = scoremap_chunks(B, HW), ppc = ceil_div(HW, nchunk);
-    scoremap_sq_partial_kernel<<<dim3(nchunk, B), kSmThreads, 0, s>>>(P, T, scratch, HW, ppc, nchunk);
+    scoremap_sq_partial_kernel<<<B * nchunk, kSmThreads, 0, s>>>(P, T, scratch, HW, ppc, nchunk);
     H3D_CHECK_LAUNCH();
     scoremap_loss_finalize_kernel<<<1, kRedThreads, 0, s>>>(scratch, vis, rms, loss, B * kSmK, HW, nchunk);
     H3D_CHECK_LAUNCH();

@@ -576,7 +576,8 @@ H3D_API int h3d_resize_bilinear_tf1_backward(h3d_ctx* ctx, const float* dy, floa
 /* PoseNet score-map loss for one predicted map (training_posenet.py:58-61):
  *   loss = sum_{b,k} vis[b,k] sqrt(mean_{h,w} (pred - target)^2) / (sum_{b,k} vis + 0.001)
  * pred, target [B,H,W,21], vis [B,21] fp32 (0 / 1, any value is accepted) -> loss (device scalar) and rms [B,21] =
- * sqrt(mean (pred - target)^2), which the backward reuses.  fp32 with separate multiply and add. */
+ * sqrt(mean (pred - target)^2), which the backward reuses.  fp32 with separate multiply and add.  Any B >= 1 is accepted (no
+ * per-image grid limit). */
 H3D_API int h3d_scoremap_loss_forward(h3d_ctx* ctx, const float* pred, const float* target, const float* vis, int B, int H, int W,
                                       float* loss, float* rms, void* stream);
 /* Its gradient: dpred [B,H,W,21] = grad_loss vis[b,k] / S (pred - target) / (H W rms[b,k]), S = sum vis + 0.001; 0 where
